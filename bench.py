@@ -1,12 +1,12 @@
 #!/usr/bin/env python
-"""bench.py - IQ Msamp/s through xcorr_pss (BASELINE.json metric) on N B200s of one node.
+"""bench.py - IQ Msamp/s through xcorr_pss (BASELINE.json metric) on N H100s of one node.
 
 A "step" is one pass of the hot path (xcorr_pss: correlate 3 PSS roots x n_f frequency
 hypotheses, fold, delay-spread, argmax, signal power) over one batch of synthetic capture
 buffers.  Workload = BASELINE.json configs[1]: 153600-sample capture buffers, +-100 ppm grid at
 739 MHz (n_f = 31), ds_comb_arm 2, synthetic rtl-sdr-like 8-bit IQ (SURVEY.md 8d).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--batch B] [--impl b200|reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--batch B] [--impl b200|reference] [--dump-outputs DIR]
 
 Launch for N>1:  python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N
 Capture buffers shard across ranks with no data-path collective (weak scaling: B buffers per
@@ -14,11 +14,15 @@ rank per step); the only collective is the max-over-ranks of the device time.
 
 Prints ONE JSON line (rank 0).  `value` = whole-job Msamp/s with inputs resident in HBM;
 `e2e` = same metric through the host-buffer C-ABI call (pinned host cu8 in, results out, copies
-inside the timed region); `roofline` = the dominant kernel against the measured peaks;
+inside the timed region); `roofline` = the dominant kernel against the H100 SXM data-sheet peaks;
 `cpu_baseline` = the CPU oracle (port of the reference loop nest, OpenMP) on a bounded sample;
 `parity_spot` = one buffer of the last timed step against the oracle; `sweep` / `tracker` = BASELINE
 configs 4 and 5 (512-channel frequency sweep with an NCCL gather of the cells; 64-channel streaming
 searcher) measured in the same run on the same ranks.
+
+--dump-outputs DIR writes what the timed path returned in its last timed step (a fixed, seeded sample of the batch's
+capture buffers: xc_incoherent_single, pow, frq, sp_incoherent) as DIR/<name>.npy, so that two builds can be compared
+output for output; the inputs depend only on the arguments.
 """
 import argparse
 import json
@@ -61,27 +65,14 @@ def f_alg(n_f, n_comb=15):
     return 8.0 * 137 * 3 * n_f * n_comb * 9600
 
 
-def ncu_traffic(kernel, capbufs):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of the dominant kernel from the committed `ncu --set full`
-    capture (profiles/traffic.json, bytes per capture buffer of the bench workload), scaled to this launch; None if absent."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "traffic.json")) as f:
-            return float(json.load(f)[kernel]["dram_bytes_per_capbuf"]) * capbufs
-    except Exception:  # noqa
-        return None
-
-
 def load_peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        d = json.load(open(p))
-        return dict(hbm_gbs=float(d["hbm_gbs"]), bf16_tflops=float(d["bf16_tflops"]),
-                    bf16_tflops_sustained=float(d.get("bf16_tflops_sustained", d["bf16_tflops"])), source="measured")
-    return dict(hbm_gbs=6650.0, bf16_tflops=1590.0, bf16_tflops_sustained=1400.0, source="fallback")
+    """NVIDIA's data-sheet figures for the H100 SXM (700 W board power): dense tensor rates and HBM3 bandwidth.  A card
+    run at a lower power limit reaches less; `clocks` in the result line shows the SM clock of the run."""
+    return dict(hbm_gbs=3350.0, bf16_tflops=989.0, int8_tops=1979.0, source="H100 SXM data sheet (700 W)")
 
 
 class ClockSampler:
-    """SM clock / throttle reasons sampled DURING the timed region (B200_PROFILING.md).  A thread polls NVML every 5 ms
+    """SM clock / throttle reasons sampled DURING the timed region.  A thread polls NVML every 5 ms
     (pynvml; the GIL is released while the main thread waits on CUDA); if NVML is unavailable one `nvidia-smi -lms 20`
     process runs across the region instead.  Only samples stamped inside the region are kept."""
     Q = ("timestamp,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
@@ -408,6 +399,19 @@ def tracker_leg(L, torch, dist, ctx, rank, world, dev, barrier, cycles=8, reps=3
             "new_cells_steady_state": n_new, "api": "lcs_sweep_track_cu8", "h2d_bytes_per_cycle": n_ch * N_CAP * 2}
 
 
+def dump_outputs(out_dir, r_last, d_single, d_pow, d_frq, d_spi, n_sample=8, seed=20240601):
+    """The outputs of the last timed step for a fixed, seeded sample of its capture buffers (about 33 MB at n_f = 31)."""
+    B = d_single[r_last].shape[0]
+    idx = np.sort(np.random.default_rng(seed).choice(B, size=min(B, n_sample), replace=False))
+    sel = lambda t: t[r_last][idx].cpu().numpy()
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"buffer_index": idx.astype(np.float64), "single": sel(d_single).astype(np.float32),
+              "pow": sel(d_pow).astype(np.float64), "frq": sel(d_frq).astype(np.float64), "sp_incoherent": sel(d_spi).astype(np.float64)}
+    assert sum(a.nbytes for a in arrays.values()) <= 64 << 20
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -417,12 +421,16 @@ def main():
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--kernel", default="auto", choices=["auto", "fp32", "tc"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
-    ap.add_argument("--no-extra-legs", action="store_true", help="skip the sweep / tracker / search legs (ncu captures)")
+    ap.add_argument("--no-extra-legs", action="store_true", help="skip the sweep / tracker / search legs (shorter runs)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write a fixed, seeded sample of the last timed step's outputs as DIR/<name>.npy")
     ap.add_argument("--workload", default="search", choices=["search", "tracker"],
                     help="search: BASELINE configs[1] (n_f=31); tracker: SURVEY 8d config 5 shape (n_f=1 at the tracked offset)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "b200" else args.warmup
     if args.impl == "reference":
+        if args.dump_outputs:
+            ap.error("--dump-outputs writes the GPU path's outputs; it cannot be combined with --impl reference")
         return run_reference(args)
 
     import torch
@@ -459,9 +467,9 @@ def main():
     plan = ctx.plan(N_CAP, f, ARM, FC, FC, FS, max_batch=B, kernel=kern)
     kernel_used = {L.KERNEL_FP32: "xcorr_fold_fp32", L.KERNEL_TC: "xcorr_fold_tc"}[plan.kernel_for(L.IQ_CU8)]
 
-    # ---- synthetic inputs: a ring of distinct batches whose inputs+outputs exceed L2 (126 MB) ----
+    # ---- synthetic inputs: a ring of distinct batches whose inputs+outputs exceed L2 (50 MB) ----
     out_bytes_per_cap = 3 * n_f * 9600 * 4 + 3 * 9600 * 12 + 9600 * 8
-    ring = max(2, int(np.ceil(300e6 / (B * (out_bytes_per_cap + N_CAP * 2)))))      # inputs+outputs in flight > L2 (126 MB)
+    ring = max(2, int(np.ceil(300e6 / (B * (out_bytes_per_cap + N_CAP * 2)))))      # inputs+outputs in flight > L2 (50 MB)
     base = np.stack([synth_cu8(SEED0 + rank * 100003 + i) for i in range(B)])      # [B][n_cap][2] u8
     h_iq = torch.from_numpy(base).pin_memory()
     d_iq, d_single, d_pow, d_frq, d_spi = [], [], [], [], []
@@ -511,6 +519,8 @@ def main():
     launches = ctx.launches - launches0
     clocks = sampler.summary() if rank == 0 else None
     ms_max = all_max(torch, dist, world, dev, ms)
+    if rank == 0 and args.dump_outputs:
+        dump_outputs(args.dump_outputs, (args.warmup + args.steps - 1) % ring, d_single, d_pow, d_frq, d_spi)
     capbufs_per_s = world * B * args.steps / (ms_max / 1e3)
     value = capbufs_per_s * N_CAP / 1e6
 
@@ -604,33 +614,21 @@ def main():
         in_bps = 2                                   # cu8 staged format
         alg_bytes = B * b_alg(n_f, in_bps)
         alg_flops = B * f_alg(n_f)
-        timed_s = ms / 1e3
         if kernel_used == "xcorr_fold_tc":
-            # burst cuBLAS figure unless the kernel ran inside a seconds-long power-capped sequence (B200_PROFILING.md)
-            long_run = timed_s > 2.0
-            pk = peaks["bf16_tflops_sustained"] if long_run else peaks["bf16_tflops"]
-            roof = {"bound": "tensor", "achieved": alg_flops / k_avg_s / 1e12, "peak": pk, "unit": "TFLOP/s",
-                    "peak_kind": ("sustained bf16 (timed region %.2f s > 2 s)" if long_run else "burst bf16 (timed region %.2f s)") % timed_s,
-                    "frac_of_burst": alg_flops / k_avg_s / 1e12 / peaks["bf16_tflops"],
-                    "frac_of_sustained": alg_flops / k_avg_s / 1e12 / peaks["bf16_tflops_sustained"],
-                    "tensor_mode": "tcgen05 kind::i8 (s8 x s8 -> s32, exact); the driver measures only a bf16 peak, int8 runs at 2x "
-                                   "that rate; achieved counts F_alg only - the kernel executes 3 int8 digit planes x 96/93 column padding "
-                                   "x 288/274 K padding x 9728/9600 tile rounding = 3.3x more MACs than F_alg"}
+            roof = {"bound": "tensor", "achieved": alg_flops / k_avg_s / 1e12, "peak": peaks["bf16_tflops"], "unit": "TFLOP/s",
+                    "peak_kind": "dense bf16, data sheet",
+                    "tensor_mode": "wgmma s8 x s8 -> s32 (exact); achieved counts F_alg only - the kernel executes 3 int8 digit "
+                                   "planes x 96/93 column padding x 288/274 K padding x 9728/9600 tile rounding = 3.3x more MACs than F_alg"}
         else:
             roof = {"bound": "hbm", "achieved": alg_bytes / k_avg_s / 1e9, "peak": peaks["hbm_gbs"], "unit": "GB/s"}
         roof["frac"] = roof["achieved"] / roof["peak"]
         if kernel_used == "xcorr_fold_tc" and args.workload == "search":
-            # executed int8 operations: 38 tiles x 15 half frames x 2 sub-tiles x 2 parts x 2 jobs per buffer, 9 UTCIMMA of
-            # M=128, N=144, K=32 B per job; against the rate a loop of nothing but these instructions sustains on all SMs
-            # (tools/microbench/umma_sustained.cu, profiles/r02_umma_sustained_microbench.txt)
-            ops = B * 38 * 15 * 2 * 2 * 2 * 9 * (2.0 * 128 * 144 * 32)
-            pops = ops / k_avg_s / 1e15
-            ceil_pops = 3.65 if (clocks and clocks.get("sm_mhz") and clocks["sm_mhz"] < 1750) else 4.1
-            roof.update({"executed_int8_pops": pops, "pure_mma_ceiling_int8_pops": ceil_pops,
-                         "pure_mma_ceiling_note": "4.1 POP/s for a burst at ~1.83 GHz, 3.65 POP/s power-capped at ~1.63 GHz (measured, profiles/r02_umma_sustained_microbench.txt); chosen by the SM clock sampled during this run",
-                         "frac_of_pure_mma_ceiling": pops / ceil_pops})
-        roof.update({"traffic": ncu_traffic(kernel_used, B), "traffic_source": "profiles/traffic.json (ncu --set full capture of this kernel, scaled to this batch)",
-                     "kernel": kernel_used, "kernel_avg_ms": k_avg_s * 1e3, "kernel_launches": kernel_n,
+            # executed int8 operations: 38 tiles x 15 half frames x 4 sub-tiles x 2 parts x 2 jobs per buffer, 9 wgmma of
+            # M=64, N=144, K=32 B per job, against the data-sheet dense int8 rate
+            ops = B * 38 * 15 * 4 * 2 * 2 * 9 * (2.0 * 64 * 144 * 32)
+            tops = ops / k_avg_s / 1e12
+            roof.update({"executed_int8_tops": tops, "int8_tops_peak": peaks["int8_tops"], "frac_of_int8_peak": tops / peaks["int8_tops"]})
+        roof.update({"kernel": kernel_used, "kernel_avg_ms": k_avg_s * 1e3, "kernel_launches": kernel_n,
                      "kernel_share_of_step": kernel_ms / ms, "alg_bytes_per_launch": alg_bytes,
                      "alg_flops_per_launch": alg_flops, "alg_tflops": alg_flops / k_avg_s / 1e12,
                      "hbm_frac": alg_bytes / k_avg_s / 1e9 / peaks["hbm_gbs"],

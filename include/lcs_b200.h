@@ -1,4 +1,4 @@
-/* lcs_b200.h - C ABI of the B200-native LTE cell-search correlator.
+/* lcs_b200.h - C ABI of the GPU-native (H100, sm_90a) LTE cell-search correlator.
  *
  * This is the drop-in boundary for the hot path of Evrytania/LTE-Cell-Scanner: the free
  * functions of the reference's include/searcher.h (compiled into its static lib LTE_MISC,
@@ -13,7 +13,7 @@
  *   - complex arrays are interleaved (re,im); "c128" = complex<double> (IT++ cvec),
  *     "cf32" = complex<float>, "cu8" = raw rtl-sdr unsigned bytes, sample = (u8-127)/128
  *     (reference src/capbuf.cpp:172-175).
- *   - there is NO CPU fallback: every compute entry point needs a CUDA device (sm_100a) and
+ *   - there is NO CPU fallback: every compute entry point needs a CUDA device (sm_90a) and
  *     fails with LCS_ERR_CUDA when none is usable.
  *   - threading: a context and the plans / sweep handles created from it belong to ONE host thread at a time (they
  *     share the context's two streams and scratch buffers).  Use one context per thread; contexts are independent.

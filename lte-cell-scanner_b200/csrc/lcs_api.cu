@@ -109,7 +109,7 @@ using namespace lcs;
 
 extern "C" {
 
-const char* lcs_version(void) { return "lcs_b200 0.2 (sm_100a)"; }
+const char* lcs_version(void) { return "lcs_b200 0.3 (sm_90a)"; }
 
 lcs_status lcs_ctx_create(int device, lcs_ctx** out) {
   if (!out) return fail(nullptr, LCS_ERR_ARG, "ctx_create: null out pointer");
@@ -122,8 +122,8 @@ lcs_status lcs_ctx_create(int device, lcs_ctx** out) {
   cudaDeviceProp prop;
   e = cudaGetDeviceProperties(&prop, device);
   if (e != cudaSuccess) return fail(nullptr, LCS_ERR_CUDA, cudaGetErrorString(e));
-  if (prop.major != 10)
-    return fail(nullptr, LCS_ERR_CUDA, "device is not compute capability 10.x (kernels are built for sm_100a only)");
+  if (prop.major != 9 || prop.minor != 0)
+    return fail(nullptr, LCS_ERR_CUDA, "device is not compute capability 9.0 (kernels are built for sm_90a only)");
   e = cudaSetDevice(device);
   if (e != cudaSuccess) return fail(nullptr, LCS_ERR_CUDA, cudaGetErrorString(e));
   std::unique_ptr<lcs_ctx> c(new lcs_ctx());
@@ -207,7 +207,6 @@ lcs_status lcs_xcorr_plan_create(lcs_ctx* ctx, uint32_t n_cap, const double* f_s
 
 void lcs_xcorr_plan_destroy(lcs_xcorr_plan* plan) {
   if (!plan) return;
-  tc_prof_dump();
   cudaSetDevice(plan->ctx->device);
   cudaDeviceSynchronize();
   for (auto& ev : plan->ev_pool) { cudaEventDestroy(ev.first); cudaEventDestroy(ev.second); }

@@ -70,10 +70,10 @@ struct PlanSet {
   // tensor-core correlator operands
   bool tc_ready = false;
   std::string tc_why;              // why not, when !tc_ready
-  tc::Layout lay{16, 3, 2};
+  tc::Layout lay{48, 2};
   uint32_t n_pass = 1;
   float inv_scale = 0;             // 1 / (S * 128)
-  DevBuf<unsigned char> d_b;       // [n_plans][n_pass][lay.b_bytes()] int8 digit planes in UMMA core-matrix order
+  DevBuf<unsigned char> d_b;       // [n_plans][n_pass][lay.b_bytes()] int8 digit planes in wgmma core-matrix order
   DevBuf<float> d_corr;            // [n_plans][n_pass][2][npad]
   DevBuf<tc::PassGeo> d_geo;       // [n_plans][n_pass]
   DevBuf<int16_t> d_dsh;           // [n_plans][n_pass][M_MAX][npad] fold offset of the column minus the pass minimum
@@ -169,7 +169,6 @@ lcs_status cell_chain_dev(lcs_ctx* ctx, const void* d_cap, int fmt, uint32_t n_c
 lcs_status tc_init(lcs_ctx* ctx);           // one-time function attributes
 int launch_xcorr_fold_tc(PlanSet& ps, const void* d_iq_cu8, uint32_t batch, const uint32_t* d_buf_plan,
                          float* d_single_planar, cudaStream_t st);
-void tc_prof_dump();
 // ---- lcs_api.cu ----
 lcs_status plan_run_device(lcs_xcorr_plan* p, const void* d_iq, int iq_format, uint32_t batch, float* d_single, double* d_pow,
                            int32_t* d_frq, double* d_spi, float* d_inc, cudaStream_t st);

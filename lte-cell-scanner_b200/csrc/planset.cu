@@ -5,8 +5,8 @@
 //          per-pass minima / spreads of the tensor-core correlator, tile geometry of the FP32 correlator
 //   device plan_build_kernel: the pre-rotated templates conj(fshift(pss_td[t], f_off, fs*k_factor))/137
 //          (searcher.cpp:145-151 with dsp.h:40-53) in double precision, rounded once to FP32 for the CUDA-core
-//          correlator and to 24-bit fixed point, split in three balanced int8 digit planes in UMMA core-matrix order,
-//          for the tcgen05 correlator, plus the per-template additive constants of the v-128 sample representation.
+//          correlator and to 24-bit fixed point, split in three balanced int8 digit planes in wgmma core-matrix order,
+//          for the tensor-core correlator, plus the per-template additive constants of the v-128 sample representation.
 #include <cmath>
 #include <cstring>
 
@@ -97,14 +97,15 @@ __global__ void __launch_bounds__(160) plan_build_kernel(const double* __restric
 }
 
 static tc::Layout pick_layout(uint32_t n_f, uint32_t& n_pass) {
+  // one consumer warpgroup per job: two jobs let one warpgroup's epilogue overlap the other one's MMAs
   n_pass = 1;
-  if (n_f <= 5) return tc::Layout{16, 1, 1};       // tracker shape (one offset): N = 48, four epilogue warps
-  if (n_f <= 16) return tc::Layout{16, 3, 1};
-  if (n_f <= 21) return tc::Layout{16, 4, 1};
-  if (n_f <= 32) return tc::Layout{16, 3, 2};
-  if (n_f <= 42) { n_pass = 2; return tc::Layout{16, 4, 1}; }
+  if (n_f <= 5) return tc::Layout{16, 1};          // tracker shape (one offset): N = 48, one consumer warpgroup
+  if (n_f <= 16) return tc::Layout{24, 2};         // N = 80
+  if (n_f <= 21) return tc::Layout{32, 2};         // N = 96
+  if (n_f <= 32) return tc::Layout{48, 2};         // N = 144
+  if (n_f <= 42) { n_pass = 2; return tc::Layout{32, 2}; }
   n_pass = (n_f + 31) / 32;
-  return tc::Layout{16, 3, 2};
+  return tc::Layout{48, 2};
 }
 
 lcs_status planset_build(lcs_ctx* ctx, PlanSet& ps, uint32_t n_cap, uint8_t arm, const std::vector<PlanCfg>& cfgs,
@@ -265,8 +266,8 @@ lcs_status planset_build(lcs_ctx* ctx, PlanSet& ps, uint32_t n_cap, uint8_t arm,
 int planset_resolve_kernel(const PlanSet& ps, int kernel, int iq_format) {
   if (kernel == LCS_KERNEL_FP32) return LCS_KERNEL_FP32;
   if (kernel == LCS_KERNEL_TC) return LCS_KERNEL_TC;
-  // AUTO: the tensor-core kernel is exact only for 8-bit IQ; for that format it is the faster one at every grid size
-  // (even the single-offset tracker shape: one N = 48 job per part, ~6 us per buffer against 11 us on the FP32 cores).
+  // AUTO: the tensor-core kernel is exact only for 8-bit IQ, so it serves that format (the single-offset tracker shape
+  // included: one N = 48 job per part); other formats go to the FP32 correlator.
   return (iq_format == LCS_IQ_CU8 && ps.tc_ready) ? LCS_KERNEL_TC : LCS_KERNEL_FP32;
 }
 

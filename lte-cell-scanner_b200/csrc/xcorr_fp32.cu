@@ -373,7 +373,7 @@ __device__ __forceinline__ float div_small_odd(float x) {
 
 // Vectorised variant for ds_comb_arm <= 4: one thread = 4 consecutive fold positions, three 128-bit loads per hypothesis
 // (previous / own / next quad; the neighbours' quads are L1 hits; 9600 % 4 == 0 so the circular wrap is a quad index
-// wrap).  HBM-bound: 5.1 TB/s in the round-2 ncu capture.
+// wrap).  HBM-bound.
 template <int ARM>
 __global__ void __launch_bounds__(128) epilogue4_kernel(const float* __restrict__ single_planar, double* __restrict__ pow_out,
                                                         int32_t* __restrict__ frq_out, float* __restrict__ incoherent_planar,

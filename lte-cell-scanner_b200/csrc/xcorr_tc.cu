@@ -1,4 +1,4 @@
-// xcorr_tc.cu - PSS correlator on the 5th-generation tensor cores (tcgen05 / TMEM), exact for 8-bit IQ.
+// xcorr_tc.cu - PSS correlator on the Hopper tensor cores (warpgroup wgmma), exact for 8-bit IQ.
 //
 // The sliding correlation is a Toeplitz GEMM: D[lag, template] = sum_j z[2*lag + j] * W[template, j],
 // j = 0..273 over the interleaved I/Q byte stream z of the capture buffer (rtl-sdr wire format,
@@ -8,21 +8,21 @@
 //   * each template component W (double, conj(fshift(pss_td))/137 of searcher.cpp:145-151) is scaled by
 //     a power of two S and rounded to a 24-bit integer, split into three balanced base-256 digits
 //     W*S = 65536 a0 + 256 a1 + a2, a_j in [-128,127] -> three int8 B operand planes (built on the device, planset.cu),
-//   * tcgen05.mma kind::i8 (s8 x s8 -> s32 accumulators in TMEM): |sum| <= 274*128*128 < 2^23, no overflow,
+//   * wgmma.mma_async ... .s32.s8.s8 (s8 x s8 -> s32 accumulators in registers): |sum| <= 274*128*128 < 2^23, no overflow,
 //   * real part uses the byte stream as is, the imaginary part a second stream with every (I,Q) pair
 //     replaced by (Q, ~I)  (~I = -I'-1): sum a[2m]*Q' + a[2m+1]*(-I'-1) with the same template rows
 //     a[2m] = Re W, a[2m+1] = -Im W.
 //
-// Operand roles: the 128 LAGS of a sub-tile are the M dimension (TMEM lanes), the templates the N dimension (TMEM columns).
-// A JOB is one UMMA N dimension holding all three digit planes of C template columns (tc_layout.hpp); a pass has J jobs.
-// Each job has its own set of epilogue warps, so the J sets work half a period apart: while one set drains TMEM the
-// other one converts and folds - the tensor pipe, TMEM reads, FP32 pipe and shared-memory traffic overlap instead of
-// arriving in bursts.
+// Operand roles: 64 LAGS of a sub-tile are the M dimension (wgmma m64), the templates the N dimension.  A JOB is one
+// wgmma N dimension holding all three digit planes of C template columns (tc_layout.hpp); a pass has J jobs and the CTA
+// one consumer warpgroup per job.  A warpgroup issues the MMAs of its job, waits for them and runs the epilogue
+// (digit recombination, |xc|^2, fold) on the accumulator registers; while one warpgroup is in its epilogue the tensor
+// core works on the other one's MMAs.
 //
 // The Toeplitz (Hankel) A operand is never materialised per lag: an "expanded" tile P[u][r][16 B] = z[16u+2r ..+15]
 // is built once per 256-lag tile in shared memory (8x expansion of ~0.8 KB of raw bytes that a 1-D TMA bulk copy,
 // cp.async.bulk + mbarrier complete_tx, stages one tile ahead); block u is exactly the 8-row x 16-byte K-major core
-// matrix of (row group g, K chunk c) for every g+c = u, so one UMMA shared-memory descriptor with LBO = SBO = 128 B
+// matrix of (row group g, K chunk c) for every g+c = u, so one wgmma shared-memory descriptor with LBO = SBO = 128 B
 // addresses the whole Hankel tile.  The template planes stay resident in shared memory in core-matrix order (loaded by
 // TMA bulk copies whenever the CTA moves to another plan / pass).
 //
@@ -39,20 +39,7 @@
 #include <cmath>
 
 #include "lcs_ctx.hpp"
-
-// Build with -DLCS_TC_PROFILE=1 to collect per-CTA cycle counters of the pipeline stages (printed when a plan is
-// destroyed with LCS_TC_PROF=1 in the environment); off by default so that the clock reads cost nothing.
-#ifndef LCS_TC_PROFILE
-#define LCS_TC_PROFILE 0
-#endif
-#ifndef LCS_TC_EXP
-#define LCS_TC_EXP 0     // timing experiments (wrong results): 1 = no fold, 2 = drain only, 3 = no write-out, 4 = slots released unread
-#endif
-#if LCS_TC_PROFILE
-#define TC_CLK() clock64()
-#else
-#define TC_CLK() 0ll
-#endif
+#include "wgmma_s8.hpp"
 
 namespace lcs {
 
@@ -60,7 +47,7 @@ struct TcParams {
   const uint8_t* iq;          // [batch][n_cap][2] raw bytes, 16-byte aligned
   unsigned long long iq_bytes;   // size of that allocation
   const uint32_t* buf_plan;   // [batch] plan of each buffer, or NULL (plan 0 for all)
-  const uint8_t* b_img;       // [plan][pass][b_bytes] digit planes in UMMA core-matrix order
+  const uint8_t* b_img;       // [plan][pass][b_bytes] digit planes in core-matrix order
   const float* corr;          // [plan][pass][2][npad] (C_re row, C_im row), MAGIC_VAL already subtracted
   const tc::PassGeo* geo;     // [plan][pass]
   const int16_t* dsh;         // [plan][pass][M_MAX][npad] fold offset of the column minus the pass minimum
@@ -70,7 +57,6 @@ struct TcParams {
   uint32_t n_tiles_total;     // n_units * tu
   float inv2s;                // 1 / (S*128)^2
   float rcp_ncomb;            // RN(1 / n_comb) when the 3-instruction division is exact for n_comb, else 0
-  long long* prof;            // optional [grid][12] cycle counters (NULL = off)
 };
 
 // ---- small PTX wrappers ----
@@ -84,8 +70,7 @@ __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
 __device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
 }
-// try_wait parks the warp until the phase completes or the suspend-time hint (ns) expires (hints of 100 ns ... 20 us
-// measured identical: the polling seen in ncu r02c does not cost kernel time)
+// try_wait parks the warp until the phase completes or the suspend-time hint (ns) expires
 #ifndef LCS_TC_WAIT_HINT_NS
 #define LCS_TC_WAIT_HINT_NS 2000
 #endif
@@ -107,48 +92,21 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst_smem, const void* src, uin
                "r"(bytes), "r"(bar)
                : "memory");
 }
+// wgmma matrix descriptor, no swizzle (K-major core matrices of 8 rows x 16 bytes): start>>4 [0,14), LBO>>4 [16,30)
+// = distance of core matrices along K, SBO>>4 [32,46) = distance of 8-row groups, base offset 0, layout type 0
 __device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  // SmemDescriptor (mma_sm100_desc.hpp): start>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46), version=1 [46,48), no swizzle
-  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)(sbo_bytes >> 4) << 32) |
-         (1ull << 46);
+  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)(sbo_bytes >> 4) << 32);
 }
-// UTCIMMA instruction descriptor (cute/arch/mma_sm100_desc.hpp InstrDescriptor): c_format S32 (2) bits[4,6);
-// a_format / b_format = 1 (signed 8 bit) bits [7,10) / [10,13); K-major A and B; N>>3 bits [17,23); M>>4 bits [24,29)
-__host__ __device__ constexpr uint32_t tc_idesc(int n) {
-  return (2u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(n >> 3) << 17) | ((128u >> 4) << 24);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait0(int (&d)[N]) {
+  asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+#pragma unroll
+  for (int i = 0; i < N; i++) asm volatile("" : "+r"(d[i])::"memory");   // the accumulators are read only after the wait
 }
-// Variants guarded by an "elected lane" flag so that the issuing warp stays convergent: the compiler then keeps
-// descriptors in uniform registers and emits one UTCIMMA per call instead of an elect-and-loop sequence.
-__device__ __forceinline__ uint32_t elect_one_flag() {
-  uint32_t r;
-  asm volatile("{\n.reg .pred p;\nelect.sync _|p, 0xffffffff;\nselp.u32 %0, 1, 0, p;\n}\n" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void umma_i8_g(uint32_t flag, uint32_t d_tmem, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p, q;\n"
-      "setp.ne.b32 q, %5, 0;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "@q tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(d_tmem), "l"(da), "l"(db), "r"(idesc), "r"(accumulate), "r"(flag)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit_g(uint32_t flag, uint32_t bar) {
-  asm volatile("{\n.reg .pred q;\nsetp.ne.b32 q, %1, 0;\n@q tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n}\n" ::"r"(bar), "r"(flag) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, int (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void epi_bar(uint32_t id, uint32_t nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
+__device__ __forceinline__ void named_bar(uint32_t id, uint32_t nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
 
 // ---- work distribution: runs of consecutive tiles (see the header comment) ----
 struct TcRun {
@@ -202,36 +160,29 @@ struct TcStep {            // (run, tile, half frame) cursor of the producer war
   }
 };
 
-// registers are allocated per group of 4 warps: 18 warps count as 20
-__host__ __device__ constexpr int tc_maxreg(int threads) {
-  const int alloc_threads = (threads + 127) / 128 * 128;
-  return (65536 / alloc_threads) / 8 * 8 > 128 ? 128 : (65536 / alloc_threads) / 8 * 8;
-}
-
 // shared-memory map
-template <int NC, int NGRP, int J>
+template <int C, int J>
 struct TcSmem {
-  static constexpr tc::Layout L{NC, NGRP, J};
+  static constexpr tc::Layout L{C, J};
   static constexpr int P = 0;                                          // [2 stages][2 variants][P_BYTES]
   static constexpr int B = P + 4 * tc::P_BYTES;                        // [J][njob/8][KCHUNKS][8][16] int8
-  static constexpr int WIN = B + L.b_bytes();                          // [npad][WSTR] float
-  static constexpr int CORR = WIN + L.npad() * tc::WSTR * 4;           // [2][npad] float
+  static constexpr int WIN = B + L.b_bytes();                          // [npad][WROW] float
+  static constexpr int CORR = WIN + L.npad() * tc::WROW * 4;           // [2][npad] float
   static constexpr int DOFF = CORR + 2 * L.npad() * 4;                 // [M_MAX][npad] int32 byte offsets (-4 * dsh)
   static constexpr int RAW = DOFF + tc::M_MAX * L.npad() * 4;          // [2][RAW_BYTES]
-  static constexpr int BAR = RAW + 2 * tc::RAW_BYTES;                  // 16 mbarriers
-  static constexpr int MISC = BAR + 16 * 8;
-  static constexpr int TOTAL = MISC + 64;
+  static constexpr int BAR = RAW + 2 * tc::RAW_BYTES;                  // 8 mbarriers
+  static constexpr int TOTAL = BAR + 8 * 8;
 };
 
-template <int NC, int NGRP, int J>
-__global__ void __maxnreg__(tc_maxreg(64 + 128 * NGRP * J))
-xcorr_fold_tc_kernel(const __grid_constant__ TcParams p) {
-  using SM = TcSmem<NC, NGRP, J>;
-  constexpr tc::Layout LAY{NC, NGRP, J};
-  constexpr int C = LAY.c(), NPAD = LAY.npad(), NJOB = LAY.njob(), NSLOT = LAY.nslot();
-  constexpr int THREADS = LAY.threads(), SET_THREADS = 32 * 4 * NGRP;     // SET_THREADS: epilogue threads of one job
-  static_assert(NC == 16, "one tcgen05.ld.x16 per digit plane");
-  static_assert(NSLOT >= 2 && NSLOT >= J, "TMEM ring too short");
+template <int C, int J>
+__global__ void __launch_bounds__(128 + 128 * J, 1) xcorr_fold_tc_kernel(const __grid_constant__ TcParams p) {
+  using SM = TcSmem<C, J>;
+  constexpr tc::Layout LAY{C, J};
+  constexpr int NPAD = LAY.npad(), NJOB = LAY.njob();
+  constexpr int NACC = NJOB / 2;          // accumulator registers per thread (m64 x NJOB s32 over 128 threads)
+  constexpr int CG = C / 8;               // 8-column groups of one digit plane
+  constexpr int NV = C / 2;               // results per thread and part: 2 rows x 2 columns per 8-column group
+  static_assert(C % 8 == 0, "digit planes must start on an 8-column group of the accumulator fragment");
   static_assert(SM::TOTAL <= 232448, "shared memory");
   extern __shared__ __align__(128) uint8_t smem[];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -240,37 +191,21 @@ xcorr_fold_tc_kernel(const __grid_constant__ TcParams p) {
   float* sCorr = reinterpret_cast<float*>(smem + SM::CORR);
   int* sDoff = reinterpret_cast<int*>(smem + SM::DOFF);
   const uint32_t bar0 = smem_u32(smem + SM::BAR);
-  // barriers (8 B each): 0,1 p_full[stage]; 2,3 p_empty[stage]; 4,5 raw_full[stage]; 6..9 slot_full; 10..13 slot_empty;
-  // 14 b_full; 15 drain
-  const uint32_t BAR_PFULL = bar0, BAR_PEMPTY = bar0 + 16, BAR_RAW = bar0 + 32, BAR_SFULL = bar0 + 48, BAR_SEMPTY = bar0 + 80,
-                 BAR_BFULL = bar0 + 112, BAR_DRAIN = bar0 + 120;
-  volatile uint32_t* tmem_slot = reinterpret_cast<volatile uint32_t*>(smem + SM::MISC);
+  // barriers (8 B each): 0,1 p_full[stage]; 2,3 p_empty[stage]; 4,5 raw_full[stage]; 6,7 b_full[job]
+  const uint32_t BAR_PFULL = bar0, BAR_PEMPTY = bar0 + 16, BAR_RAW = bar0 + 32, BAR_BFULL = bar0 + 48;
 
   // ---- one-time setup ----
-  for (int i = tid; i < NPAD * tc::WSTR; i += THREADS) sWin[i] = 0.f;
+  for (int i = tid; i < NPAD * tc::WROW; i += LAY.threads()) sWin[i] = 0.f;
   if (tid == 0) {
     for (int i = 0; i < 2; i++) {
       mbar_init(BAR_PFULL + 8 * i, 1);
-      mbar_init(BAR_PEMPTY + 8 * i, 1);        // tcgen05.commit
+      mbar_init(BAR_PEMPTY + 8 * i, 4 * J);    // every consumer warp, after its warpgroup's MMAs on the stage retired
       mbar_init(BAR_RAW + 8 * i, 1);           // arrive.expect_tx of the producer + TMA bytes
+      mbar_init(BAR_BFULL + 8 * i, 1);
     }
-    for (int i = 0; i < 4; i++) {
-      mbar_init(BAR_SFULL + 8 * i, 1);         // tcgen05.commit
-      mbar_init(BAR_SEMPTY + 8 * i, 4 * NGRP); // the epilogue warps of the job that used the slot
-    }
-    mbar_init(BAR_BFULL, 1);
-    mbar_init(BAR_DRAIN, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {  // TMEM allocation (whole warp), address lands in shared memory
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32((const void*)tmem_slot)),
-                 "r"(tc::TMEM_COLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   if (warp == 0) {
     // ================= producer: raw bytes by TMA one step ahead, expansion into the Hankel tile =================
@@ -343,129 +278,46 @@ xcorr_fold_tc_kernel(const __grid_constant__ TcParams p) {
       zo_cur = zo_nxt;
       if (nxt.ok) nxt.advance(p);
     }
-  } else if (warp == 1) {
-    // ================= MMA issuer: the whole warp walks the pipeline convergently, one elected lane issues ====
-    const uint32_t sP_addr = smem_u32(sP), sB_addr = smem_u32(smem + SM::B);
-    const uint32_t flag = elect_one_flag();
-    constexpr uint32_t IDESC = tc_idesc(NJOB);
-    // descriptors advance by adding to the 14-bit (address >> 4) field: +16 per 256-byte K step
-    uint32_t slot = 0, ph = 0;          // TMEM ring position of the next job
-    uint32_t cur_pp = 0xffffffffu, drain_par = 0, bfull_par = 0, step = 0;
-    long long t_pwait = 0, t_swait = 0, t_bload = 0, t_start = TC_CLK();
-    TcRunIter it;
-    it.init(p);
-    TcRun r;
-    while (it.next(p, r)) {
-      if (r.pp != cur_pp) {
-        // another plan / pass: wait until every MMA that reads the resident templates has retired, then TMA the new ones
-        long long c0 = TC_CLK();
-        if (cur_pp != 0xffffffffu) {
-          umma_commit_g(flag, BAR_DRAIN);
-          mbar_wait(BAR_DRAIN, drain_par);
-          drain_par ^= 1;
-        }
-        if (lane == 0) {
-          constexpr uint32_t B_BYTES = (uint32_t)LAY.b_bytes(), CHUNK = 27648;     // 12 row groups of 2304 B per copy
-          mbar_arrive_expect_tx(BAR_BFULL, B_BYTES);
-          const uint8_t* src = p.b_img + (size_t)r.pp * B_BYTES;
-          for (uint32_t o = 0; o < B_BYTES; o += CHUNK) bulk_g2s(sB_addr + o, src + o, min(CHUNK, B_BYTES - o), BAR_BFULL);
-        }
-        __syncwarp();
-        mbar_wait(BAR_BFULL, bfull_par);
-        bfull_par ^= 1;
-        cur_pp = r.pp;
-        t_bload += TC_CLK() - c0;
-      }
-      for (uint32_t km = 0; km < r.n_tiles * p.n_comb; km++, step++) {
-        const uint32_t stage = step & 1, use = step >> 1;
-        long long c0 = TC_CLK();
-        mbar_wait(BAR_PFULL + 8 * stage, use & 1);
-        t_pwait += TC_CLK() - c0;
-        tc_fence_after();
-#pragma unroll 1
-        for (int q = 0; q < tc::NSUB; q++) {
+  } else if (warp >= 4) {
+    // ================= consumers: one warpgroup per job - MMAs, then |xc|^2 and the fold on the accumulators =========
+    const int job = (warp >> 2) - 1;
+    const int wq = warp & 3;                        // warp of the warpgroup: accumulator rows 16*wq .. +15
+    const int wt = tid - 128 * (job + 1);           // thread of the warpgroup
+    const int cb = 2 * (lane & 3);                  // first of the two columns this thread holds in each 8-column group
+    const uint32_t BAR_ID = 1 + job;                // named barrier of the warpgroup
+    const uint32_t sP_addr = smem_u32(sP), sBj_addr = smem_u32(smem + SM::B + job * LAY.b_job_bytes());
+    const uint32_t my_bfull = BAR_BFULL + 8 * job;
+    // window row of column (job*C + cb) at the fold position of accumulator row (lane>>2) of this warp's 16 rows
+    char* myWinB = reinterpret_cast<char*>(sWin + (job * C + cb) * tc::WROW + tc::HALO + 16 * wq + (lane >> 2));
+    const float* cre = sCorr + job * C + cb;
+    const float* cim = sCorr + NPAD + job * C + cb;
+    uint32_t cur_pp = 0xffffffffu, bfull_par = 0, step = 0;
+    // One part (re or im) of one 64-lag sub-tile: 9 MMAs over K, then value = (a0*256 + a1)*256 + a2 + constant for the
+    // 2 rows x C/4 columns of this thread.  acc register 4*g + 2*h + e holds row (lane>>2) + 8h, column 8g + cb + e.
+    auto mma_part = [&](int (&acc)[NACC], uint32_t a_addr) {
+      const uint64_t a_desc = make_desc(a_addr, 128, 128), b_desc = make_desc(sBj_addr, 128, tc::B_SBO);
+      wgmma_fence();
 #pragma unroll
-          for (int v = 0; v < 2; v++) {
-            const uint64_t a_desc = make_desc(sP_addr + (stage * 2 + v) * tc::P_BYTES + q * (tc::NSUBL / 8) * 128, 128, 128);
+      for (int s = 0; s < tc::KSTEPS; s++) tc::wgmma_s8<NJOB>(acc, a_desc + (uint64_t)(s * 16), b_desc + (uint64_t)(s * 16), s > 0);
+      wgmma_commit();
+      wgmma_wait0(acc);
+    };
+    auto recombine = [&](const int (&acc)[NACC], float (&x)[NV], const float* kc) {
 #pragma unroll
-            for (int g = 0; g < J; g++) {
-              const uint64_t b_desc = make_desc(sB_addr + g * LAY.b_job_bytes(), 128, tc::B_SBO);
-              c0 = TC_CLK();
-              mbar_wait(BAR_SEMPTY + 8 * slot, ph ^ 1);
-              t_swait += TC_CLK() - c0;
-              tc_fence_after();
+      for (int g = 0; g < CG; g++) {
+        const float2 k2 = *reinterpret_cast<const float2*>(kc + 8 * g);
+        const float kk[2] = {k2.x, k2.y};
 #pragma unroll
-              for (int s = 0; s < tc::KSTEPS; s++)
-                umma_i8_g(flag, tmem_base + slot * NJOB, a_desc + (uint64_t)(s * 16), b_desc + (uint64_t)(s * 16), IDESC, s > 0);
-              umma_commit_g(flag, BAR_SFULL + 8 * slot);
-              if (++slot == NSLOT) { slot = 0; ph ^= 1; }
-            }
+        for (int h = 0; h < 2; h++)
+#pragma unroll
+          for (int e = 0; e < 2; e++) {
+            const int r = 4 * g + 2 * h + e;
+            const int t = acc[r] * 256 + acc[r + 4 * CG];
+            // float(a2) without an I2F: |a2| < 2^22, so the bit pattern MAGIC_BITS + a2 is the float 1.5*2^23 + a2 (exact);
+            // the constant kk already has -1.5*2^23 folded in
+            const float f2 = __int_as_float((int)tc::MAGIC_BITS + acc[r + 8 * CG]);
+            x[(g * 2 + h) * 2 + e] = __fadd_rn(__fmaf_rn((float)t, 256.f, f2), kk[e]);
           }
-        }
-        umma_commit_g(flag, BAR_PEMPTY + 8 * stage);                  // P stage free again
-      }
-    }
-    if (LCS_TC_PROFILE && p.prof && lane == 0) {
-      p.prof[blockIdx.x * 12 + 0] = TC_CLK() - t_start;
-      p.prof[blockIdx.x * 12 + 1] = t_pwait;
-      p.prof[blockIdx.x * 12 + 2] = t_swait;
-      p.prof[blockIdx.x * 12 + 3] = t_bload;
-    }
-  } else {
-    // ================= epilogue: TMEM -> |xc|^2 -> fold =================
-    const int ewarp = warp - 2;                     // epilogue numbering
-    const int quarter = warp & 3;                   // TMEM lanes 32*quarter .. +31 are accessible to this warp
-    const int cell = ewarp >> 2;                    // (job, column group)
-    const int job = cell / NGRP, grp = cell - job * NGRP;
-    const int Lg = quarter * 32 + lane;             // lag row of the sub-tile
-    const int col0 = job * C + grp * NC;            // first template column (of the pass) of this warp
-    char* myWinB = reinterpret_cast<char*>(sWin + col0 * tc::WSTR + tc::HALO + Lg);
-    const float* cre = sCorr + col0;
-    const float* cim = sCorr + NPAD + col0;
-    const uint32_t lane_base = tmem_base + ((uint32_t)(quarter * 32) << 16) + grp * NC;
-    uint32_t slot = job % NSLOT, ph = 0;            // TMEM ring position of this job set's next job
-    uint32_t cur_pp = 0xffffffffu;
-    long long t_fwait = 0, t_ld = 0, t_wout = 0, e_start = TC_CLK();
-    // One part (re or im) of one sub-tile: wait for the job, pull the three digit planes of this warp's 32 lags x NC
-    // templates into registers, release the TMEM slot, recombine: value = (a0*256 + a1)*256 + a2 + constant.
-    auto drain_part = [&](float (&x)[NC], const float* kc) {
-      int t[NC], a[NC];
-      long long c0 = TC_CLK();
-      mbar_wait(BAR_SFULL + 8 * slot, ph);
-      long long c1 = TC_CLK();
-      t_fwait += c1 - c0;
-      tc_fence_after();
-      const uint32_t src = lane_base + slot * NJOB;
-#if LCS_TC_EXP == 4          // timing experiment: slots released unread (wrong results)
-      for (int c = 0; c < NC; c++) { t[c] = c; a[c] = c; }
-      if (false)
-#endif
-      {
-      tmem_ld16(src, t);
-      tmem_ld16(src + C, a);
-      tmem_ld_wait();
-#pragma unroll
-      for (int c = 0; c < NC; c++) t[c] = t[c] * 256 + a[c];
-      tmem_ld16(src + 2 * C, a);
-      tmem_ld_wait();
-      }
-      t_ld += TC_CLK() - c1;
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(BAR_SEMPTY + 8 * slot);
-      slot += J;
-      if (slot >= NSLOT) { slot -= NSLOT; ph ^= 1; }
-#pragma unroll
-      for (int c = 0; c < NC; c += 4) {
-        const float4 k4 = *reinterpret_cast<const float4*>(kc + c);
-        const float kk[4] = {k4.x, k4.y, k4.z, k4.w};
-#pragma unroll
-        for (int e = 0; e < 4; e++) {
-          // float(a2) without an I2F: |a2| < 2^22, so the bit pattern MAGIC_BITS + a2 is the float 1.5*2^23 + a2 (exact);
-          // the constant kk already has -1.5*2^23 folded in
-          const float f2 = __int_as_float((int)tc::MAGIC_BITS + a[c + e]);
-          x[c + e] = __fadd_rn(__fmaf_rn((float)t[c + e], 256.f, f2), kk[e]);
-        }
       }
     };
     TcRunIter it;
@@ -473,80 +325,95 @@ xcorr_fold_tc_kernel(const __grid_constant__ TcParams p) {
     TcRun r;
     while (it.next(p, r)) {
       if (r.pp != cur_pp) {
-        // constants and fold offsets of the new plan / pass: every job set loads those of its own C columns
-        epi_bar(1 + job, SET_THREADS);
-        const int et = (ewarp - job * 4 * NGRP) * 32 + lane;       // thread index inside the set
+        // another plan / pass: this job's templates by TMA (every MMA that read the old ones has been waited for), its
+        // constants and fold offsets by the warpgroup
+        named_bar(BAR_ID, 128);
+        if (wt == 0) {
+          constexpr uint32_t B_BYTES = (uint32_t)LAY.b_job_bytes(), CHUNK = 27648;     // 12 row groups of 2304 B per copy
+          mbar_arrive_expect_tx(my_bfull, B_BYTES);
+          const uint8_t* src = p.b_img + (size_t)r.pp * LAY.b_bytes() + (size_t)job * B_BYTES;
+          for (uint32_t o = 0; o < B_BYTES; o += CHUNK) bulk_g2s(sBj_addr + o, src + o, min(CHUNK, B_BYTES - o), my_bfull);
+        }
         const float* gc = p.corr + (size_t)r.pp * 2 * NPAD;
         const int16_t* gd = p.dsh + (size_t)r.pp * tc::M_MAX * NPAD;
-        for (int i = et; i < 2 * C; i += SET_THREADS) {
+        for (int i = wt; i < 2 * C; i += 128) {
           const int o = (i / C) * NPAD + job * C + i % C;
           sCorr[o] = __ldg(gc + o);
         }
-        for (int i = et; i < (int)p.n_comb * C; i += SET_THREADS) {
+        for (int i = wt; i < (int)p.n_comb * C; i += 128) {
           const int o = (i / C) * NPAD + job * C + i % C;
           sDoff[o] = -4 * (int)__ldg(gd + o);
         }
-        epi_bar(1 + job, SET_THREADS);
+        named_bar(BAR_ID, 128);
+        mbar_wait(my_bfull, bfull_par);
+        bfull_par ^= 1;
         cur_pp = r.pp;
       }
       const int f0 = __ldg(&p.geo[r.pp].f0);
       const uint32_t n_templ = 3u * (uint32_t)__ldg(&p.geo[r.pp].n_f);
       for (uint32_t k = 0; k < r.n_tiles; k++) {
-        for (uint32_t m = 0; m < p.n_comb; m++) {
-          const int* doff = sDoff + m * NPAD + col0;        // -4 * (fold offset of the column - pass minimum), bytes
+        for (uint32_t m = 0; m < p.n_comb; m++, step++) {
+          const uint32_t stage = step & 1, use = step >> 1;
+          // -4 * (fold offset of the column - pass minimum), bytes, for the C/4 columns of this thread
+          int d[CG][2];
 #pragma unroll
+          for (int g = 0; g < CG; g++) {
+            const int2 d2 = *reinterpret_cast<const int2*>(sDoff + m * NPAD + job * C + cb + 8 * g);
+            d[g][0] = d2.x;
+            d[g][1] = d2.y;
+          }
+          mbar_wait(BAR_PFULL + 8 * stage, use & 1);
+          const uint32_t a_stage = sP_addr + stage * 2 * tc::P_BYTES;
+#pragma unroll 1
           for (int q = 0; q < tc::NSUB; q++) {
-            float x[NC], rr[NC];
-#if LCS_TC_EXP == 2 || LCS_TC_EXP == 4   // timing experiments: drain + release only (wrong results)
-            drain_part(x, cre);
-            drain_part(rr, cim);
-            if (x[0] + rr[1] == 1.2345f) sWin[0] = 1.f;
-            continue;
-#endif
-            drain_part(x, cre);
+            int acc[NACC];
+            float x[NV], rr[NV];
+            mma_part(acc, a_stage + q * (tc::NSUBL / 8) * 128);
+            recombine(acc, x, cre);
 #pragma unroll
-            for (int c = 0; c < NC; c++) rr[c] = __fmul_rn(x[c], x[c]);
-            drain_part(x, cim);
+            for (int v = 0; v < NV; v++) rr[v] = __fmul_rn(x[v], x[v]);
+            mma_part(acc, a_stage + tc::P_BYTES + q * (tc::NSUBL / 8) * 128);
+            if (q == tc::NSUB - 1 && lane == 0) mbar_arrive(BAR_PEMPTY + 8 * stage);     // P stage free again
+            recombine(acc, x, cim);
             // |xc|^2 = re^2 + im^2 (searcher.cpp:300), in the integer scale of the templates; the power-of-two scale
             // factor is applied when the tile is written out
 #pragma unroll
-            for (int c = 0; c < NC; c++) rr[c] = __fmaf_rn(x[c], x[c], rr[c]);
-            // fold into the sliding window: lag q*128 + Lg of the tile lands at window index lag + HALO - dsh; all loads
+            for (int v = 0; v < NV; v++) rr[v] = __fmaf_rn(x[v], x[v], rr[v]);
+            // fold into the sliding window: lag q*64 + row of the tile lands at window index lag + HALO - dsh; all loads
             // of the read-modify-write first, then add + store
-            int d[NC];
 #pragma unroll
-            for (int c = 0; c < NC; c += 4) {
-              const int4 d4 = *reinterpret_cast<const int4*>(doff + c);
-              d[c] = d4.x; d[c + 1] = d4.y; d[c + 2] = d4.z; d[c + 3] = d4.w;
-            }
-#if LCS_TC_EXP == 1          // timing experiment: no fold (wrong results)
-            if (rr[0] == 1.2345f) sWin[0] = rr[NC - 1];
-            continue;
-#endif
+            for (int g = 0; g < CG; g++)
 #pragma unroll
-            for (int c = 0; c < NC; c++) x[c] = *reinterpret_cast<const float*>(myWinB + d[c] + (c * tc::WSTR + q * tc::NSUBL) * 4);
+              for (int h = 0; h < 2; h++)
 #pragma unroll
-            for (int c = 0; c < NC; c++) *reinterpret_cast<float*>(myWinB + d[c] + (c * tc::WSTR + q * tc::NSUBL) * 4) = __fadd_rn(x[c], rr[c]);
+                for (int e = 0; e < 2; e++)
+                  x[(g * 2 + h) * 2 + e] =
+                      *reinterpret_cast<const float*>(myWinB + d[g][e] + ((8 * g + e) * tc::WROW + q * tc::NSUBL + 8 * h) * 4);
+#pragma unroll
+            for (int g = 0; g < CG; g++)
+#pragma unroll
+              for (int h = 0; h < 2; h++)
+#pragma unroll
+                for (int e = 0; e < 2; e++) {
+                  const int v = (g * 2 + h) * 2 + e;
+                  *reinterpret_cast<float*>(myWinB + d[g][e] + ((8 * g + e) * tc::WROW + q * tc::NSUBL + 8 * h) * 4) = __fadd_rn(x[v], rr[v]);
+                }
           }
-          // The four lane-quarter warps of a column group fold into the same window rows; a lag of one quarter at this
-          // half frame and a lag of its neighbour at the next one (different fold offset) can hit the same window index.
-          // The MMA pipeline keeps them a job apart in practice; this 128-thread barrier makes the ordering a guarantee.
-          epi_bar(3 + cell, 128);
+          // A lag of one warp at this half frame and a lag of another warp at the next one (different fold offset) can hit
+          // the same window index: the warpgroup finishes one half frame's read-modify-writes before the next one starts.
+          named_bar(BAR_ID, 128);
         }
         // ---- tile done: the 256 oldest window positions are final -> xc_incoherent_single rows (coalesced); the HALO
-        // youngest carry over to the next tile of the run ----
-        // A job set owns the window rows of its C columns exclusively, so the two sets write out independently (named
-        // barrier 1 + job): while one set is in its write-out the other keeps draining its jobs.
-        long long c0 = TC_CLK();
-        epi_bar(1 + job, SET_THREADS);
+        // youngest carry over to the next tile of the run.  A warpgroup owns the window rows of its C columns exclusively,
+        // so the jobs write out independently: while one is in its write-out the other keeps the tensor core busy. ----
         const float ncf = (float)p.n_comb, rcp = p.rcp_ncomb;
         const int pb = r.p0 + (int)(tc::NT * k) - tc::HALO;       // fold position of window index 0
         const bool last = k + 1 == r.n_tiles;
         const uint32_t row_end = min(n_templ, (uint32_t)((job + 1) * C));
-        for (uint32_t row = job * C + (ewarp - job * 4 * NGRP); row < (LCS_TC_EXP == 3 ? 0u : row_end); row += 4 * NGRP) {
+        for (uint32_t row = job * C + wq; row < row_end; row += 4) {
           const uint32_t rf = row / 3, rt = row - 3 * rf;
           float* dst = p.single_planar + (((size_t)r.b * 3 + rt) * p.n_f_stride + f0 + rf) * tc::N_FOLD;
-          float* src = sWin + row * tc::WSTR;
+          float* src = sWin + row * tc::WROW;
 #pragma unroll
           for (int j = lane; j < tc::NT; j += 32) {
             const int pos = pb + j;
@@ -569,61 +436,26 @@ xcorr_fold_tc_kernel(const __grid_constant__ TcParams p) {
 #pragma unroll
           for (int j = tc::HALO + lane; j < tc::WSTR; j += 32) src[j] = 0.f;
         }
-        epi_bar(1 + job, SET_THREADS);
-        t_wout += TC_CLK() - c0;
+        named_bar(BAR_ID, 128);
       }
     }
-    if (LCS_TC_PROFILE && p.prof && lane == 0 && (ewarp == 0 || ewarp == 4 * NGRP)) {
-      const int o = ewarp == 0 ? 4 : 8;
-      p.prof[blockIdx.x * 12 + o + 0] = TC_CLK() - e_start;
-      p.prof[blockIdx.x * 12 + o + 1] = t_fwait;
-      p.prof[blockIdx.x * 12 + o + 2] = t_ld;
-      p.prof[blockIdx.x * 12 + o + 3] = t_wout;
-    }
   }
-
-  // ---- teardown ----
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(tc::TMEM_COLS));
-  }
+  // warps 1..3 of the producer warpgroup have no work
 }
 
 // =============================================================================================
 // Host side
 // =============================================================================================
+template <int C, int J>
+static cudaError_t tc_set_smem() {
+  return cudaFuncSetAttribute(xcorr_fold_tc_kernel<C, J>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcSmem<C, J>::TOTAL);
+}
 lcs_status tc_init(lcs_ctx* ctx) {
-  LCS_CUDA(ctx, cudaFuncSetAttribute(xcorr_fold_tc_kernel<16, 1, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcSmem<16, 1, 1>::TOTAL));
-  LCS_CUDA(ctx, cudaFuncSetAttribute(xcorr_fold_tc_kernel<16, 3, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcSmem<16, 3, 1>::TOTAL));
-  LCS_CUDA(ctx, cudaFuncSetAttribute(xcorr_fold_tc_kernel<16, 4, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcSmem<16, 4, 1>::TOTAL));
-  LCS_CUDA(ctx, cudaFuncSetAttribute(xcorr_fold_tc_kernel<16, 3, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcSmem<16, 3, 2>::TOTAL));
+  LCS_CUDA(ctx, (tc_set_smem<16, 1>()));
+  LCS_CUDA(ctx, (tc_set_smem<24, 2>()));
+  LCS_CUDA(ctx, (tc_set_smem<32, 2>()));
+  LCS_CUDA(ctx, (tc_set_smem<48, 2>()));
   return LCS_OK;
-}
-
-// LCS_TC_PROF=1 (library built with -DLCS_TC_PROFILE=1): per-CTA cycle counters of the pipeline stages, printed by tc_prof_dump().
-static long long* g_prof = nullptr;
-static long long* tc_prof_buffer() {
-#if LCS_TC_PROFILE
-  static const bool on = std::getenv("LCS_TC_PROF") != nullptr;
-  if (!on) return nullptr;
-  if (!g_prof) { cudaMalloc((void**)&g_prof, 148 * 12 * 8); cudaMemset(g_prof, 0, 148 * 12 * 8); }
-  return g_prof;
-#else
-  return nullptr;
-#endif
-}
-void tc_prof_dump() {
-  if (!g_prof) return;
-  std::vector<long long> h(148 * 12);
-  cudaDeviceSynchronize();
-  cudaMemcpy(h.data(), g_prof, h.size() * 8, cudaMemcpyDeviceToHost);
-  for (int b : {0, 1, 73, 147}) {
-    const long long* q = &h[b * 12];
-    std::printf("[tc stage waits] cta %3d: mma total %lld  wait_P %lld  wait_slot_empty %lld  template_reload %lld | epilogue set 0: total %lld  wait_slot_full %lld  "
-                "tmem_ld %lld  write_out %lld | set 1: total %lld  wait_slot_full %lld  tmem_ld %lld  write_out %lld\n",
-                b, q[0], q[1], q[2], q[3], q[4], q[5], q[6], q[7], q[8], q[9], q[10], q[11]);
-  }
 }
 
 int launch_xcorr_fold_tc(PlanSet& ps, const void* d_iq_cu8, uint32_t batch, const uint32_t* d_buf_plan, float* d_single_planar,
@@ -649,7 +481,6 @@ int launch_xcorr_fold_tc(PlanSet& ps, const void* d_iq_cu8, uint32_t batch, cons
   static const bool kExactRcp[25] = {false, true, true, true, true, true, false, true, true, true, false, true, false,
                                      true, false, true, true, true, false, true, false, true, false, true, false};
   q.rcp_ncomb = (g.n_comb_xc <= 24 && kExactRcp[g.n_comb_xc]) ? 1.0f / (float)g.n_comb_xc : 0.f;
-  q.prof = tc_prof_buffer();
   // tiles per unit: T tiles of a run give 256 T - 32 positions, and a unit is cut into at most ceil(tu / t_cta) + 1 runs
   const uint32_t n_units = batch * ps.n_pass, n_sm = (uint32_t)ps.ctx->n_sm;
   uint32_t tu = (tc::N_FOLD + tc::HALO + tc::NT - 1) / tc::NT, t_cta = 1;
@@ -663,10 +494,10 @@ int launch_xcorr_fold_tc(PlanSet& ps, const void* d_iq_cu8, uint32_t batch, cons
   q.n_tiles_total = n_units * tu;
   const uint32_t grid = (q.n_tiles_total + t_cta - 1) / t_cta;
   const tc::Layout& L = ps.lay;
-  if (L.ngrp == 1 && L.j == 1) xcorr_fold_tc_kernel<16, 1, 1><<<grid, L.threads(), TcSmem<16, 1, 1>::TOTAL, st>>>(q);
-  else if (L.ngrp == 3 && L.j == 1) xcorr_fold_tc_kernel<16, 3, 1><<<grid, L.threads(), TcSmem<16, 3, 1>::TOTAL, st>>>(q);
-  else if (L.ngrp == 4 && L.j == 1) xcorr_fold_tc_kernel<16, 4, 1><<<grid, L.threads(), TcSmem<16, 4, 1>::TOTAL, st>>>(q);
-  else xcorr_fold_tc_kernel<16, 3, 2><<<grid, L.threads(), TcSmem<16, 3, 2>::TOTAL, st>>>(q);
+  if (L.cj == 16) xcorr_fold_tc_kernel<16, 1><<<grid, L.threads(), TcSmem<16, 1>::TOTAL, st>>>(q);
+  else if (L.cj == 24) xcorr_fold_tc_kernel<24, 2><<<grid, L.threads(), TcSmem<24, 2>::TOTAL, st>>>(q);
+  else if (L.cj == 32) xcorr_fold_tc_kernel<32, 2><<<grid, L.threads(), TcSmem<32, 2>::TOTAL, st>>>(q);
+  else xcorr_fold_tc_kernel<48, 2><<<grid, L.threads(), TcSmem<48, 2>::TOTAL, st>>>(q);
   return 1;
 }
 

@@ -2,8 +2,8 @@
 
 This module is plumbing for tests/, bench.py and __graft_entry__.py: every call goes through the
 same `extern "C"` entry points a C++/IT++ host would bind (INTEGRATION.md).  There is no CPU
-fallback: importing works anywhere (the symbols are checked), but every compute call needs a
-B200 and raises LcsError otherwise.
+fallback: importing works anywhere (the symbols are checked), but every compute call needs an
+H100 and raises LcsError otherwise.
 """
 import ctypes as C
 import os
@@ -42,7 +42,7 @@ class Cell(C.Structure):
 
 
 def build(force=False):
-    """Compile the CUDA library in-tree (nvcc cross-compiles sm_100a without a GPU)."""
+    """Compile the CUDA library in-tree (nvcc cross-compiles sm_90a without a GPU)."""
     if force or not os.path.exists(LIB_PATH):
         subprocess.check_call(["make", "-C", HERE, "-s", "-j8"])
     else:

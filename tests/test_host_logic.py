@@ -15,7 +15,7 @@ def test_library_exports_every_declared_symbol(lcs):
     assert len(names) >= 25
     missing = [n for n in names if not hasattr(l, n)]
     assert not missing, missing
-    assert b"sm_100a" in l.lcs_version()
+    assert b"sm_90a" in l.lcs_version()
     assert C.sizeof(lcs.Cell) == 104
 
 
@@ -175,7 +175,7 @@ def test_framer_matches_producer_thread(lcs):
 
 
 def test_tc_integer_formulation_numpy(oracle):
-    """The arithmetic of the tcgen05 correlator (DESIGN.md 4.2) restated in numpy integers and checked against the oracle's
+    """The arithmetic of the tensor-core correlator (DESIGN.md 4.2) restated in numpy integers and checked against the oracle's
     `xc`: 24-bit fixed-point templates in three balanced base-256 digits, x' = byte-128, second byte stream (Q', ~I') for the
     imaginary part, additive corrections sum(a) / sum(a[even]), int32-safe partial sums, exact reconstruction."""
     from conftest import synth_cu8, cu8_to_c128
@@ -221,7 +221,7 @@ def test_tc_integer_formulation_numpy(oracle):
 
 
 def test_tc_run_decomposition_covers_every_position_once():
-    """The tcgen05 correlator distributes work in tile space (xcorr_tc.cu: launch_xcorr_fold_tc / TcRunIter): CTA i takes
+    """The tensor-core correlator distributes work in tile space (xcorr_tc.cu: launch_xcorr_fold_tc / TcRunIter): CTA i takes
     tiles [i*t_cta, (i+1)*t_cta) of the sequence [unit][tu]; a run of T tiles yields 256*T - 32 fold positions.  Restated
     here: for many (units, SMs) every position 0..9599 of every unit is produced by exactly one run, and no run needs more
     tiles than it was given."""
@@ -236,7 +236,7 @@ def test_tc_run_decomposition_covers_every_position_once():
                 return tu, t_cta
             tu += 1
 
-    for n_units, n_sm in [(1, 148), (2, 148), (3, 7), (8, 148), (32, 148), (64, 148), (128, 148), (384, 148), (768, 148), (5, 1), (37, 13)]:
+    for n_units, n_sm in [(1, 132), (2, 132), (3, 7), (8, 132), (32, 132), (64, 132), (128, 132), (384, 132), (768, 132), (5, 1), (37, 13)]:
         tu, t_cta = plan(n_units, n_sm)
         total = n_units * tu
         cover = np.zeros((n_units, NF), np.int32)
@@ -278,9 +278,10 @@ def test_three_instruction_division_matches_ieee_on_samples():
         assert np.array_equal(q2, (x / d).astype(np.float32)), n
 
 
-def test_library_contains_blackwell_native_instructions(lcs):
-    """The shipped liblcs_b200.so must carry the tcgen05 / TMEM / TMA code paths (SASS mnemonics of B200_PROFILING.md):
-    UTCIMMA = tcgen05.mma kind::i8, LDTM = tcgen05.ld, UTCBAR = tcgen05.commit, UBLKCP = cp.async.bulk (1-D TMA)."""
+def test_library_contains_hopper_native_instructions(lcs):
+    """The shipped liblcs_b200.so must carry the warpgroup-MMA / TMA / mbarrier code paths of the tensor-core correlator
+    (SASS mnemonics): IGMMA = wgmma.mma_async on s8 operands, WARPGROUP.ARRIVE = wgmma.fence, UBLKCP = cp.async.bulk
+    (1-D TMA), SYNCS.ARRIVE.TRANS64 = mbarrier arrive / expect_tx."""
     import os
     import shutil
     import subprocess
@@ -288,6 +289,6 @@ def test_library_contains_blackwell_native_instructions(lcs):
     if not os.path.exists(exe):
         pytest.skip("cuobjdump not available")
     sass = subprocess.run([exe, "-sass", lcs.LIB_PATH], capture_output=True, text=True, timeout=600).stdout
-    for mnemonic in ("UTCIMMA", "LDTM", "UTCBAR", "UBLKCP"):
+    for mnemonic in ("IGMMA.64x144x32.S8.S8", "WARPGROUP.ARRIVE", "UBLKCP", "SYNCS.ARRIVE.TRANS64"):
         assert sass.count(mnemonic) > 0, mnemonic
-    assert "sm_100a" in subprocess.run([exe, "-lelf", lcs.LIB_PATH], capture_output=True, text=True, timeout=600).stdout
+    assert "sm_90a" in subprocess.run([exe, "-lelf", lcs.LIB_PATH], capture_output=True, text=True, timeout=600).stdout

@@ -1,9 +1,9 @@
 #!/usr/bin/env python
 """Regenerate tests/golden/*.npz from the reference's own fixtures.
 
-Runs only where /root/reference exists (the build container).  The .it files are the
-reference's golden vectors (SURVEY.md section 4.1); they travel to the GPU box as
-compressed .npz so that no test needs /root/reference at run time.
+Needs a checkout of the reference project: `python tools/make_golden.py <reference dir>` (or
+LCS_REFERENCE=<dir>).  The .it files are the reference's golden vectors (SURVEY.md section 4.1);
+they are stored as compressed .npz so that no test needs the reference at run time.
 
   capbuf_0000.npz       real 8-bit capture (test/capbuf_0000.it) as raw cu8 + fc
   ref_xcorr_pss.npz     test/test_xcorr_pss.it  (Matlab-era semantics -> oracle legacy mode)
@@ -22,7 +22,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
 from itfile import read_it  # noqa: E402
 
-REF = os.environ.get("LCS_REFERENCE", "/root/reference")
+REF = sys.argv[1] if len(sys.argv) > 1 else os.environ.get("LCS_REFERENCE", "")
 OUT = os.path.join(HERE, "..", "tests", "golden")
 
 

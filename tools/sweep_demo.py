@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Multi-GPU frequency sweep demo (BASELINE config 4 in miniature): N ranks, channels round-robin, each rank
-runs its channels through lcs_sweep_search_cu8 on its own B200, NCCL all_gather of the cell records, dedup on rank 0.
+runs its channels through lcs_sweep_search_cu8 on its own GPU, NCCL all_gather of the cell records, dedup on rank 0.
 Channel 739.0 MHz carries the reference's real capture (tests/golden/capbuf_0000.npz); the others are synthetic noise.
   python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 tools/sweep_demo.py [n_channels]
 """
