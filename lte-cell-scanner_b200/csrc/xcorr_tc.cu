@@ -15,9 +15,10 @@
 //
 // Operand roles: 64 LAGS of a sub-tile are the M dimension (wgmma m64), the templates the N dimension.  A JOB is one
 // wgmma N dimension holding all three digit planes of C template columns (tc_layout.hpp); a pass has J jobs and the CTA
-// one consumer warpgroup per job.  A warpgroup issues the MMAs of its job, waits for them and runs the epilogue
-// (digit recombination, |xc|^2, fold) on the accumulator registers; while one warpgroup is in its epilogue the tensor
-// core works on the other one's MMAs.
+// one consumer warpgroup per job.  A warpgroup issues the MMAs of its job and runs the epilogue (digit recombination,
+// |xc|^2, fold) on the accumulator registers.  It keeps two accumulator sets and issues the MMAs of the next part before
+// the epilogue of the current one, so the tensor core works on its own MMAs as well as on the other warpgroup's while
+// it is in an epilogue; setmaxnreg moves the registers the second set needs from the producer warpgroup to the consumers.
 //
 // The Toeplitz (Hankel) A operand is never materialised per lag: an "expanded" tile P[u][r][16 B] = z[16u+2r ..+15]
 // is built once per 256-lag tile in shared memory (8x expansion of ~0.8 KB of raw bytes that a 1-D TMA bulk copy,
@@ -99,12 +100,18 @@ __device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes
 }
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void wgmma_wait0(int (&d)[N]) {
-  asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+// wait until at most PENDING committed groups are in flight; d holds the accumulators of a group that has retired then
+template <int PENDING, int N>
+__device__ __forceinline__ void wgmma_wait(int (&d)[N]) {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(PENDING) : "memory");
 #pragma unroll
   for (int i = 0; i < N; i++) asm volatile("" : "+r"(d[i])::"memory");   // the accumulators are read only after the wait
 }
+// hand registers from the producer warpgroup to the consumer warpgroups (executed by every warp of a warpgroup)
+template <uint32_t R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <uint32_t R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void named_bar(uint32_t id, uint32_t nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
 
@@ -184,6 +191,11 @@ __global__ void __launch_bounds__(128 + 128 * J, 1) xcorr_fold_tc_kernel(const _
   constexpr int NV = C / 2;               // results per thread and part: 2 rows x 2 columns per 8-column group
   static_assert(C % 8 == 0, "digit planes must start on an 8-column group of the accumulator fragment");
   static_assert(SM::TOTAL <= 232448, "shared memory");
+  // Registers per thread once the producer warpgroup has handed its surplus to the consumers (setmaxnreg).  The pool is
+  // what the launch gave the CTA: 65536 / 384 = 168 per thread for J = 2, so 128 * 40 + 256 * 232 = 168 * 384.  J = 1
+  // (256 threads) is launched at the consumers' 240 registers, so its increase is already covered by the launch.
+  constexpr uint32_t PROD_REGS = 40, CONS_REGS = J == 2 ? 232 : 240;
+  static_assert(128 * PROD_REGS + 128 * J * CONS_REGS <= 65536, "register file");
   extern __shared__ __align__(128) uint8_t smem[];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   uint8_t* sP = smem + SM::P;
@@ -207,7 +219,9 @@ __global__ void __launch_bounds__(128 + 128 * J, 1) xcorr_fold_tc_kernel(const _
   }
   __syncthreads();
 
-  if (warp == 0) {
+  if (warp < 4) {
+    setmaxnreg_dec<PROD_REGS>();
+    if (warp != 0) return;     // warps 1..3 of the producer warpgroup have no work
     // ================= producer: raw bytes by TMA one step ahead, expansion into the Hankel tile =================
     const uint64_t iq_lo = reinterpret_cast<uint64_t>(p.iq), iq_hi = iq_lo + p.iq_bytes;
     const uint32_t raw_addr = smem_u32(smem + SM::RAW);
@@ -278,8 +292,9 @@ __global__ void __launch_bounds__(128 + 128 * J, 1) xcorr_fold_tc_kernel(const _
       zo_cur = zo_nxt;
       if (nxt.ok) nxt.advance(p);
     }
-  } else if (warp >= 4) {
+  } else {
     // ================= consumers: one warpgroup per job - MMAs, then |xc|^2 and the fold on the accumulators =========
+    setmaxnreg_inc<CONS_REGS>();
     const int job = (warp >> 2) - 1;
     const int wq = warp & 3;                        // warp of the warpgroup: accumulator rows 16*wq .. +15
     const int wt = tid - 128 * (job + 1);           // thread of the warpgroup
@@ -292,16 +307,18 @@ __global__ void __launch_bounds__(128 + 128 * J, 1) xcorr_fold_tc_kernel(const _
     const float* cre = sCorr + job * C + cb;
     const float* cim = sCorr + NPAD + job * C + cb;
     uint32_t cur_pp = 0xffffffffu, bfull_par = 0, step = 0;
-    // One part (re or im) of one 64-lag sub-tile: 9 MMAs over K, then value = (a0*256 + a1)*256 + a2 + constant for the
-    // 2 rows x C/4 columns of this thread.  acc register 4*g + 2*h + e holds row (lane>>2) + 8h, column 8g + cb + e.
+    // One part (re or im) of one 64-lag sub-tile: 9 MMAs over K, committed as one group; its epilogue later computes
+    // value = (a0*256 + a1)*256 + a2 + constant for the 2 rows x C/4 columns of this thread.  acc register 4*g + 2*h + e
+    // holds row (lane>>2) + 8h, column 8g + cb + e.
     auto mma_part = [&](int (&acc)[NACC], uint32_t a_addr) {
       const uint64_t a_desc = make_desc(a_addr, 128, 128), b_desc = make_desc(sBj_addr, 128, tc::B_SBO);
       wgmma_fence();
 #pragma unroll
       for (int s = 0; s < tc::KSTEPS; s++) tc::wgmma_s8<NJOB>(acc, a_desc + (uint64_t)(s * 16), b_desc + (uint64_t)(s * 16), s > 0);
       wgmma_commit();
-      wgmma_wait0(acc);
     };
+    // Two accumulator sets: re parts accumulate in acc_re, im parts in acc_im.
+    int acc_re[NACC], acc_im[NACC];
     auto recombine = [&](const int (&acc)[NACC], float (&x)[NV], const float* kc) {
 #pragma unroll
       for (int g = 0; g < CG; g++) {
@@ -354,33 +371,43 @@ __global__ void __launch_bounds__(128 + 128 * J, 1) xcorr_fold_tc_kernel(const _
       for (uint32_t k = 0; k < r.n_tiles; k++) {
         for (uint32_t m = 0; m < p.n_comb; m++, step++) {
           const uint32_t stage = step & 1, use = step >> 1;
-          // -4 * (fold offset of the column - pass minimum), bytes, for the C/4 columns of this thread
-          int d[CG][2];
-#pragma unroll
-          for (int g = 0; g < CG; g++) {
-            const int2 d2 = *reinterpret_cast<const int2*>(sDoff + m * NPAD + job * C + cb + 8 * g);
-            d[g][0] = d2.x;
-            d[g][1] = d2.y;
-          }
           mbar_wait(BAR_PFULL + 8 * stage, use & 1);
           const uint32_t a_stage = sP_addr + stage * 2 * tc::P_BYTES;
-#pragma unroll 1
+          // Software pipeline over the 2 * NSUB parts of the half frame, (re, im) per sub-tile: the MMAs of the next part
+          // are issued before the epilogue of the current one, so the tensor core works on them meanwhile.  The sub-tile
+          // loop is unrolled: in-flight accumulators then never cross a branch or loop edge, where the compiler would copy
+          // them and thereby serialise the MMAs.  The last im epilogue of the half frame follows wait_group 0.
+          mma_part(acc_re, a_stage);
+#pragma unroll
           for (int q = 0; q < tc::NSUB; q++) {
-            int acc[NACC];
             float x[NV], rr[NV];
-            mma_part(acc, a_stage + q * (tc::NSUBL / 8) * 128);
-            recombine(acc, x, cre);
+            mma_part(acc_im, a_stage + tc::P_BYTES + q * (tc::NSUBL / 8) * 128);
+            wgmma_wait<1>(acc_re);                  // re of sub-tile q retired, im in flight
+            recombine(acc_re, x, cre);
 #pragma unroll
             for (int v = 0; v < NV; v++) rr[v] = __fmul_rn(x[v], x[v]);
-            mma_part(acc, a_stage + tc::P_BYTES + q * (tc::NSUBL / 8) * 128);
-            if (q == tc::NSUB - 1 && lane == 0) mbar_arrive(BAR_PEMPTY + 8 * stage);     // P stage free again
-            recombine(acc, x, cim);
+            if (q + 1 < tc::NSUB) {
+              mma_part(acc_re, a_stage + (q + 1) * (tc::NSUBL / 8) * 128);
+              wgmma_wait<1>(acc_im);
+            } else {
+              wgmma_wait<0>(acc_im);
+              if (lane == 0) mbar_arrive(BAR_PEMPTY + 8 * stage);     // every MMA on the P stage retired
+            }
+            recombine(acc_im, x, cim);
             // |xc|^2 = re^2 + im^2 (searcher.cpp:300), in the integer scale of the templates; the power-of-two scale
             // factor is applied when the tile is written out
 #pragma unroll
             for (int v = 0; v < NV; v++) rr[v] = __fmaf_rn(x[v], x[v], rr[v]);
             // fold into the sliding window: lag q*64 + row of the tile lands at window index lag + HALO - dsh; all loads
-            // of the read-modify-write first, then add + store
+            // of the read-modify-write first, then add + store.  d = -4 * (fold offset of the column - pass minimum),
+            // bytes, for the C/4 columns of this thread, read per sub-tile to keep it out of the registers the MMAs overlap.
+            int d[CG][2];
+#pragma unroll
+            for (int g = 0; g < CG; g++) {
+              const int2 d2 = *reinterpret_cast<const int2*>(sDoff + m * NPAD + job * C + cb + 8 * g);
+              d[g][0] = d2.x;
+              d[g][1] = d2.y;
+            }
 #pragma unroll
             for (int g = 0; g < CG; g++)
 #pragma unroll
@@ -440,7 +467,6 @@ __global__ void __launch_bounds__(128 + 128 * J, 1) xcorr_fold_tc_kernel(const _
       }
     }
   }
-  // warps 1..3 of the producer warpgroup have no work
 }
 
 // =============================================================================================
