@@ -253,6 +253,57 @@ lcs_status lcs_tracker_search_cu8(lcs_ctx* ctx, const uint8_t* capbuf_cu8, uint3
                                   const int32_t* tracked_n_id_cell, uint32_t n_tracked, lcs_cell* cells,
                                   double* frame_timing, uint32_t max_cells, uint32_t* n_cells);
 
+/* ---- cell tracking: the per-cell tracker loop of LTE-Tracker for many cells and channels ------------------------- */
+/* A track handle follows every detected cell of n_ch channels over time: the per-cell slicer of
+ * src/producer_thread.cpp:163-250 and the tracker loop of src/tracker_thread.cpp:856-1067 (get_fd, CRS channel
+ * estimation and filtering, FOE / TOE, interpolation, CRS and PSS/SSS measurements, MIB decoding, dropping a cell after
+ * CELL_DROP_THRESHOLD = 400 failures).  The schedule is deterministic (DESIGN.md section 4.5): each channel's stream is
+ * cut into blocks of LCS_TRACK_BLOCK samples counted from its start; a block is processed once it is complete, in one
+ * launch per push for every channel.  The channel's frequency offset (moved by every cell's FOE) and each cell's frame
+ * timing (moved by its TOE) are sampled at each block start.  Cells added between pushes take part from the first block
+ * not yet processed, starting at slot 0, symbol 0. */
+#define LCS_TRACK_BLOCK 10000
+
+typedef struct lcs_track lcs_track;
+
+/* One tracked cell as lcs_track_read reports it (the measurements of the reference's tracked_cell_t).  Measurements
+ * start as NaN, channel estimates as 0. */
+typedef struct lcs_track_cell {
+  int32_t n_id_cell, n_ports, cp_type;
+  int32_t dropped;               /* 1: dropped (MIB failures reached 400); reported once, then its slot is freed */
+  int64_t drop_sample;           /* stream sample one past the symbol whose MIB attempt dropped the cell (-1: live) */
+  int64_t n_symbols;             /* OFDM symbols sliced and processed */
+  int64_t last_slice_start;      /* stream sample of the first sample of the latest symbol (-1: none yet) */
+  int64_t mib_attempts, mib_successes;
+  double frame_timing;           /* LTE samples modulo 19200, in the tracker's time stamps */
+  double mib_decode_failures;
+  double crs_tp[4], crs_sp_raw[4], crs_np[4];
+  double crs_tp_av[4], crs_sp_raw_av[4], crs_np_av[4];
+  double sync_tp, sync_sp, sync_np, sync_np_blank;
+  double sync_tp_av, sync_sp_av, sync_np_av, sync_np_blank_av;
+  double sync_ce[72][2];         /* c128, latest PSS/SSS channel estimate */
+  double ce[4][72][2];           /* c128, latest interpolated CRS channel estimate per port */
+} lcs_track_cell;
+
+/* fc_requested[n_ch]; fc_programmed[n_ch] or NULL (= fc_requested); frequency_offset[n_ch] the initial offsets (the
+ * kalibrate result); max_cells per channel, 1 to 32 (one slicing thread per cell slot in the channel's CTA). */
+lcs_status lcs_track_create(lcs_ctx* ctx, uint32_t n_ch, const double* fc_requested, const double* fc_programmed,
+                            double fs_programmed, const double* frequency_offset, uint32_t max_cells, lcs_track** out);
+void lcs_track_destroy(lcs_track* track);
+/* Start tracking a cell found by lcs_tracker_search_cu8 on channel ch: cell->n_id_1/n_id_2, cp_type, n_ports (1, 2 or
+ * 4), n_rb_dl, phich_duration and phich_resource are used; frame_timing in [0, 19200) is the handed-over timing. */
+lcs_status lcs_track_add_cell(lcs_track* track, uint32_t ch, const lcs_cell* cell, double frame_timing);
+/* Feed n samples of every channel: iq_host is cu8 [n_ch][n][2].  All complete blocks run in one launch. */
+lcs_status lcs_track_push_cu8(lcs_track* track, const uint8_t* iq_host, uint32_t n);
+lcs_status lcs_track_frequency_offset(const lcs_track* track, double* frequency_offset /*[n_ch]*/);
+/* The cells of channel ch in the order they were added (at most max; *n = number written). */
+lcs_status lcs_track_read(lcs_track* track, uint32_t ch, lcs_track_cell* out, uint32_t max, uint32_t* n);
+/* Time stamp of the last processed sample of channel ch (the lcs_framer_sample_time recurrence). */
+lcs_status lcs_track_sample_time(const lcs_track* track, uint32_t ch, double* sample_time);
+/* Summed device time of the tracker kernel (CUDA events around each launch, ms) and the number of launches since the
+ * last read; resets both. */
+lcs_status lcs_track_timing_read(lcs_track* track, double* kernel_ms, uint64_t* launches);
+
 #ifdef __cplusplus
 }
 #endif

@@ -324,22 +324,6 @@ namespace {
 const int kGen[3] = {0133, 0171, 0165};
 inline int par(int x) { return __builtin_parity((unsigned)x); }
 
-// position of every rate-matched bit e[k] in the 3 x 40 coded block (36.212 5.1.4.2; lte_lib.cpp:409-463)
-void pbch_ratematch_positions(int n_e, std::vector<int>& pos) {
-  static const int perm[32] = {1,17,9,25,5,21,13,29,3,19,11,27,7,23,15,31,0,16,8,24,4,20,12,28,2,18,10,26,6,22,14,30};
-  const int D = 40, C = 32, R = 2, K = R * C, ND = K - D;
-  std::vector<int> w;  // circular buffer of d positions, -1 = <NULL>
-  for (int s = 0; s < 3; s++)
-    for (int col = 0; col < C; col++)
-      for (int r = 0; r < R; r++) {
-        const int y = r * C + perm[col];
-        w.push_back(y < ND ? -1 : s * D + (y - ND));
-      }
-  pos.clear();
-  for (size_t j = 0; (int)pos.size() < n_e; j = (j + 1) % w.size())
-    if (w[j] >= 0) pos.push_back(w[j]);
-}
-
 // exact maximum-likelihood tail-biting Viterbi: best path over all 64 (start==end) states.
 // llr > 0 means bit 0 (lte_lib.cpp:465-468, 535-537).
 // The 64 constrained decodes (one per start state) are independent: their path metrics are kept side by side,
@@ -412,6 +396,23 @@ void crc16(const uint8_t* a, int n, uint8_t* p) {  // x^16+x^12+x^5+1, zero init
   for (int i = 0; i < 16; i++) p[i] = (reg >> (15 - i)) & 1u;
 }
 }  // namespace
+
+// position of every rate-matched bit e[k] in the 3 x 40 coded block (36.212 5.1.4.2; lte_lib.cpp:409-463)
+void pbch_ratematch_positions(int n_e, std::vector<int>& pos) {
+  static const int perm[32] = {1,17,9,25,5,21,13,29,3,19,11,27,7,23,15,31,0,16,8,24,4,20,12,28,2,18,10,26,6,22,14,30};
+  const int D = 40, C = 32, R = 2, K = R * C, ND = K - D;
+  std::vector<int> w;  // circular buffer of d positions, -1 = <NULL>
+  for (int s = 0; s < 3; s++)
+    for (int col = 0; col < C; col++)
+      for (int r = 0; r < R; r++) {
+        const int y = r * C + perm[col];
+        w.push_back(y < ND ? -1 : s * D + (y - ND));
+      }
+  pos.clear();
+  for (size_t j = 0; (int)pos.size() < n_e; j = (j + 1) % w.size())
+    if (w[j] >= 0) pos.push_back(w[j]);
+}
+
 
 // ---------------------------------------------------------------------------------------------
 // decode_mib  (src/searcher.cpp:1526-1692).  tfg row-major [n_ofdm][72].

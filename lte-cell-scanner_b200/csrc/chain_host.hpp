@@ -25,5 +25,7 @@ void chan_est(const RsDl& rs, const cd* tfg, int n_ofdm, int port, std::vector<c
 void decode_mib(const lcs_cell& cell, const cd* tfg, int n_ofdm, const RsDl& rs, lcs_cell& out);
 void dedup(const lcs_cell* cells, uint32_t n, std::vector<lcs_cell>& fin);
 std::vector<double> f_search_set_for(double freq_start, double ppm);
+// position in the 3 x 40 coded block of every rate-matched PBCH bit e[k] (lte_lib.cpp:409-463)
+void pbch_ratematch_positions(int n_e, std::vector<int>& pos);
 
 }  // namespace lcs

@@ -82,6 +82,14 @@ def lib():
         _lib.lcs_framer_request.restype = None
         _lib.lcs_framer_sample_time.argtypes = [C.c_void_p]
         _lib.lcs_framer_sample_time.restype = C.c_double
+        _lib.lcs_track_destroy.argtypes = [C.c_void_p]
+        _lib.lcs_track_destroy.restype = None
+        _lib.lcs_track_add_cell.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_double]
+        _lib.lcs_track_push_cu8.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
+        _lib.lcs_track_frequency_offset.argtypes = [C.c_void_p, C.c_void_p]
+        _lib.lcs_track_read.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p]
+        _lib.lcs_track_sample_time.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p]
+        _lib.lcs_track_timing_read.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
     return _lib
 
 
@@ -468,6 +476,99 @@ class Framer:
 
     def __del__(self):
         self.close()
+
+
+class TrackCell(C.Structure):
+    """lcs_track_cell: one tracked cell as lcs_track_read reports it."""
+    _fields_ = [
+        ("n_id_cell", C.c_int32), ("n_ports", C.c_int32), ("cp_type", C.c_int32), ("dropped", C.c_int32),
+        ("drop_sample", C.c_int64), ("n_symbols", C.c_int64), ("last_slice_start", C.c_int64),
+        ("mib_attempts", C.c_int64), ("mib_successes", C.c_int64),
+        ("frame_timing", C.c_double), ("mib_decode_failures", C.c_double),
+        ("crs_tp", C.c_double * 4), ("crs_sp_raw", C.c_double * 4), ("crs_np", C.c_double * 4),
+        ("crs_tp_av", C.c_double * 4), ("crs_sp_raw_av", C.c_double * 4), ("crs_np_av", C.c_double * 4),
+        ("sync_tp", C.c_double), ("sync_sp", C.c_double), ("sync_np", C.c_double), ("sync_np_blank", C.c_double),
+        ("sync_tp_av", C.c_double), ("sync_sp_av", C.c_double), ("sync_np_av", C.c_double),
+        ("sync_np_blank_av", C.c_double),
+        ("sync_ce", C.c_double * 144), ("ce", C.c_double * (4 * 144)),
+    ]
+
+    def as_dict(self):
+        """Plain Python / numpy values; sync_ce is complex [72], ce complex [4][72]."""
+        d = {}
+        for k, _ in self._fields_:
+            v = getattr(self, k)
+            if k == "sync_ce":
+                v = np.ctypeslib.as_array(v).copy().view(np.complex128)
+            elif k == "ce":
+                v = np.ctypeslib.as_array(v).copy().view(np.complex128).reshape(4, 72)
+            elif not isinstance(v, (int, float)):
+                v = np.ctypeslib.as_array(v).copy()
+            d[k] = v
+        return d
+
+
+TRACK_BLOCK = 10000
+
+
+class Tracker:
+    """lcs_track: the per-cell tracker loop of LTE-Tracker for every cell of n_ch channels, one launch per push."""
+
+    def __init__(self, ctx, fc_requested, frequency_offset, fs_programmed=1.92e6, fc_programmed=None, max_cells=8):
+        self.ctx = ctx
+        fc = np.ascontiguousarray(np.atleast_1d(fc_requested), np.float64)
+        self.n_ch = fc.size
+        fcp = None if fc_programmed is None else np.ascontiguousarray(np.atleast_1d(fc_programmed), np.float64)
+        fo = np.ascontiguousarray(np.broadcast_to(np.asarray(frequency_offset, np.float64), (self.n_ch,)))
+        self.max_cells = int(max_cells)
+        self._h = C.c_void_p()
+        _chk(lib().lcs_track_create(ctx._h, C.c_uint32(self.n_ch), _p(fc), _p(fcp), C.c_double(fs_programmed), _p(fo),
+                                    C.c_uint32(self.max_cells), C.byref(self._h)), ctx._h)
+
+    def add_cell(self, ch, cell, frame_timing):
+        _chk(lib().lcs_track_add_cell(self._h, C.c_uint32(ch), C.byref(cell), C.c_double(frame_timing)), self.ctx._h)
+
+    def push_cu8(self, iq_cu8):
+        """iq_cu8: uint8 [n_ch][n][2] (or [n][2] for one channel)."""
+        iq = np.ascontiguousarray(iq_cu8, np.uint8)
+        n = iq.shape[-2]
+        if iq.size != self.n_ch * n * 2:
+            raise ValueError("push_cu8: expected [n_ch][n][2] samples")
+        _chk(lib().lcs_track_push_cu8(self._h, _p(iq), C.c_uint32(n)), self.ctx._h)
+
+    def frequency_offset(self):
+        fo = np.zeros(self.n_ch)
+        _chk(lib().lcs_track_frequency_offset(self._h, _p(fo)), self.ctx._h)
+        return fo
+
+    def sample_time(self, ch=0):
+        v = C.c_double(0)
+        _chk(lib().lcs_track_sample_time(self._h, C.c_uint32(ch), C.byref(v)), self.ctx._h)
+        return v.value
+
+    def timing_read(self):
+        """(kernel ms, launches) since the last read, from CUDA events around each launch."""
+        ms = C.c_double(0); n = C.c_uint64(0)
+        _chk(lib().lcs_track_timing_read(self._h, C.byref(ms), C.byref(n)), self.ctx._h)
+        return ms.value, n.value
+
+    def read(self, ch=0):
+        """The channel's cells in the order added, as dicts; a dropped cell is reported once."""
+        out = (TrackCell * self.max_cells)()
+        n = C.c_uint32(0)
+        _chk(lib().lcs_track_read(self._h, C.c_uint32(ch), out, C.c_uint32(self.max_cells), C.byref(n)), self.ctx._h)
+        return [out[i].as_dict() for i in range(n.value)]
+
+    def close(self):
+        if self._h:
+            lib().lcs_track_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
 
 
 def declared_symbols():
