@@ -304,6 +304,53 @@ lcs_status lcs_track_sample_time(const lcs_track* track, uint32_t ch, double* sa
  * last read; resets both. */
 lcs_status lcs_track_timing_read(lcs_track* track, double* kernel_ms, uint64_t* launches);
 
+/* ---- wideband channelizer: many LTE raster channels out of one wideband ci16 recording (DESIGN.md section 4.6) ------ */
+/* One digital down-converter per channel, all channels in one launch per push; the output of channel c is the 1.92 Msps
+ * cu8 stream a dongle tuned to fc_ch[c] would deliver (fc_requested = fc_programmed = fc_ch[c], fs_programmed =
+ * 1.92e6 * correction when the recording's LO and sample clock share one crystal).
+ *   fs_in = D * 1 920 000 Hz, D integer in [2, 64]; channel offset delta_c = fc_ch[c] - fc_in an integer number of Hz
+ *   (within 1e-6) with |delta_c| <= fs_in/2 - 960 kHz; 1 <= n_ch <= 1024; anything else is LCS_ERR_ARG.
+ *   input  x[m] = (I[m] + jQ[m]) / 32768, m counted from the start of the stream (interleaved little-endian int16 I/Q).
+ *   mixer  p_c[m] = (m * delta_c) mod fs_in in exact 64-bit integers; x~_c[m] = x[m] exp(-j2pi p_c[m]/fs_in).
+ *   filter h: real, symmetric, odd length L = 2M+1, Kaiser-windowed sinc (cutoff 0.96 MHz), designed in double and kept
+ *          as float; passband deviation <= 0.01 dB for |f| <= 0.70 MHz, stopband >= 70 dB for |f| >= 1.22 MHz, the
+ *          shortest such odd L (37, 73, 133, 263, 523, 1045 taps at D = 2, 4, 8, 16, 32, 64: about 16D+5).  The passband holds the central 72 subcarriers (+-0.54 MHz) plus a carrier
+ *          offset of up to +-160 kHz.
+ *   output y_c[n] = sum_{k=-M..M} h[k+M] x~_c[nD-k] (x~ = 0 before the stream starts).  Output n is emitted once input
+ *          sample nD+M has been pushed: after N input samples there are max(0, floor((N-1-M)/D)+1) outputs; output n
+ *          belongs to input instant nD.  Any sequence of pushes gives bitwise the bytes of one push of the whole stream.
+ *   bytes  v = 127 + 128 g_c Re(y) (and Im), rounded to nearest (ties to even), clamped to [0, 255] - the (u8-127)/128
+ *          convention of capbuf.cpp:172-175; the clamped components are counted per channel.
+ *   gain   g_c from lcs_chan_create (NULL: 1.0), or lcs_chan_auto_gain_ci16: 0.25 / sqrt(mean |y_c[n]|^2) over the outputs
+ *          a FRESH channelizer would produce from the given samples (1.0 when that is 0); it leaves the stream alone. */
+typedef struct lcs_chan lcs_chan;
+/* host only, no device needed: the prototype filter h for fs_in; taps may be NULL to query *n_taps (on input, the
+ * capacity of taps) */
+lcs_status lcs_chan_design_taps(double fs_in, float* taps, uint32_t* n_taps);
+lcs_status lcs_chan_create(lcs_ctx* ctx, double fs_in, double fc_in, uint32_t n_ch, const double* fc_ch,
+                           const float* gain /*[n_ch] or NULL*/, lcs_chan** out);
+void lcs_chan_destroy(lcs_chan* chan);
+/* iq_host is ci16 [n][2] */
+lcs_status lcs_chan_auto_gain_ci16(lcs_chan* chan, const int16_t* iq_host, uint32_t n);
+lcs_status lcs_chan_gain(const lcs_chan* chan, float* gain /*[n_ch]*/);
+/* the number of outputs per channel the next push of n_in samples yields */
+lcs_status lcs_chan_n_out(const lcs_chan* chan, uint64_t n_in, uint32_t* n_out);
+/* Push n_in samples (ci16 [n_in][2], host).  out: cu8 [n_ch][out_capacity][2] in host memory, or device memory when
+ * out_on_device; *n_out outputs per channel are written from column 0.  n_clipped[n_ch] (may be NULL): components
+ * clamped in this push.  out_capacity < the outputs of this push -> LCS_ERR_ARG and nothing is consumed.  Large pushes
+ * run in chunks that bound the device scratch. */
+lcs_status lcs_chan_push_ci16(lcs_chan* chan, const int16_t* iq_host, uint32_t n_in, uint8_t* out, uint32_t out_capacity,
+                              int out_on_device, uint32_t* n_out, uint64_t* n_clipped);
+/* Summed device time of the channelizer kernel (CUDA events around each launch, ms) and the number of launches since
+ * the last read; resets both. */
+lcs_status lcs_chan_timing_read(lcs_chan* chan, double* kernel_ms, uint64_t* launches);
+
+/* lcs_sweep_search_cu8 on capture buffers already in device memory (e.g. a channelizer's output): d_iq is cu8
+ * [n_ch][n_cap][2], 16-byte aligned, and is read in place (no copy).  Same arguments and results otherwise. */
+lcs_status lcs_sweep_search_cu8_device(lcs_sweep* sweep, const uint8_t* d_iq, uint32_t n_ch, const double* fc_requested,
+                                       const double* fc_programmed, double fs_programmed, const double* f_search_set,
+                                       uint32_t n_f, lcs_cell* cells, uint32_t max_cells, uint32_t* n_cells);
+
 #ifdef __cplusplus
 }
 #endif

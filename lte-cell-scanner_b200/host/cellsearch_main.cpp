@@ -38,6 +38,10 @@ static void print_usage() {
   cout << "  -d --data-dir dir              directory of the capbuf_XXXX.it files" << endl;
   cout << "     --raw                       with -l: read capbuf_XXXX.bin raw rtl_sdr byte dumps instead" << endl;
   cout << "     --sweep                     with -l --raw: all centre frequencies in one batched call (lcs_sweep_search_cu8)" << endl;
+  cout << "     --wideband FILE             search every 100 kHz raster point in [fs, fe] in one wideband recording: raw" << endl;
+  cout << "                                 little-endian int16 I/Q (ci16, no header), channelized on the GPU" << endl;
+  cout << "     --fs-in FS                  with --wideband: the recording's sample rate, D * 1.92 MHz with D in [2, 64]" << endl;
+  cout << "     --fc-in FC                  with --wideband: the recording's centre frequency" << endl;
   cout << "  -r --record / -i --device-index need a live rtl-sdr dongle: not supported by this build" << endl;
 }
 
@@ -55,12 +59,14 @@ static string freq_formatter(const double& freq) {   // CellSearch.cpp:322-341
 int main(int argc, char* const argv[]) {
   double freq_start = -1, freq_end = -1, ppm = 120, correction = 1;
   bool save_cap = false, use_recorded_data = false, raw = false, batched = false;
-  string data_dir = ".";
+  string data_dir = ".", wideband;
+  double fs_in = -1, fc_in = -1;
   static struct option long_options[] = {
       {"help", no_argument, 0, 'h'},          {"verbose", no_argument, 0, 'v'},       {"brief", no_argument, 0, 'b'},
       {"freq-start", required_argument, 0, 's'}, {"freq-end", required_argument, 0, 'e'}, {"ppm", required_argument, 0, 'p'},
       {"correction", required_argument, 0, 'c'}, {"record", no_argument, 0, 'r'},        {"load", no_argument, 0, 'l'},
       {"data-dir", required_argument, 0, 'd'},   {"device-index", required_argument, 0, 'i'}, {"raw", no_argument, 0, 'R'}, {"sweep", no_argument, 0, 'W'},
+      {"wideband", required_argument, 0, 'B'},   {"fs-in", required_argument, 0, 'F'},   {"fc-in", required_argument, 0, 'C'},
       {0, 0, 0, 0}};
   for (;;) {
     int idx = 0;
@@ -80,6 +86,9 @@ int main(int argc, char* const argv[]) {
       case 'd': data_dir = optarg; break;
       case 'R': raw = true; break;
       case 'W': batched = true; break;
+      case 'B': wideband = optarg; break;
+      case 'F': fs_in = strtod(optarg, &endp); if (optarg == endp || *endp) { cerr << "Error: could not parse --fs-in" << endl; return -1; } break;
+      case 'C': fc_in = strtod(optarg, &endp); if (optarg == endp || *endp) { cerr << "Error: could not parse --fc-in" << endl; return -1; } break;
       case 'i': break;
       default: return -1;
     }
@@ -100,9 +109,43 @@ int main(int argc, char* const argv[]) {
   if (ppm < 0) { cerr << "Error: ppm value must be positive" << endl; return -1; }
   if (ppm > 200) cout << "Warning: ppm value appears to be set unreasonably high" << endl;
   if (abs(correction - 1) > 1000e-6) cout << "Warning: crystal correction factor appears to be unreasonable" << endl;
-  if (save_cap || !use_recorded_data) {
-    cerr << "Error: live capture / recording needs an rtl-sdr dongle, which this build does not support; use -l" << endl;
+  const bool wide = !wideband.empty();
+  if (save_cap || (!use_recorded_data && !wide)) {
+    cerr << "Error: live capture / recording needs an rtl-sdr dongle, which this build does not support; use -l or --wideband" << endl;
     return -1;
+  }
+  // wideband recording: every argument and the file length are checked before any device work
+  vector<int16_t> wide_iq;
+  uint32_t wide_n = 0;
+  if (wide) {
+    if (use_recorded_data || batched) { cerr << "Error: --wideband cannot be combined with -l or --sweep" << endl; return -1; }
+    if (fc_in <= 0) { cerr << "Error: --wideband needs --fc-in" << endl; return -1; }
+    uint32_t n_taps = 0;
+    if (lcs_chan_design_taps(fs_in, nullptr, &n_taps) != LCS_OK) {
+      cerr << "Error: --fs-in must be D * 1.92 MHz with an integer D in [2, 64]" << endl;
+      return -1;
+    }
+    const int D = (int)std::lround(fs_in / 1.92e6), M = (int)(n_taps - 1) / 2;
+    const int n_fc = (int)floor((freq_end - freq_start) / 100e3) + 1;                     // the raster of the search loop
+    for (int fci = 0; fci < n_fc; fci++) {
+      const double fc = freq_start + fci * 100e3, d = fc - fc_in;
+      if (std::fabs(d - std::round(d)) > 1e-6 || std::fabs(std::round(d)) > fs_in / 2 - 960e3) {
+        cerr << "Error: raster point " << setprecision(10) << fc / 1e6
+             << " MHz lies outside the input band of the recording (its 1.92 MHz channel must fit in fc-in +- fs-in/2)" << endl;
+        return -1;
+      }
+    }
+    wide_n = 153599u * D + M + 1;   // 153 600 outputs per channel
+    // only the prefix the search uses is read (a recording may be far longer)
+    FILE* f = std::fopen(wideband.c_str(), "rb");
+    if (!f) { cerr << "Error: cannot read " << wideband << endl; return -1; }
+    wide_iq.resize((size_t)wide_n * 2);
+    const size_t got = std::fread(wide_iq.data(), 4, wide_n, f);
+    std::fclose(f);
+    if (got < wide_n) {
+      cerr << "Error: " << wideband << " holds " << got << " ci16 samples; 153600 outputs per channel need " << wide_n << endl;
+      return -1;
+    }
   }
   if (verbosity >= 1) {
     cout << "LTE CellSearch (GPU drop-in, " << lcs_version() << ") beginning" << endl;
@@ -112,7 +155,11 @@ int main(int argc, char* const argv[]) {
     stringstream temp;
     temp << setprecision(20) << correction;
     cout << "  correction: " << temp.str() << endl;
-    cout << "  Captured data will be read from capbufXXXX." << (raw ? "bin" : "it") << " files" << endl;
+    if (wide)
+      cout << "  Captured data will be read from the wideband recording " << wideband << " (" << fs_in / 1e6 << " Msps at "
+           << fc_in / 1e6 << " MHz)" << endl;
+    else
+      cout << "  Captured data will be read from capbufXXXX." << (raw ? "bin" : "it") << " files" << endl;
   }
 
   try {
@@ -123,6 +170,13 @@ int main(int argc, char* const argv[]) {
     const int n_fc = (int)floor((freq_end - freq_start) / 100e3) + 1;                   // :465
     vector<list<Cell> > detected_cells(n_fc);
     xcorr_pss_skip_debug_outputs(true);
+    if (wide) {
+      // every raster point channelized out of the one recording on the device, then the batched search in place
+      vector<double> fcs;
+      for (int fci = 0; fci < n_fc; fci++) fcs.push_back(freq_start + fci * 100e3);
+      if (verbosity >= 1) cout << "Channelizing and examining " << n_fc << " center frequencies of one wideband recording ..." << endl;
+      wideband_search_ci16(wide_iq.data(), wide_n, fs_in, fc_in, fcs, f_search_set, fs_programmed, detected_cells);
+    }
     if (batched) {
       // every centre frequency of the sweep in one call: the raw byte dumps are concatenated and handed to the batched
       // search (same per-channel results as the loop below, CellSearch.cpp:465-558)
@@ -142,6 +196,8 @@ int main(int argc, char* const argv[]) {
       }
       if (verbosity >= 1) cout << "Examining " << n_fc << " center frequencies in one batched sweep ..." << endl;
       sweep_search_cu8(all, n_cap, fcs, f_search_set, fs_programmed, detected_cells);
+    }
+    if (batched || wide) {
       if (verbosity >= 1)
         for (int fci = 0; fci < n_fc; fci++)
           for (list<Cell>::iterator it = detected_cells[fci].begin(); it != detected_cells[fci].end(); ++it) {
@@ -151,7 +207,7 @@ int main(int argc, char* const argv[]) {
             cout << "    residual frequency offset: " << (*it).freq_superfine << " Hz" << endl;
           }
     }
-    for (int fci = 0; fci < (batched ? 0 : n_fc); fci++) {
+    for (int fci = 0; fci < (batched || wide ? 0 : n_fc); fci++) {
       const double fc_requested = freq_start + fci * 100e3;
       if (verbosity >= 1) cout << "Examining center frequency " << fc_requested / 1e6 << " MHz ..." << endl;
       cvec capbuf;

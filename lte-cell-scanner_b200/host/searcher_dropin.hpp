@@ -96,4 +96,8 @@ void xcorr_pss_skip_debug_outputs(bool skip);
 // lcs_sweep_search_cu8 (one plan per centre frequency, one correlator launch per 64 channels).  detected_cells as in :469.
 void sweep_search_cu8(const std::vector<unsigned char>& iq, uint32_t n_cap, const std::vector<double>& fc_requested,
                       const itpp::vec& f_search_set, const double& fs_programmed, std::vector<std::list<Cell> >& detected_cells);
+// The same sweep fed from one wideband ci16 recording (iq [n][2] at fs_in, centred on fc_in): lcs_chan auto gain, every
+// channel channelized into device memory (153 600 samples each), then lcs_sweep_search_cu8_device.
+void wideband_search_ci16(const int16_t* iq, uint32_t n, double fs_in, double fc_in, const std::vector<double>& fc_requested,
+                          const itpp::vec& f_search_set, const double& fs_programmed, std::vector<std::list<Cell> >& detected_cells);
    // skip the 136 MB `xc`/`sp`/`xc_incoherent` debug outputs (CLI does)

@@ -90,6 +90,16 @@ def lib():
         _lib.lcs_track_read.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p]
         _lib.lcs_track_sample_time.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p]
         _lib.lcs_track_timing_read.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+        _lib.lcs_chan_design_taps.argtypes = [C.c_double, C.c_void_p, C.c_void_p]
+        _lib.lcs_chan_create.argtypes = [C.c_void_p, C.c_double, C.c_double, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]
+        _lib.lcs_chan_destroy.argtypes = [C.c_void_p]
+        _lib.lcs_chan_destroy.restype = None
+        _lib.lcs_chan_auto_gain_ci16.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
+        _lib.lcs_chan_gain.argtypes = [C.c_void_p, C.c_void_p]
+        _lib.lcs_chan_n_out.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p]
+        _lib.lcs_chan_push_ci16.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_int, C.c_void_p,
+                                            C.c_void_p]
+        _lib.lcs_chan_timing_read.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
     return _lib
 
 
@@ -415,6 +425,29 @@ class Sweep:
                                         _p(f), C.c_uint32(f.size), cells, C.c_uint32(max_cells), n), self.ctx._h)
         return [[_copy(cells[b * max_cells + k]) for k in range(min(n[b], max_cells))] for b in range(n_ch)]
 
+    def search_cu8_device(self, iq, fc_requested, f_set, fs_programmed=1.92e6, fc_programmed=None, max_cells=8, n_ch=None):
+        """search_cu8 on capture buffers in device memory, read in place: iq is a uint8 CUDA tensor [n_ch][n_cap][2]
+        (16-byte aligned, contiguous) or a raw device pointer (int) with n_ch given.  The caller's writes to it must be
+        complete; for a tensor, its stream is synchronised first."""
+        fc = np.ascontiguousarray(fc_requested, np.float64)
+        n_ch = fc.size
+        fcp = None if fc_programmed is None else np.ascontiguousarray(fc_programmed, np.float64)
+        f = np.ascontiguousarray(f_set, np.float64)
+        if isinstance(iq, int):
+            ptr = iq
+        else:
+            if not (iq.is_cuda and iq.is_contiguous() and iq.numel() >= n_ch * self.n_cap * 2):
+                raise ValueError("search_cu8_device: expected a contiguous uint8 CUDA tensor [n_ch][n_cap][2]")
+            import torch
+            torch.cuda.current_stream(iq.device).synchronize()
+            ptr = iq.data_ptr()
+        cells = (Cell * (n_ch * max_cells))()
+        n = (C.c_uint32 * n_ch)()
+        _chk(lib().lcs_sweep_search_cu8_device(self._h, C.c_void_p(ptr), C.c_uint32(n_ch), _p(fc), _p(fcp),
+                                               C.c_double(fs_programmed), _p(f), C.c_uint32(f.size), cells,
+                                               C.c_uint32(max_cells), n), self.ctx._h)
+        return [[_copy(cells[b * max_cells + k]) for k in range(min(n[b], max_cells))] for b in range(n_ch)]
+
     def track_cu8(self, iq_cu8, frequency_offset, fc_requested, fs_programmed=1.92e6, fc_programmed=None, late=None, tracked=None,
                   max_cells=8, host_ptr=None):
         """searcher_thread.cpp:95-232 for all channels.  tracked: list (per channel) of lists of n_id_cell.  Returns a
@@ -562,6 +595,98 @@ class Tracker:
     def close(self):
         if self._h:
             lib().lcs_track_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def chan_design_taps(fs_in):
+    """The channelizer's prototype low-pass for input rate fs_in (host only, no device needed): float32 [L]."""
+    n = C.c_uint32(0)
+    _chk(lib().lcs_chan_design_taps(C.c_double(fs_in), None, C.byref(n)))
+    h = np.zeros(n.value, np.float32)
+    _chk(lib().lcs_chan_design_taps(C.c_double(fs_in), _p(h), C.byref(n)))
+    return h
+
+
+def _ci16(iq):
+    iq = np.ascontiguousarray(iq, np.int16)
+    if iq.ndim != 2 or iq.shape[1] != 2:
+        raise ValueError("expected ci16 samples [n][2]")
+    return iq
+
+
+class Channelizer:
+    """lcs_chan: wideband ci16 recording -> one 1.92 Msps cu8 stream per LTE raster channel (DESIGN.md section 4.6)."""
+
+    def __init__(self, ctx, fs_in, fc_in, fc_ch, gain=None):
+        self.ctx = ctx
+        fc = np.ascontiguousarray(np.atleast_1d(fc_ch), np.float64)
+        self.n_ch = fc.size
+        self.fc_ch = fc
+        g = None if gain is None else np.ascontiguousarray(np.broadcast_to(np.asarray(gain, np.float32), (self.n_ch,)))
+        self.taps = chan_design_taps(fs_in)
+        self.M = (self.taps.size - 1) // 2
+        self.D = int(round(fs_in / 1.92e6))
+        self._h = C.c_void_p()
+        _chk(lib().lcs_chan_create(ctx._h, C.c_double(fs_in), C.c_double(fc_in), C.c_uint32(self.n_ch), _p(fc), _p(g),
+                                   C.byref(self._h)), ctx._h)
+
+    def auto_gain(self, iq):
+        """Set every channel's gain to 0.25 / RMS of its output over these samples (the stream is not touched)."""
+        iq = _ci16(iq)
+        _chk(lib().lcs_chan_auto_gain_ci16(self._h, _p(iq), C.c_uint32(iq.shape[0])), self.ctx._h)
+        return self.gain
+
+    @property
+    def gain(self):
+        g = np.zeros(self.n_ch, np.float32)
+        _chk(lib().lcs_chan_gain(self._h, _p(g)), self.ctx._h)
+        return g
+
+    def n_out(self, n_in):
+        k = C.c_uint32(0)
+        _chk(lib().lcs_chan_n_out(self._h, C.c_uint64(n_in), C.byref(k)), self.ctx._h)
+        return k.value
+
+    def push_ci16(self, iq):
+        """Push ci16 [n][2] samples.  Returns (cu8 [n_ch][n_out][2], n_clipped [n_ch])."""
+        iq = _ci16(iq)
+        k = self.n_out(iq.shape[0])
+        out = np.zeros((self.n_ch, k, 2), np.uint8)
+        clip = np.zeros(self.n_ch, np.uint64)
+        got = C.c_uint32(0)
+        _chk(lib().lcs_chan_push_ci16(self._h, _p(iq), C.c_uint32(iq.shape[0]), _p(out), C.c_uint32(k), 0, C.byref(got),
+                                      _p(clip)), self.ctx._h)
+        return out, clip
+
+    def push_ci16_device(self, iq, out):
+        """Push ci16 [n][2] samples, writing the bytes into the uint8 CUDA tensor out [n_ch][capacity][2] from column 0
+        on.  Returns (n_out, n_clipped [n_ch])."""
+        iq = _ci16(iq)
+        if not (out.is_cuda and out.is_contiguous() and str(out.dtype) == "torch.uint8" and out.dim() == 3 and
+                out.shape[0] == self.n_ch and out.shape[2] == 2):
+            raise ValueError("push_ci16_device: expected a contiguous uint8 CUDA tensor [n_ch][capacity][2]")
+        cap = out.shape[1]
+        clip = np.zeros(self.n_ch, np.uint64)
+        got = C.c_uint32(0)
+        _chk(lib().lcs_chan_push_ci16(self._h, _p(iq), C.c_uint32(iq.shape[0]), C.c_void_p(out.data_ptr()),
+                                      C.c_uint32(cap), 1, C.byref(got), _p(clip)), self.ctx._h)
+        return got.value, clip
+
+    def timing_read(self):
+        """(kernel ms, launches) since the last read, from CUDA events around each launch."""
+        ms = C.c_double(0); n = C.c_uint64(0)
+        _chk(lib().lcs_chan_timing_read(self._h, C.byref(ms), C.byref(n)), self.ctx._h)
+        return ms.value, n.value
+
+    def close(self):
+        if self._h:
+            lib().lcs_chan_destroy(self._h)
             self._h = C.c_void_p()
 
     def __del__(self):

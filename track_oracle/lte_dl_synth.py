@@ -128,6 +128,41 @@ def synth_cu8(n_samples, cells, f_true=0.0, fc=739e6, fc_programmed=None, fs_pro
     k = (fc - f_true) / fcp
     n = np.arange(n_samples)
     t = n / (fs_programmed * k)                            # sampling instants (seconds)
+    x = _cells_baseband(t, cells, rng)
+    if stop_at is not None:
+        x[stop_at:] = 0
+    x *= np.exp(2j * np.pi * f_true * t)
+    sigma2 = AMP ** 2 / 10 ** (snr_db / 10)
+    x += np.sqrt(sigma2 / 2) * (rng.standard_normal(n_samples) + 1j * rng.standard_normal(n_samples))
+    iq = np.stack([x.real, x.imag], axis=1)
+    return np.clip(np.round(iq * 128 + 127), 0, 255).astype(np.uint8)
+
+
+def synth_wide_ci16(n, fs_in, fc_in, carriers, f_true=0.0, snr_db=10.0, seed=0, scale=4096.0):
+    """A wideband recording as interleaved int16 I/Q [n][2]: several LTE carriers seen through one receiver whose LO
+    and sample clock share one crystal.  carriers: list of (fc_c, cells, relative power), cells as in synth_cu8.
+
+    One oscillator ratio k = (fc_in - f_true) / fc_in: sample m is taken at t_m = m / (fs_in * k) and every OFDM symbol is
+    evaluated directly at those instants; carrier c sits at baseband fc_c - k * fc_in, so a channelizer channel at fc_c
+    (whose mixer runs in nominal samples) sees exactly the offset fc_c * (1 - k) a dongle tuned to fc_c would see.
+    AWGN of variance D * AMP^2 / 10^(snr_db/10) over the whole band (D = fs_in / 1.92 MHz) gives every 1.92 MHz channel
+    the per-resource-element SNR snr_db of synth_cu8 at relative power 1.  The sum is scaled by `scale` and rounded to
+    int16 (clamped)."""
+    rng = np.random.default_rng(seed)
+    k = (fc_in - f_true) / fc_in
+    t = np.arange(n) / (fs_in * k)
+    x = np.zeros(n, complex)
+    for fc_c, cells, rel in carriers:
+        x += np.sqrt(rel) * _cells_baseband(t, cells, rng) * np.exp(2j * np.pi * (fc_c - k * fc_in) * t)
+    sigma2 = (fs_in / FS_LTE16) * AMP ** 2 / 10 ** (snr_db / 10)
+    x += np.sqrt(sigma2 / 2) * (rng.standard_normal(n) + 1j * rng.standard_normal(n))
+    iq = np.stack([x.real, x.imag], axis=1)
+    return np.clip(np.round(iq * scale), -32768, 32767).astype(np.int16)
+
+
+def _cells_baseband(t, cells, rng):
+    """Sum of the cells' transmitted signals (per-port channel gains applied) at the instants t (seconds)."""
+    n_samples = t.size
     u = t * FS_LTE16                                       # in LTE samples
     x = np.zeros(n_samples, complex)
     for cell in cells:
@@ -158,13 +193,7 @@ def synth_cu8(n_samples, cells, f_true=0.0, fc=739e6, fc_programmed=None, fs_pro
             ph = np.exp(2j * np.pi * np.outer(d[sl], cn) / 128)
             v = np.sum(Xc[gg] * ph, axis=1) / np.sqrt(128)
             x[sl] += np.where(ok[sl], v, 0)
-    if stop_at is not None:
-        x[stop_at:] = 0
-    x *= np.exp(2j * np.pi * f_true * t)
-    sigma2 = AMP ** 2 / 10 ** (snr_db / 10)
-    x += np.sqrt(sigma2 / 2) * (rng.standard_normal(n_samples) + 1j * rng.standard_normal(n_samples))
-    iq = np.stack([x.real, x.imag], axis=1)
-    return np.clip(np.round(iq * 128 + 127), 0, 255).astype(np.uint8)
+    return x
 
 
 def to_c128(cu8):
