@@ -16,7 +16,7 @@
  *   - there is NO CPU fallback: every compute entry point needs a CUDA device (sm_90a) and
  *     fails with LCS_ERR_CUDA when none is usable.
  *   - threading: a context and the plans / sweep handles created from it belong to ONE host thread at a time (they
- *     share the context's two streams and scratch buffers).  Use one context per thread; contexts are independent.
+ *     share the context's three streams and scratch buffers).  Use one context per thread; contexts are independent.
  *   - array layouts are stated per argument; "ref layout" is the reference's own
  *     (vf3d [t][idx][f]; IT++ mat/imat column-major).
  */
@@ -195,11 +195,12 @@ lcs_status lcs_kalibrate_cu8(lcs_ctx* ctx, const uint8_t* capbuf_cu8, uint32_t n
  * capture buffers, everything on the device: only the PSS peaks return.  iq_host is [batch][n_cap] in iq_format;
  * peaks is [batch][max_peaks] (fc_requested, fc_programmed, pss_pow, ind, freq, n_id_2 filled as by peak_search,
  * in the reference's order), n_peaks[batch] the number found per buffer (may exceed max_peaks: list truncated).
- * Chunks of up to 64 buffers are double-buffered over the plan's two streams. */
+ * Chunks of up to 64 buffers rotate over the context's three streams. */
 lcs_status lcs_xcorr_peaks_batch_host(lcs_xcorr_plan* plan, const void* iq_host, int iq_format, uint32_t batch,
                                       lcs_cell* peaks, uint32_t max_peaks, uint32_t* n_peaks);
 /* The whole chain of CellSearch.cpp:497-558 for every buffer of a batch of raw rtl-sdr byte buffers (cu8
- * [batch][n_cap][2]); cells is [batch][max_cells], n_cells[batch].  Same results as lcs_cell_search_cu8 per buffer. */
+ * [batch][n_cap][2]); cells is [batch][max_cells], n_cells[batch].  lcs_cell_search_cu8 runs the same implementation
+ * on a batch of one. */
 lcs_status lcs_cell_search_batch_cu8(lcs_xcorr_plan* plan, const uint8_t* iq_host, uint32_t batch, lcs_cell* cells,
                                      uint32_t max_cells, uint32_t* n_cells);
 
@@ -219,8 +220,8 @@ lcs_status lcs_sweep_search_cu8(lcs_sweep* sweep, const uint8_t* iq_host, uint32
                                 lcs_cell* cells, uint32_t max_cells, uint32_t* n_cells);
 /* One searcher cycle (src/searcher_thread.cpp:95-232) for n_ch tracked channels: channel c is searched at the single
  * offset frequency_offset[c]; tracked_n_id_cell is [n_ch][tracked_stride] with n_tracked[c] valid entries (both may be
- * NULL); late[n_ch] or NULL; cells / frame_timing are [n_ch][max_cells].  Same results per channel as
- * lcs_tracker_search_cu8. */
+ * NULL); late[n_ch] or NULL; cells / frame_timing are [n_ch][max_cells].  lcs_tracker_search_cu8 runs the same
+ * implementation on a single channel. */
 lcs_status lcs_sweep_track_cu8(lcs_sweep* sweep, const uint8_t* iq_host, uint32_t n_ch, const double* frequency_offset,
                                const double* fc_requested, const double* fc_programmed, double fs_programmed,
                                const double* late, const int32_t* tracked_n_id_cell, const uint32_t* n_tracked,

@@ -43,12 +43,8 @@ static lcs_status build_plan(lcs_ctx* ctx, uint32_t n_cap, const double* f_searc
   cfg[0].f.assign(f_search_set, f_search_set + n_f);
   cudaStream_t st = ctx->streams[0];
   lcs_status rc = planset_build(ctx, p->ps, n_cap, arm, cfg, true, st);
+  if (rc == LCS_OK) rc = planset_finish(ctx, p->ps, st);
   if (rc != LCS_OK) return rc;
-  // the plan is used from arbitrary streams afterwards: finish the build here and read the builder's diagnostics
-  int flag = 0;
-  LCS_CUDA(ctx, cudaMemcpyAsync(&flag, p->ps.d_flag.p, 4, cudaMemcpyDeviceToHost, st));
-  LCS_CUDA(ctx, cudaStreamSynchronize(st));
-  if (flag) { p->ps.tc_ready = false; p->ps.tc_why = "template digits outside the exact range of the integer formulation"; }
   *out = p.release();
   return LCS_OK;
 }
@@ -82,11 +78,6 @@ static lcs_status run_device(lcs_xcorr_plan* p, const void* d_iq, int iq_format,
     p->ev_used.erase(p->ev_used.begin(), p->ev_used.begin() + 512);
   }
   return LCS_OK;
-}
-
-lcs_status plan_run_device(lcs_xcorr_plan* p, const void* d_iq, int iq_format, uint32_t batch, float* d_single, double* d_pow,
-                           int32_t* d_frq, double* d_spi, float* d_inc, cudaStream_t st) {
-  return run_device(p, d_iq, iq_format, batch, d_single, d_pow, d_frq, d_spi, d_inc, st);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -260,7 +251,7 @@ lcs_status lcs_xcorr_pss_batch_host(lcs_xcorr_plan* p, const void* h_iq, int iq_
   if (!h_iq || !h_pow || !h_frq || !h_spi) return fail(ctx, LCS_ERR_ARG, "xcorr_pss_batch_host: null pointer");
   if (batch == 0) return LCS_OK;
   const XcorrGeom& g = p->ps.geom;
-  const size_t samp_bytes = iq_format == LCS_IQ_CU8 ? 2 : (iq_format == LCS_IQ_CF32 ? 8 : (iq_format == LCS_IQ_C128 ? 16 : 0));
+  const size_t samp_bytes = iq_sample_bytes(iq_format);
   if (!samp_bytes) return fail(ctx, LCS_ERR_ARG, "xcorr_pss_batch_host: bad iq_format");
   LCS_CUDA(ctx, cudaSetDevice(ctx->device));
   // chunk: large enough that the persistent correlator CTAs get many tiles each (64 buffers x 38 tiles = 16.4 tiles per
@@ -308,13 +299,14 @@ lcs_status lcs_xcorr_pss(lcs_ctx* ctx, const double* capbuf, uint32_t n_cap, con
   const XcorrGeom& g = p->ps.geom;
   cudaStream_t st = ctx->streams[0];
   const size_t n_single = (size_t)3 * n_f * LCS_N_FOLD;
+  auto& hb = p->hb[0];
   LCS_CUDA(ctx, ctx->d_capbuf.ensure((size_t)n_cap * 2));
-  LCS_CUDA(ctx, ctx->d_single.ensure(n_single));
+  LCS_CUDA(ctx, hb.single.ensure(n_single));
   LCS_CUDA(ctx, ctx->d_ref.ensure(n_single));
   LCS_CUDA(ctx, ctx->d_inc.ensure(n_single));
-  LCS_CUDA(ctx, ctx->d_pow.ensure(3 * LCS_N_FOLD));
-  LCS_CUDA(ctx, ctx->d_frq.ensure(3 * LCS_N_FOLD));
-  LCS_CUDA(ctx, ctx->d_spi.ensure(LCS_N_FOLD));
+  LCS_CUDA(ctx, hb.pow.ensure(3 * LCS_N_FOLD));
+  LCS_CUDA(ctx, hb.frq.ensure(3 * LCS_N_FOLD));
+  LCS_CUDA(ctx, hb.spi.ensure(LCS_N_FOLD));
   LCS_CUDA(ctx, cudaMemcpyAsync(ctx->d_capbuf.p, capbuf, (size_t)n_cap * 16, cudaMemcpyHostToDevice, st));
   // 8-bit exact input (an rtl-sdr capture, capbuf.cpp:172-175) goes to the tensor-core correlator
   const void* d_in = ctx->d_capbuf.p;
@@ -330,11 +322,10 @@ lcs_status lcs_xcorr_pss(lcs_ctx* ctx, const double* capbuf, uint32_t n_cap, con
     LCS_CUDA(ctx, cudaStreamSynchronize(st));
     if (!inexact) { d_in = ctx->d_cu8.p; fmt = LCS_IQ_CU8; }
   }
-  rc = run_device(p, d_in, fmt, 1, ctx->d_single.p, ctx->d_pow.p, ctx->d_frq.p, ctx->d_spi.p,
-                  incoherent ? ctx->d_inc.p : nullptr, st);
+  rc = run_device(p, d_in, fmt, 1, hb.single.p, hb.pow.p, hb.frq.p, hb.spi.p, incoherent ? ctx->d_inc.p : nullptr, st);
   if (rc != LCS_OK) return rc;
   // reference layouts: vf3d [t][idx][f]; mat(3,9600) column-major
-  ctx->launches += launch_planar_to_ref(g, ctx->d_single.p, ctx->d_ref.p, st);
+  ctx->launches += launch_planar_to_ref(g, hb.single.p, ctx->d_ref.p, st);
   LCS_CUDA(ctx, cudaMemcpyAsync(single, ctx->d_ref.p, n_single * 4, cudaMemcpyDeviceToHost, st));
   if (incoherent) {
     LCS_CUDA(ctx, cudaStreamSynchronize(st));
@@ -343,9 +334,9 @@ lcs_status lcs_xcorr_pss(lcs_ctx* ctx, const double* capbuf, uint32_t n_cap, con
   }
   std::vector<double> hpow(3 * LCS_N_FOLD);
   std::vector<int32_t> hfrq(3 * LCS_N_FOLD);
-  LCS_CUDA(ctx, cudaMemcpyAsync(hpow.data(), ctx->d_pow.p, hpow.size() * 8, cudaMemcpyDeviceToHost, st));
-  LCS_CUDA(ctx, cudaMemcpyAsync(hfrq.data(), ctx->d_frq.p, hfrq.size() * 4, cudaMemcpyDeviceToHost, st));
-  LCS_CUDA(ctx, cudaMemcpyAsync(sp_incoherent, ctx->d_spi.p, LCS_N_FOLD * 8, cudaMemcpyDeviceToHost, st));
+  LCS_CUDA(ctx, cudaMemcpyAsync(hpow.data(), hb.pow.p, hpow.size() * 8, cudaMemcpyDeviceToHost, st));
+  LCS_CUDA(ctx, cudaMemcpyAsync(hfrq.data(), hb.frq.p, hfrq.size() * 4, cudaMemcpyDeviceToHost, st));
+  LCS_CUDA(ctx, cudaMemcpyAsync(sp_incoherent, hb.spi.p, LCS_N_FOLD * 8, cudaMemcpyDeviceToHost, st));
   if (xc) {
     const size_t n_xc = (size_t)3 * (n_cap - 136) * n_f;
     DevBuf<float2> d_xc;

@@ -101,10 +101,7 @@ struct lcs_ctx {
   double tc_scale = 0;                         // power of two S: |template component| * S fits 24 bits for every offset
   // scratch of the drop-in host calls
   lcs::DevBuf<double> d_capbuf;                // c128 capture buffer (2 doubles / sample)
-  lcs::DevBuf<float> d_single, d_ref, d_inc;
-  lcs::DevBuf<double> d_pow, d_spi;
-  lcs::DevBuf<int32_t> d_frq;
-  lcs::DevBuf<double> d_work;                  // sss / tfg kernels
+  lcs::DevBuf<float> d_ref, d_inc;
   lcs::DevBuf<unsigned char> d_cu8;
   lcs::DevBuf<int> d_flag8;                    // 8-bit exactness probe of lcs_xcorr_pss
   void* chain = nullptr;                       // lcs::ChainScratch (chain_api.cu), owned
@@ -120,7 +117,7 @@ struct lcs_xcorr_plan {
   std::vector<std::pair<cudaEvent_t, cudaEvent_t>> ev_pool, ev_used;
   double ev_acc_ms = 0;                        // time of event pairs already harvested from ev_used
   uint64_t ev_acc_n = 0;
-  // per-stream device buffers of the host-batch entry points
+  // per-stream device buffers of the host-input entry points (lcs_xcorr_pss uses stream 0's)
   struct HostBatchBufs {
     lcs::DevBuf<unsigned char> iq;
     lcs::DevBuf<float> single;
@@ -150,6 +147,9 @@ lcs_status fail(lcs_ctx* ctx, lcs_status st, const std::string& msg);
 // want_fp32: also build the FP32 correlator's templates (skipped for 8-bit-only sweeps).
 lcs_status planset_build(lcs_ctx* ctx, PlanSet& ps, uint32_t n_cap, uint8_t arm, const std::vector<PlanCfg>& cfgs,
                          bool want_fp32, cudaStream_t st);
+// Wait for the builds queued on `st` (the plans are used from every stream afterwards) and read the builder's
+// diagnostics: a digit plane out of range takes the set off the tensor-core correlator.
+lcs_status planset_finish(lcs_ctx* ctx, PlanSet& ps, cudaStream_t st);
 // Which kernel AUTO resolves to for this set and input format.
 int planset_resolve_kernel(const PlanSet& ps, int kernel, int iq_format);
 // xcorr_pss for `batch` device-resident capture buffers: correlator + sp_est + delay spread / argmax.  d_buf_plan
@@ -169,8 +169,5 @@ lcs_status cell_chain_dev(lcs_ctx* ctx, const void* d_cap, int fmt, uint32_t n_c
 lcs_status tc_init(lcs_ctx* ctx);           // one-time function attributes
 int launch_xcorr_fold_tc(PlanSet& ps, const void* d_iq_cu8, uint32_t batch, const uint32_t* d_buf_plan,
                          float* d_single_planar, cudaStream_t st);
-// ---- lcs_api.cu ----
-lcs_status plan_run_device(lcs_xcorr_plan* p, const void* d_iq, int iq_format, uint32_t batch, float* d_single, double* d_pow,
-                           int32_t* d_frq, double* d_spi, float* d_inc, cudaStream_t st);
 
 }  // namespace lcs

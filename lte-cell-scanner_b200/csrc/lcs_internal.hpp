@@ -13,6 +13,11 @@ namespace lcs {
 
 typedef std::complex<double> cd;
 
+// Bytes per complex sample of an LCS_IQ_* format; 0 for anything else.
+inline size_t iq_sample_bytes(int iq_format) {
+  return iq_format == LCS_IQ_CU8 ? 2 : iq_format == LCS_IQ_CF32 ? 8 : iq_format == LCS_IQ_C128 ? 16 : 0;
+}
+
 // ---- geometry of the fused FP32 correlator (xcorr_fp32.cu) ----
 constexpr int XC_R = 7;                 // lags per lane (7*8 B stride is LDS.64 bank-conflict free)
 constexpr int XC_TI = 32 * XC_R;        // 224 fold positions per block

@@ -263,6 +263,14 @@ lcs_status planset_build(lcs_ctx* ctx, PlanSet& ps, uint32_t n_cap, uint8_t arm,
   return LCS_OK;
 }
 
+lcs_status planset_finish(lcs_ctx* ctx, PlanSet& ps, cudaStream_t st) {
+  int flag = 0;
+  LCS_CUDA(ctx, cudaMemcpyAsync(&flag, ps.d_flag.p, 4, cudaMemcpyDeviceToHost, st));
+  LCS_CUDA(ctx, cudaStreamSynchronize(st));
+  if (flag) { ps.tc_ready = false; ps.tc_why = "template digits outside the exact range of the integer formulation"; }
+  return LCS_OK;
+}
+
 int planset_resolve_kernel(const PlanSet& ps, int kernel, int iq_format) {
   if (kernel == LCS_KERNEL_FP32) return LCS_KERNEL_FP32;
   if (kernel == LCS_KERNEL_TC) return LCS_KERNEL_TC;

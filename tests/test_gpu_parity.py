@@ -355,8 +355,8 @@ def test_device_peak_search_matches_host(ctx, lcs, capbuf0000):
 
 
 def test_cell_search_batch_matches_single(ctx, lcs, capbuf0000):
-    """lcs_cell_search_batch_cu8 == lcs_cell_search_cu8 per buffer (cells 277/271 on the real capture, none on noise);
-    more buffers than one chunk so that both streams and the chunk hand-over are exercised."""
+    """lcs_cell_search_batch_cu8 == lcs_cell_search_cu8 (a batch of one) per buffer (cells 277/271 on the real capture,
+    none on noise); more buffers than one chunk so that the stream rotation and the chunk hand-over are exercised."""
     fc = capbuf0000["fc"]
     f = lcs.f_search_set(fc, 120.0)
     real = capbuf0000["cu8"]
@@ -447,6 +447,37 @@ def test_device_peak_search_vs_oracle(ctx, lcs, oracle, capbuf0000):
     for a, b in zip(got[0], o_peaks):
         assert abs(a.pss_pow - b.pss_pow) < REL * o_peaks[0].pss_pow
     assert got[1] == []
+    plan.close()
+
+
+def test_peak_list_overflow_falls_back_to_host(ctx, lcs, oracle):
+    """A buffer with more PSS peaks than the device peak list holds (32) has its peak_search redone on the host: 16
+    copies of every root's pss_td, 600 samples apart within a root and 200 samples between roots so that no two overlap,
+    repeated in every half frame so that they fold coherently, over weak noise.  The batched peak search (the buffer
+    second in its chunk) and the single-buffer cell search report exactly the host list, which matches the oracle's."""
+    fc = 739e6
+    f = lcs.f_search_set(fc, 120.0)
+    half = np.zeros(9600, np.complex128)
+    for r in range(3):
+        for k in range(16):
+            s = 200 * r + 600 * k
+            half[s:s + 137] += oracle.pss_td(r)
+    sig = np.tile(half, 16) * (40.0 / np.abs(half).max())
+    cu8 = np.clip(np.round(synth_cu8(0x5EED, sigma=3.0) + np.stack([sig.real, sig.imag], axis=1)), 0, 255).astype(np.uint8)
+    key = lambda peaks: [(p.n_id_2, p.ind, p.freq, p.pss_pow) for p in peaks]
+    plan = ctx.plan(cu8.shape[0], f, 2, fc, fc, 1.92e6, max_batch=2)
+    ref = _host_peaks(ctx, lcs, plan, cu8, f, fc)
+    assert len(ref) > 32
+    got = plan.peaks_batch(np.stack([synth_cu8(0xC0FFEE), cu8]), lcs.IQ_CU8, max_peaks=128)
+    assert got[0] == [] and key(got[1]) == key(ref)
+    o = oracle.xcorr_pss(cu8_to_c128(cu8), f, 2, fc, fc, 1.92e6)
+    z = oracle.calc_Z_th1(o["sp_incoherent"], o["n_comb_xc"], 2)
+    o_peaks = oracle.peak_search(o["pow"], o["frq"], z, f, fc, fc, o["single"], 2)
+    assert [(p.n_id_2, p.ind, p.freq) for p in got[1]] == [(p.n_id_2, p.ind, p.freq) for p in o_peaks]
+    for a, b in zip(got[1], o_peaks):
+        assert abs(a.pss_pow - b.pss_pow) < REL * o_peaks[0].pss_pow
+    _, peaks = ctx.cell_search(cu8, f, fc, fc, 1.92e6, max_cells=128)
+    assert key(peaks) == key(ref)
     plan.close()
 
 
