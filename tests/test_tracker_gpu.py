@@ -10,7 +10,7 @@ sys.path.insert(0, os.path.join(ROOT, "track_oracle"))
 
 import lte_dl_synth as S  # noqa: E402
 import track_oracle as TO  # noqa: E402
-from test_tracker_oracle import FC, FS, cell_dict, lcs_cell  # noqa: E402
+from test_tracker_oracle import FC, FS, cell_dict, lcs_cell, true_frame_timing  # noqa: E402
 
 DISCRETE = ("n_id_cell", "n_ports", "cp_type", "dropped", "drop_sample", "n_symbols", "last_slice_start", "mib_attempts",
             "mib_successes", "mib_decode_failures")
@@ -34,12 +34,14 @@ def compare(g, o, gfo, ofo):
             assert np.abs(a[k] - b[k]).max() <= 1e-9 * max(np.abs(b[k]).max(), 1e-30), k
 
 
-def run_pair(lcs, ctx, cu8s, cells, fo0, step, fc=None, max_cells=4):
-    """cu8s: [n_ch][n][2]; cells: per channel list of (lcs_cell, frame_timing).  Compares after every push."""
+def run_pair(lcs, ctx, cu8s, cells, fo0, step, fc=None, max_cells=4, fc_programmed=None, fs_programmed=1.92e6,
+             history=None):
+    """cu8s: [n_ch][n][2]; cells: per channel list of (lcs_cell, frame_timing).  Compares after every push; each push's
+    device read of every channel is appended to `history` when one is given."""
     n_ch = len(cu8s)
     fc = np.full(n_ch, FC) if fc is None else np.asarray(fc)
-    g = lcs.Tracker(ctx, fc, fo0, max_cells=max_cells)
-    o = TO.Tracker(fc, fo0, max_cells=max_cells)
+    g = lcs.Tracker(ctx, fc, fo0, fs_programmed=fs_programmed, fc_programmed=fc_programmed, max_cells=max_cells)
+    o = TO.Tracker(fc, fo0, fs_programmed=fs_programmed, fc_programmed=fc_programmed, max_cells=max_cells)
     for ch in range(n_ch):
         for c, ft in cells[ch]:
             g.add_cell(ch, c, ft)
@@ -50,21 +52,172 @@ def run_pair(lcs, ctx, cu8s, cells, fo0, step, fc=None, max_cells=4):
         g.push_cu8(blk)
         o.push_cu8(blk)
         gfo, ofo = g.frequency_offset(), o.frequency_offset()
+        reads = [g.read(ch) for ch in range(n_ch)]
         for ch in range(n_ch):
-            compare(g.read(ch), o.read(ch), gfo, ofo)
+            compare(reads[ch], o.read(ch), gfo, ofo)
+        if history is not None:
+            history.append(reads)
     out = [g.read(ch) for ch in range(n_ch)], g.frequency_offset()
     g.close()
     return out
 
 
+def read_raw(read_fn, h, ch, m):
+    """lcs_track_read / to_read with room for m cells."""
+    import ctypes as C
+    import lcs_b200
+    out = (lcs_b200.TrackCell * m)()
+    n = C.c_uint32(0)
+    assert read_fn(h, ch, out, m, C.byref(n)) == 0
+    return [out[i].as_dict() for i in range(n.value)]
+
+
+# Cells of the tiled stream: one of each kind the tracker distinguishes (1, 2 and 4 ports; normal and extended CP), at
+# distinct CRS shifts (n_id_cell % 6).  Cell "a" is the strongest; the others, 3 to 4.5 dB down, still lock their MIB
+# under its interference.
+TILE_CELLS = dict(
+    a=dict(cell_dict(n_id_cell=277, n_ports=2, t0=1234.0), gains=[1.0, 0.8 * np.exp(0.7j)]),
+    c=dict(cell_dict(n_id_cell=100, n_ports=1, t0=7000.0), gains=[0.7]),
+    d=dict(cell_dict(n_id_cell=431, n_ports=4, t0=15000.0), gains=[0.6, 0.5j, -0.55, 0.45 * np.exp(-2j)]),
+    e=dict(cell_dict(n_id_cell=62, n_ports=2, cp_type=2, t0=11000.5), gains=[0.7, -0.5]),
+)
+
+
+@pytest.fixture(scope="module")
+def tile():
+    """20 frames (five PBCH periods) of the TILE_CELLS at f_true = 0.  With k = 1 every sample falls on the grid of the
+    frame, so repeats of the tile form one continuous, exactly periodic stream of any length."""
+    return S.synth_cu8(20 * 19200, list(TILE_CELLS.values()), f_true=0.0, snr_db=10, seed=9)
+
+
 @pytest.mark.gpu
-@pytest.mark.parametrize("n_ports,cp_type,declared", [(1, 1, 1), (2, 1, 2), (2, 2, 2), (2, 1, 4)])
+@pytest.mark.parametrize("n_ports,cp_type,declared", [(1, 1, 1), (2, 1, 2), (2, 2, 2), (2, 1, 4), (4, 1, 4), (4, 2, 4)])
 def test_tracker_matches_oracle_synthetic(lcs, ctx, n_ports, cp_type, declared):
     d = cell_dict(n_id_cell=277 if cp_type == 1 else 271, n_ports=n_ports, cp_type=cp_type)
     cu8 = S.synth_cu8(int(0.6 * FS), [d], f_true=3000.0, snr_db=10, seed=20 + n_ports + cp_type)
     (cells,), fo = run_pair(lcs, ctx, cu8[None], [[(lcs_cell(d, declared), d["t0"] - 2 + 0.6)]], 2700.0, 96000)
     if declared == n_ports:
         assert cells[0]["mib_successes"] == cells[0]["mib_attempts"] > 0
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("cp_type", [1, 2])
+def test_cell_search_four_port_cell_matches_oracle(ctx, oracle, cp_type):
+    """The searcher's four-port MIB decode (SFBC-FSTD combining, CRC mask) on the captures of
+    test_synthetic_cell_found_by_oracle_search, field by field against the oracle."""
+    d = cell_dict(n_id_cell=277 if cp_type == 1 else 271, n_ports=4, cp_type=cp_type)
+    cu8 = S.synth_cu8(153600, [d], f_true=3000.0, snr_db=10, seed=4 * 10 + cp_type)
+    f = np.arange(-10000, 10001, 5000.0)
+    o_cells, o_peaks = oracle.cell_search_one(S.to_c128(cu8), f, FC, FC, FS)
+    p_cells, p_peaks = ctx.cell_search(cu8, f, FC, FC, FS)
+    assert [(p.n_id_2, p.ind, p.freq) for p in p_peaks] == [(p.n_id_2, p.ind, p.freq) for p in o_peaks]
+    assert [c.n_id_cell() for c in p_cells] == [d["n_id_cell"]] == [c.n_id_cell() for c in o_cells]
+    for a, b in zip(p_cells, o_cells):
+        for k in ("n_id_1", "n_id_2", "cp_type", "ind", "n_ports", "n_rb_dl", "phich_duration", "phich_resource", "sfn"):
+            assert getattr(a, k) == getattr(b, k), k
+        assert abs(a.frame_start - b.frame_start) < 1e-9
+        assert abs(a.freq_fine - b.freq_fine) < 1e-6 and abs(a.freq_superfine - b.freq_superfine) < 1e-6
+    assert (p_cells[0].n_ports, p_cells[0].cp_type, p_cells[0].sfn) == (4, cp_type, 100)
+
+
+@pytest.mark.gpu
+def test_tracker_frame_timing_wrap_matches_oracle(lcs, ctx):
+    """A frame start 0.2 samples after the wrap, handed over 0.4 samples early (at 19199.8): the timing loop carries it
+    across 19200 -> 0 and, as the time stamps drift, back across 0 -> 19200."""
+    d = cell_dict(t0=2.2)
+    cu8 = S.synth_cu8(int(0.6 * FS), [d], f_true=3000.0, snr_db=10, seed=8)
+    hist = []
+    (cells,), _ = run_pair(lcs, ctx, cu8[None], [[(lcs_cell(d), (d["t0"] - 2 - 0.4) % 19200)]], 2700.0, 48000,
+                           history=hist)
+    ft = np.array([h[0][0]["frame_timing"] for h in hist])
+    first_low = np.flatnonzero(ft < 1)
+    assert first_low.size and np.any(ft[first_low[0]:] > 19199.9)
+    assert cells[0]["mib_successes"] == cells[0]["mib_attempts"] > 0
+
+
+@pytest.mark.gpu
+def test_tracker_programmed_rates_match_oracle(lcs, ctx):
+    """A tuner that reports a programmed carrier and sample rate other than the requested ones: both enter the time
+    stamps and get_fd through k = (fc_requested - f) / fc_programmed."""
+    fcp, fsp = FC - 2500.0, 1.92e6 * (1 + 4e-6)
+    d = cell_dict()
+    cu8 = S.synth_cu8(int(0.6 * FS), [d], f_true=3000.0, fc_programmed=fcp, fs_programmed=fsp, snr_db=10, seed=7)
+    (cells,), _ = run_pair(lcs, ctx, cu8[None], [[(lcs_cell(d), d["t0"] - 2 + 0.6)]], 2700.0, 96000,
+                           fc_programmed=[fcp], fs_programmed=fsp)
+    assert cells[0]["mib_successes"] == cells[0]["mib_attempts"] > 0
+
+
+@pytest.mark.gpu
+def test_tracker_full_channel_matches_oracle(lcs, ctx, tile):
+    """max_cells = 32: channel 0 fills all 32 slots (the four cells on the air, spread over the slots so that every pass
+    of the kernel's warp loop has one, between absent ids declaring 1, 2 and 4 ports), channel 1 tracks three."""
+    rng = np.random.default_rng(11)
+    on_air = {3: "a", 12: "d", 21: "e", 30: "c"}
+    absent = [int(i) for i in rng.permutation(504) if i not in (277, 100, 431, 62, 271)]
+    cells0 = []
+    for slot in range(32):
+        if slot in on_air:
+            d = TILE_CELLS[on_air[slot]]
+            cells0.append((lcs_cell(d), d["t0"] - 2 + 0.6))
+        else:
+            d = cell_dict(n_id_cell=absent.pop(), n_ports=(1, 2, 4)[slot % 3], cp_type=1 + (slot % 5 == 0))
+            cells0.append((lcs_cell(d), float(rng.uniform(0, 19200))))
+    d1 = cell_dict(n_id_cell=271, n_ports=4, cp_type=2, t0=3333.0)
+    ch1 = S.synth_cu8(2 * tile.shape[0], [d1], f_true=1500.0, fc=FC + 5e6, snr_db=10, seed=12)
+    cells1 = [(lcs_cell(d1), d1["t0"] - 2 + 0.6), (lcs_cell(cell_dict(n_id_cell=5, n_ports=1)), 4000.0),
+              (lcs_cell(cell_dict(n_id_cell=6, n_ports=2, cp_type=2)), 19100.0)]
+    cu8s = np.stack([np.concatenate([tile, tile]), ch1])
+    res, _ = run_pair(lcs, ctx, cu8s, [cells0, cells1], np.array([-300.0, 1200.0]), 96000, fc=[FC, FC + 5e6],
+                      max_cells=32)
+    assert [r["n_id_cell"] for r in res[0]] == [c.n_id_cell() for c, _ in cells0]
+    for slot, r in enumerate(res[0]):
+        assert r["mib_attempts"] > 0
+        assert (r["mib_successes"] == r["mib_attempts"]) == (slot in on_air)
+    assert len(res[1]) == 3 and res[1][0]["mib_successes"] == res[1][0]["mib_attempts"] > 0
+
+
+@pytest.mark.gpu
+def test_tracker_drop_in_the_middle_then_reuse_slot(lcs, ctx, tile):
+    """Cells a, b, c where b is not on the air: b drops after 1600 attempts while a and c stay locked.  A read with room
+    for one cell leaves the unreported drop in place; the next full read reports it and frees its slot, c moves down,
+    and d (four ports) is added into the freed slot and tracked for about a second."""
+    n_tiles = int(np.ceil(18.0 * FS / tile.shape[0]))
+    cu8 = np.concatenate([tile] * n_tiles)
+    a, c, d = TILE_CELLS["a"], TILE_CELLS["c"], TILE_CELLS["d"]
+    b = cell_dict(n_id_cell=11, n_ports=2)
+    g = lcs.Tracker(ctx, FC, -200.0, max_cells=3)
+    o = TO.Tracker(FC, -200.0, max_cells=3)
+    for x, ft in ((a, a["t0"] - 2 + 0.6), (b, 5000.0), (c, c["t0"] - 2 - 0.5)):
+        g.add_cell(0, lcs_cell(x), ft)
+        o.add_cell(0, lcs_cell(x), ft)
+    added_at = None
+    step = 1920000
+    for i in range(0, cu8.shape[0], step):
+        g.push_cu8(cu8[i:i + step])
+        o.push_cu8(cu8[i:i + step])
+        gfo, ofo = g.frequency_offset(), o.frequency_offset()
+        first = read_raw(lcs.lib().lcs_track_read, g._h, 0, 1)
+        compare(first, read_raw(TO.lib().to_read, o._h, 0, 1), gfo, ofo)
+        assert [r["n_id_cell"] for r in first] == [277]
+        gr, orr = g.read(0), o.read(0)
+        compare(gr, orr, gfo, ofo)
+        ids = [r["n_id_cell"] for r in gr]
+        if added_at is None:
+            assert ids == [277, 11, 100]
+            assert gr[0]["mib_successes"] == gr[0]["mib_attempts"] and gr[2]["mib_successes"] == gr[2]["mib_attempts"]
+            if gr[1]["dropped"]:
+                assert gr[1]["mib_attempts"] == 1600 and gr[1]["mib_successes"] == 0
+                ft = true_frame_timing(g, d, i + step, 0.0)
+                g.add_cell(0, lcs_cell(d), ft)
+                o.add_cell(0, lcs_cell(d), ft)
+                added_at = i + step
+            else:
+                assert gr[1]["mib_attempts"] < 1600
+        else:
+            assert ids == [277, 100, 431] and not any(r["dropped"] for r in gr)
+    assert added_at is not None and cu8.shape[0] - added_at >= 0.9 * FS
+    assert all(r["mib_successes"] == r["mib_attempts"] > 0 for r in gr)
+    g.close()
 
 
 @pytest.mark.gpu

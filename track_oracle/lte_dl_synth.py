@@ -1,8 +1,8 @@
 """Synthetic LTE downlink (6 centre RBs) as raw rtl-sdr bytes.  TEST INFRASTRUCTURE ONLY.
 
-Built on numpy and the searcher oracle's tables (oracle/lcs_oracle.py): PSS, SSS, CRS for 1 or 2 ports, PBCH carrying
-a chosen MIB (SFN advancing every frame, each frame carrying its quarter of the rate-matched bits), random QPSK on the
-other resource elements, normal or extended CP.
+Built on numpy and the searcher oracle's tables (oracle/lcs_oracle.py): PSS, SSS, CRS for 1, 2 or 4 ports, PBCH carrying
+a chosen MIB (SFN advancing every frame, each frame carrying its quarter of the rate-matched bits; transmit diversity by
+Alamouti for 2 ports and SFBC-FSTD for 4), random QPSK on the other resource elements, normal or extended CP.
 
 Oscillator model (the reference's crystal model): one oscillator error moves both the carrier and the sample clock.
 Sample n is taken at t_n = n / (fs_programmed * k), k = (fc - f_true) / fc_programmed, and every OFDM symbol's 72
@@ -99,6 +99,12 @@ def _grid(cell, n_frames, sfn0, rng):
                     X[:, g] = 0
                     if P == 1:
                         X[0, g, sc] = y
+                    elif P == 4:                            # SFBC-FSTD over RE quadruples (36.211 6.3.4.3)
+                        q0, q1, q2, q3 = y[0::4], y[1::4], y[2::4], y[3::4]
+                        X[0, g, sc[0::4]], X[0, g, sc[1::4]] = q0 / np.sqrt(2), q1 / np.sqrt(2)
+                        X[2, g, sc[0::4]], X[2, g, sc[1::4]] = -np.conj(q1) / np.sqrt(2), np.conj(q0) / np.sqrt(2)
+                        X[1, g, sc[2::4]], X[1, g, sc[3::4]] = q2 / np.sqrt(2), q3 / np.sqrt(2)
+                        X[3, g, sc[2::4]], X[3, g, sc[3::4]] = -np.conj(q3) / np.sqrt(2), np.conj(q2) / np.sqrt(2)
                     else:                                   # Alamouti over RE pairs
                         s0, s1 = y[0::2], y[1::2]
                         X[0, g, sc[0::2]], X[0, g, sc[1::2]] = s0 / np.sqrt(2), s1 / np.sqrt(2)
@@ -120,7 +126,7 @@ def _grid(cell, n_frames, sfn0, rng):
 
 def synth_cu8(n_samples, cells, f_true=0.0, fc=739e6, fc_programmed=None, fs_programmed=1.92e6, snr_db=10.0,
               seed=0, stop_at=None):
-    """cu8 [n][2].  cells: list of dicts with n_id_cell, n_ports (1/2), cp_type (1/2), n_rb_dl, phich_duration,
+    """cu8 [n][2].  cells: list of dicts with n_id_cell, n_ports (1/2/4), cp_type (1/2), n_rb_dl, phich_duration,
     phich_resource, t0 (frame start in LTE samples), sfn0, gains (per-port complex channel gains).
     snr_db: per resource element, relative to AMP^2.  stop_at: the cells stop transmitting at that sample."""
     rng = np.random.default_rng(seed)
@@ -170,7 +176,7 @@ def _cells_baseband(t, cells, rng):
         rel = u - cell.get("t0", 0.0)
         n_frames = int(np.ceil((rel.max() + 1) / FRAME)) + 1
         X, n_symb = _grid(cell, n_frames, cell.get("sfn0", 0), rng)
-        gains = cell.get("gains", [1.0, 0.8 * np.exp(0.7j)])[:cell["n_ports"]]
+        gains = cell.get("gains", [1.0, 0.8 * np.exp(0.7j), 0.9 * np.exp(-1.1j), 0.7 * np.exp(2.2j)])[:cell["n_ports"]]
         Xc = AMP * np.tensordot(np.asarray(gains), X, axes=1)
         fr = np.floor(rel / FRAME)
         p = rel - fr * FRAME
