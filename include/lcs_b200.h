@@ -284,6 +284,18 @@ typedef struct lcs_track_cell {
   double sync_tp_av, sync_sp_av, sync_np_av, sync_np_blank_av;
   double sync_ce[72][2];         /* c128, latest PSS/SSS channel estimate */
   double ce[4][72][2];           /* c128, latest interpolated CRS channel estimate per port */
+  /* Channel autocorrelations (do_ac_fd / do_ac_td, tracker_thread.cpp:318-370), c128, 0 until their first update.  Each
+   * update is normalised by the CRS signal power sp = max(1e-5, tp - np/7) of the estimate that makes it.  Every port
+   * of the cell updates the same arrays, ports in ascending order within a symbol.
+   * ac_fd[d]: lag d CRS subcarriers = 6d subcarriers = 90d kHz.  Each CRS symbol is weighted by 1/np_d, np_d =
+   *   (np^2/sp^2 + 2 np/sp) / (12 - d), against a prior of weight 1e5, so at high SNR it converges within about a second (ac_fd[0] about 1 on a flat channel).
+   * ac_td[t]: lag t CRS symbols of one port (ports 0/1: 4 and 3 OFDM symbols alternately, ports 2/3: one slot),
+   *   updated from the port's 72nd processed estimate on, each update with weight 1 against 1e5: after n updates it
+   *   is about n * 1e-5 times the mean correlation, so only its shape over t is meaningful for n << 1e5.
+   * Coherence bandwidth (display_thread.cpp:166-177): the first d in 1..11 with |ac_fd[d]| <= 0.5 gives 90d kHz,
+   * none gives more than 990 kHz. */
+  double ac_fd[12][2];
+  double ac_td[72][2];
 } lcs_track_cell;
 
 /* fc_requested[n_ch]; fc_programmed[n_ch] or NULL (= fc_requested); frequency_offset[n_ch] the initial offsets (the

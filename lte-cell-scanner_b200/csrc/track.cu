@@ -30,6 +30,7 @@ constexpr int GROUPS = THREADS / 64;        // FFT groups
 constexpr int MAX_PDU = 80;                 // symbols one cell completes in a block (<= 10000/137 + 1)
 constexpr int RING = 32;                    // data / interpolated-CE ring depth
 constexpr int TAIL = 128;                   // samples of the previous block kept in front of a push
+constexpr int HIST = 72;                    // raw CRS estimates per port kept for do_ac_td (tracker_thread.cpp:351)
 constexpr double kPi = 3.14159265358979323846;
 constexpr double kFs16 = 30720000.0 / 16;
 
@@ -52,6 +53,7 @@ struct Hdr {
   int ih[4], in_[4];        // interpolated-CE ring head / count
   int dh, dn;               // data ring
   int mh, mn, mib_sync;     // MIB ring
+  int ah[4], an[4];         // CE history ring of do_ac_td: head (oldest) / count
   int n_foe;                // FOE updates queued in this block
   double frame_timing;
 };
@@ -72,6 +74,8 @@ struct CellState {
   DataEnt data[RING];
   MibEnt mib[16];
   double2 sss_sym[72];
+  double2 hist[4][12][HIST];   // ce_history (tracker_thread.cpp:850): the port's last 72 raw estimates, subcarrier-major
+                               // so that the lanes of do_ac_td read consecutive entries
   lcs_track_cell out;
 };
 
@@ -274,6 +278,46 @@ __device__ int mib_attempt(const CellState& c, const Hdr& h, const Tables& tb, S
   return __shfl_sync(0xffffffffu, ok, 0);
 }
 
+// do_ac_fd and do_ac_td (tracker_thread.cpp:318-370) on port p's current raw estimate rc, one whole warp.  sp and np
+// are the values of do_toe_v2.  Lane d < 12 owns lag d of ac_fd; every lane owns lags lane, lane + 32 and lane + 64 of
+// ac_td and sums its 12 products in ascending order.
+__device__ void ac_update(CellState& c, Hdr& h, int p, const CeRaw& rc, double sp, double np, int lane) {
+  lcs_track_cell& o = c.out;
+  if (lane < 12) {
+    const int d = lane;
+    double2 a = make_double2(0, 0);
+    for (int t = 0; t < 12 - d; t++) a = cadd(a, cmul(conj2(rc.ce[t]), rc.ce[t + d]));
+    a = cdiv(cdiv(a, (double)(12 - d)), sp);
+    const double w = 1.0 / ((np * np / (sp * sp) + 2 * np / sp) / (12 - d));
+    o.ac_fd[d][0] = (o.ac_fd[d][0] * (1 / .00001) + a.x * w) / (1 / .00001 + w);
+    o.ac_fd[d][1] = (o.ac_fd[d][1] * (1 / .00001) + a.y * w) / (1 / .00001 + w);
+  }
+  // push the estimate into the history; once it holds 72 the oldest is overwritten (push_back, then pop_front)
+  const int nw = h.an[p] < HIST ? (h.ah[p] + h.an[p]) % HIST : h.ah[p];
+  if (lane < 12) c.hist[p][lane][nw] = rc.ce[lane];
+  __syncwarp();
+  if (h.an[p] < HIST) h.an[p]++;
+  else h.ah[p] = (h.ah[p] + 1) % HIST;
+  if (h.an[p] != HIST) return;
+  // ce_history[71] is entry nw; ce_history[71 - t] is t entries older
+  double2 x[3] = {make_double2(0, 0), make_double2(0, 0), make_double2(0, 0)};
+  for (int i = 0; i < 12; i++) {
+    const double2 ci = conj2(c.hist[p][i][nw]);
+    for (int j = 0; j < 3; j++) {
+      const int t = lane + 32 * j;
+      if (t < HIST) x[j] = cadd(x[j], cmul(ci, c.hist[p][i][(nw - t + HIST) % HIST]));
+    }
+  }
+  for (int j = 0; j < 3; j++) {
+    const int t = lane + 32 * j;
+    if (t >= HIST) continue;
+    const double2 v = cdiv(cdiv(x[j], 12.0), sp);
+    o.ac_td[t][0] = (o.ac_td[t][0] * (1 / .00001) + v.x * 1 / 1) / (1 / .00001 + 1);
+    o.ac_td[t][1] = (o.ac_td[t][1] * (1 / .00001) + v.y * 1 / 1) / (1 / .00001 + 1);
+  }
+  __syncwarp();                                     // all reads done before the next push overwrites the oldest entry
+}
+
 // The tracker loop for one symbol (tracker_thread.cpp:870-1066), one whole warp.  Returns 1 when the cell is dropped.
 __device__ int tracker_step(CellState& c, Hdr& h, const Tables& tb, Scratch& s, const ChanState& chn, double fs_prog, int k,
                             int lane) {
@@ -357,6 +401,7 @@ __device__ int tracker_step(CellState& c, Hdr& h, const Tables& tb, Scratch& s, 
     double diff = wrapd((rc.ft + delay) - h.frame_timing, -9600.0, 9600.0);
     diff = (0 * (1 / .0001) + diff * (1 / delay_np)) / (1 / .0001 + 1 / delay_np);
     const double ft_new = mmod(h.frame_timing + diff, 19200.0);
+    ac_update(c, h, p, rc, sp, np, lane);
     // push the filtered estimate, pop the oldest raw one
     CeFilt& fl = c.filt[p][h.n_filt[p]];
     if (lane < 12) fl.ce[lane] = f[lane];

@@ -8,13 +8,16 @@
 // offset (global_thread_data.frequency_offset(), moved by every cell's FOE), new cells are handed to the tracker, the
 // tracker's live cells are the searcher's skip list (so a dropped cell can be found again), and every N frames one status
 // line per cell is printed (id, ports, frame timing, offset, CRS SNR per port, MIB health as in display_thread.cpp:124),
-// plus a line for every dropped cell.
+// plus a line for every dropped cell.  -x (expert, with -t) adds what the reference's expert display prints under each
+// cell (display_thread.cpp:117-210, averaged values): the power of the unused subcarriers around PSS/SSS, one line per
+// port with CRS SP/NP/SNR in dB and the coherence bandwidth from the cell's frequency-domain channel autocorrelation, and
+// the PSS/SSS SP/NP/SNR.
 //
 // Like LTE-Tracker's main (src/LTE-Tracker.cpp:795-798) it first calibrates the oscillator with kalibrate
 // (src/LTE-Tracker.cpp:565-741, lcs_kalibrate_cu8) on the first 153600 samples of the stream unless -o gives the offset.
 //
 //   StreamSearch_b200 -f <fc Hz> [-o <frequency offset Hz>] [-p <ppm>] [-c <correction>] [-n <max cycles>]
-//                     [-t <status every N frames>] stream.bin
+//                     [-t <status every N frames> [-x]] stream.bin
 #include <getopt.h>
 
 #include <cmath>
@@ -24,9 +27,26 @@
 
 #include "../../include/lcs_b200.h"
 
+static double db10(double x) { return 10 * std::log10(x); }
+
+// The expert lines of one cell (display_thread.cpp:121-123, 151-177, 190-195).
+static void print_expert(const lcs_track_cell& t) {
+  printf("    UOS pwr %5.1f dB\n", db10(t.sync_np_blank_av));
+  for (int p = 0; p < t.n_ports; p++) {
+    printf("    P%d SP/NP/SNR %5.1f/%5.1f/%5.1f dB", p, db10(t.crs_sp_raw_av[p]), db10(t.crs_np_av[p]),
+           db10(t.crs_sp_raw_av[p] / t.crs_np_av[p]));
+    int cb = -1;                                 // coherence bandwidth: first lag with |ac_fd| <= 0.5, 90 kHz per lag
+    for (int k = 1; k < 12; k++)
+      if (std::hypot(t.ac_fd[k][0], t.ac_fd[k][1]) <= 0.5) { cb = k; break; }
+    if (cb == -1) printf("  CB >990 kHz\n");
+    else printf("  CB %d kHz\n", cb * 90);
+  }
+  printf("    S  SP/NP/SNR %5.1f/%5.1f/%5.1f dB\n", db10(t.sync_sp_av), db10(t.sync_np_av), db10(t.sync_sp_av / t.sync_np_av));
+}
+
 // The full tracker loop (-t): see the header comment.
 static int run_tracking(lcs_ctx* ctx, FILE* fp, double fc, double fc_programmed, double fs_programmed, uint32_t n_cap,
-                        double f_off, long max_cycles, long status_frames) {
+                        double f_off, long max_cycles, long status_frames, bool expert) {
   const uint32_t max_cells = 16;
   lcs_framer* fr = nullptr;
   lcs_track* tr = nullptr;
@@ -73,6 +93,7 @@ static int run_tracking(lcs_ctx* ctx, FILE* fp, double fc, double fc_programmed,
         printf("  cell %3d  ports %d  frame timing %9.3f  CRS SNR", t.n_id_cell, t.n_ports, t.frame_timing);
         for (int p = 0; p < t.n_ports; p++) printf(" %5.1f", 10 * std::log10(t.crs_sp_raw_av[p] / t.crs_np_av[p]));
         printf(" dB  MIB %lld/%lld  failures %.2f\n", (long long)t.mib_successes, (long long)t.mib_attempts, t.mib_decode_failures);
+        if (expert) print_expert(t);
       }
     }
     if (!searching || !ready) continue;
@@ -104,10 +125,10 @@ static int run_tracking(lcs_ctx* ctx, FILE* fp, double fc, double fc_programmed,
 
 int main(int argc, char** argv) {
   double fc = -1, f_off = 0, correction = 1, ppm = 120;
-  bool have_off = false;
+  bool have_off = false, expert = false;
   long max_cycles = -1, status_frames = -1;
   int c;
-  while ((c = getopt(argc, argv, "f:o:c:n:p:t:h")) != -1) {
+  while ((c = getopt(argc, argv, "f:o:c:n:p:t:xh")) != -1) {
     switch (c) {
       case 'f': fc = strtod(optarg, nullptr); break;
       case 'o': f_off = strtod(optarg, nullptr); have_off = true; break;
@@ -115,13 +136,14 @@ int main(int argc, char** argv) {
       case 'c': correction = strtod(optarg, nullptr); break;
       case 'n': max_cycles = strtol(optarg, nullptr, 10); break;
       case 't': status_frames = strtol(optarg, nullptr, 10); break;
+      case 'x': expert = true; break;
       default:
-        fprintf(stderr, "usage: %s -f <fc Hz> [-o <offset Hz>] [-p <ppm>] [-c <correction>] [-n <max cycles>] [-t <status frames>] stream.bin\n", argv[0]);
+        fprintf(stderr, "usage: %s -f <fc Hz> [-o <offset Hz>] [-p <ppm>] [-c <correction>] [-n <max cycles>] [-t <status frames> [-x]] stream.bin\n", argv[0]);
         return c == 'h' ? 0 : -1;
     }
   }
-  if (fc <= 0 || optind >= argc) {
-    fprintf(stderr, "usage: %s -f <fc Hz> [-o <offset Hz>] [-p <ppm>] [-c <correction>] [-n <max cycles>] [-t <status frames>] stream.bin\n", argv[0]);
+  if (fc <= 0 || optind >= argc || (expert && status_frames < 0)) {
+    fprintf(stderr, "usage: %s -f <fc Hz> [-o <offset Hz>] [-p <ppm>] [-c <correction>] [-n <max cycles>] [-t <status frames> [-x]] stream.bin\n", argv[0]);
     return -1;
   }
   FILE* fp = fopen(argv[optind], "rb");
@@ -149,7 +171,7 @@ int main(int argc, char** argv) {
     f_off = best.freq_superfine;                                                 // global_thread_data.frequency_offset(initial_freq_offset)
   }
   if (status_frames >= 0) {
-    const int rc = run_tracking(ctx, fp, fc, fc_programmed, fs_programmed, n_cap, f_off, max_cycles, status_frames);
+    const int rc = run_tracking(ctx, fp, fc, fc_programmed, fs_programmed, n_cap, f_off, max_cycles, status_frames, expert);
     lcs_ctx_destroy(ctx);
     fclose(fp);
     return rc;

@@ -524,14 +524,15 @@ class TrackCell(C.Structure):
         ("sync_tp_av", C.c_double), ("sync_sp_av", C.c_double), ("sync_np_av", C.c_double),
         ("sync_np_blank_av", C.c_double),
         ("sync_ce", C.c_double * 144), ("ce", C.c_double * (4 * 144)),
+        ("ac_fd", C.c_double * 24), ("ac_td", C.c_double * 144),
     ]
 
     def as_dict(self):
-        """Plain Python / numpy values; sync_ce is complex [72], ce complex [4][72]."""
+        """Plain Python / numpy values; sync_ce and ac_td are complex [72], ac_fd complex [12], ce complex [4][72]."""
         d = {}
         for k, _ in self._fields_:
             v = getattr(self, k)
-            if k == "sync_ce":
+            if k in ("sync_ce", "ac_fd", "ac_td"):
                 v = np.ctypeslib.as_array(v).copy().view(np.complex128)
             elif k == "ce":
                 v = np.ctypeslib.as_array(v).copy().view(np.complex128).reshape(4, 72)

@@ -167,38 +167,52 @@ def synth_wide_ci16(n, fs_in, fc_in, carriers, f_true=0.0, snr_db=10.0, seed=0, 
 
 
 def _cells_baseband(t, cells, rng):
-    """Sum of the cells' transmitted signals (per-port channel gains applied) at the instants t (seconds)."""
+    """Sum of the cells' received signals at the instants t (seconds): per-port channel gains, then the cell's
+    multipath channel.  A cell's optional `paths` [(delay_s, complex_gain, doppler_hz), ...] sum copies of its signal
+    evaluated at t - delay_s (exact for any delay, also inside the cyclic prefix), each times
+    complex_gain * exp(j 2 pi doppler_hz t).  Without `paths` the cell is received as transmitted."""
     n_samples = t.size
     u = t * FS_LTE16                                       # in LTE samples
     x = np.zeros(n_samples, complex)
     for cell in cells:
-        cp = cell["cp_type"]
         rel = u - cell.get("t0", 0.0)
         n_frames = int(np.ceil((rel.max() + 1) / FRAME)) + 1
         X, n_symb = _grid(cell, n_frames, cell.get("sfn0", 0), rng)
         gains = cell.get("gains", [1.0, 0.8 * np.exp(0.7j), 0.9 * np.exp(-1.1j), 0.7 * np.exp(2.2j)])[:cell["n_ports"]]
         Xc = AMP * np.tensordot(np.asarray(gains), X, axes=1)
-        fr = np.floor(rel / FRAME)
-        p = rel - fr * FRAME
-        slot = np.floor(p / 960)
-        q = p - slot * 960
-        if cp == 1:
-            sym = np.where(q < 138, 0, 1 + np.floor((q - 138) / 137))
-            start = np.where(sym == 0, 0, 138 + (sym - 1) * 137)
-            d = q - start - np.where(sym == 0, 10, 9)
-        else:
-            sym = np.floor(q / 160)
-            d = q - sym * 160 - 32
-        g = ((fr + 1) * 20 + slot) * n_symb + sym          # frame index shifted by one: samples before t0
-        g = g.astype(np.int64) - 20 * n_symb
-        ok = (g >= 0) & (g < X.shape[1])
-        cn = np.concatenate([np.arange(-36, 0), np.arange(1, 37)])
-        for c0 in range(0, n_samples, 65536):
-            sl = slice(c0, min(c0 + 65536, n_samples))
-            gg = np.where(ok[sl], g[sl], 0)
-            ph = np.exp(2j * np.pi * np.outer(d[sl], cn) / 128)
-            v = np.sum(Xc[gg] * ph, axis=1) / np.sqrt(128)
-            x[sl] += np.where(ok[sl], v, 0)
+        if "paths" not in cell:
+            x += _eval_grid(Xc, n_symb, cell["cp_type"], rel)
+            continue
+        for delay, gain, doppler in cell["paths"]:
+            x += gain * np.exp(2j * np.pi * doppler * t) * _eval_grid(Xc, n_symb, cell["cp_type"], rel - delay * FS_LTE16)
+    return x
+
+
+def _eval_grid(Xc, n_symb, cp, rel):
+    """The OFDM signal of the grid Xc [n_sym][72] at rel (LTE samples after the cell's frame start); 0 outside it."""
+    n_samples = rel.size
+    x = np.zeros(n_samples, complex)
+    fr = np.floor(rel / FRAME)
+    p = rel - fr * FRAME
+    slot = np.floor(p / 960)
+    q = p - slot * 960
+    if cp == 1:
+        sym = np.where(q < 138, 0, 1 + np.floor((q - 138) / 137))
+        start = np.where(sym == 0, 0, 138 + (sym - 1) * 137)
+        d = q - start - np.where(sym == 0, 10, 9)
+    else:
+        sym = np.floor(q / 160)
+        d = q - sym * 160 - 32
+    g = ((fr + 1) * 20 + slot) * n_symb + sym          # frame index shifted by one: samples before t0
+    g = g.astype(np.int64) - 20 * n_symb
+    ok = (g >= 0) & (g < Xc.shape[0])
+    cn = np.concatenate([np.arange(-36, 0), np.arange(1, 37)])
+    for c0 in range(0, n_samples, 65536):
+        sl = slice(c0, min(c0 + 65536, n_samples))
+        gg = np.where(ok[sl], g[sl], 0)
+        ph = np.exp(2j * np.pi * np.outer(d[sl], cn) / 128)
+        v = np.sum(Xc[gg] * ph, axis=1) / np.sqrt(128)
+        x[sl] += np.where(ok[sl], v, 0)
     return x
 
 

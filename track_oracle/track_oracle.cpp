@@ -7,6 +7,7 @@
 // block.  It is compiled together with the searcher oracle (oracle/lcs_oracle.cpp), whose tables, FFT, rate matching,
 // Viterbi, CRC and QPSK demodulator it uses.  It lives apart from oracle/, whose restatement of the searcher is pinned
 // by the reference's golden vectors and left as it is.  Nothing under lte-cell-scanner_b200/ uses this file.
+#include <array>
 #include <cmath>
 #include <cstring>
 #include <deque>
@@ -69,6 +70,7 @@ struct TCell {
   std::deque<MibPdu> mib_fifo;
   bool mib_sync = false;
   cd sss_sym[72];
+  std::deque<std::array<cd, 12>> ce_history[4];   // tracker_thread.cpp:850
   TCell(const lcs_cell& c, double ft)
       : info(c), n_id_cell(c.n_id_2 + 3 * c.n_id_1), n_id_1(c.n_id_1), n_id_2(c.n_id_2), n_ports(c.n_ports),
         cp_type(c.cp_type), n_symb(c.cp_type == 1 ? 7 : 6), frame_timing(ft), rs(n_id_cell, 6, c.cp_type) {
@@ -199,6 +201,45 @@ void do_toe_v2(TCell& c, const CeRaw& p, const CeRaw& cu, double sp, double np) 
   double diff = wrap((cu.frame_timing + delay) - c.frame_timing, -19200.0 / 2, 19200.0 / 2);
   diff = (0 * (1 / .0001) + diff * (1 / delay_np)) / (1 / .0001 + 1 / delay_np);
   c.frame_timing = matlab_mod(c.frame_timing + diff, 19200.0);
+}
+
+// do_ac_fd, tracker_thread.cpp:318-340
+void do_ac_fd(TCell& c, const CeRaw& cu, double sp, double np) {
+  cd ac[12];
+  for (int d = 0; d < 12; d++) {
+    ac[d] = 0;
+    for (int t = 0; t < 12 - d; t++) ac[d] += std::conj(cu.ce[t]) * cu.ce[t + d];
+    ac[d] = ac[d] / (double)(12 - d);
+  }
+  for (int d = 0; d < 12; d++) ac[d] = ac[d] / sp;
+  for (int d = 0; d < 12; d++) {
+    const double ac_np = (np * np / (sp * sp) + 2 * np / sp) / (12 - d);   // matlab_range(12.0, -1.0, 1.0)
+    double* o = c.out.ac_fd[d];
+    const double w = 1.0 / ac_np;
+    o[0] = (o[0] * (1 / .00001) + ac[d].real() * w) / (1 / .00001 + w);
+    o[1] = (o[1] * (1 / .00001) + ac[d].imag() * w) / (1 / .00001 + w);
+  }
+}
+
+// do_ac_td, tracker_thread.cpp:343-370
+void do_ac_td(TCell& c, const CeRaw& cu, double sp, std::deque<std::array<cd, 12>>& ce_history) {
+  std::array<cd, 12> v;
+  for (int i = 0; i < 12; i++) v[i] = cu.ce[i];
+  ce_history.push_back(v);
+  if (ce_history.size() > 72) ce_history.pop_front();
+  if (ce_history.size() != 72) return;
+  cd xc[72];
+  for (int t = 0; t < 72; t++) {
+    cd s = 0;
+    for (int i = 0; i < 12; i++) s += std::conj(ce_history[71][i]) * ce_history[71 - t][i];
+    xc[t] = s / 12.0;
+  }
+  for (int t = 0; t < 72; t++) xc[t] = xc[t] / sp;
+  for (int t = 0; t < 72; t++) {
+    double* o = c.out.ac_td[t];
+    o[0] = (o[0] * (1 / .00001) + xc[t].real() * 1 / 1) / (1 / .00001 + 1);
+    o[1] = (o[1] * (1 / .00001) + xc[t].imag() * 1 / 1) / (1 / .00001 + 1);
+  }
 }
 
 // interp72, tracker_thread.cpp:372-393
@@ -423,6 +464,8 @@ bool tracker_step(TCell& c, Channel& chn, double fs_prog, const TdPdu& pdu) {
     c.filt[p].push_back(f);
     do_foe(chn, fs_prog, rp, rn, np, f.ce_filt);
     do_toe_v2(c, rp, rc, sp, np);
+    do_ac_fd(c, rc, sp, np);                  // tracker_thread.cpp:955
+    do_ac_td(c, rc, sp, c.ce_history[p]);     // tracker_thread.cpp:958
     c.raw[p].pop_front();
   }
   for (int p = 0; p < c.n_ports; p++) {
