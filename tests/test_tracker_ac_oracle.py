@@ -1,6 +1,6 @@
 """CPU checks of the tracker oracle's channel autocorrelations (do_ac_fd / do_ac_td, tracker_thread.cpp:318-370) and of
 the synthetic generator's multipath model they are tested on.  The streams are built here and shared with
-tests/test_tracker_ac_gpu.py."""
+tests/test_tracker_gpu.py."""
 import hashlib
 import os
 import sys

@@ -1,5 +1,7 @@
 """The device cell tracker (lcs_track_*) against its CPU oracle (track_oracle/), on synthetic and recorded streams."""
 import os
+import re
+import subprocess
 import sys
 
 import numpy as np
@@ -10,28 +12,39 @@ sys.path.insert(0, os.path.join(ROOT, "track_oracle"))
 
 import lte_dl_synth as S  # noqa: E402
 import track_oracle as TO  # noqa: E402
+from lcs_b200 import TrackCell  # noqa: E402
+from test_tracker_ac_oracle import STREAMS, crs_estimates, stream  # noqa: E402
 from test_tracker_oracle import FC, FS, cell_dict, lcs_cell, true_frame_timing  # noqa: E402
 
+# Every field of lcs_track_cell is in exactly one of these classes, each with its own tolerance.
 DISCRETE = ("n_id_cell", "n_ports", "cp_type", "dropped", "drop_sample", "n_symbols", "last_slice_start", "mib_attempts",
             "mib_successes", "mib_decode_failures")
 MEAS = ("crs_tp", "crs_sp_raw", "crs_np", "crs_tp_av", "crs_sp_raw_av", "crs_np_av", "sync_tp", "sync_sp", "sync_np",
         "sync_np_blank", "sync_tp_av", "sync_sp_av", "sync_np_av", "sync_np_blank_av")
+COMPLEX = ("ce", "sync_ce", "ac_fd", "ac_td")
 
 
 def compare(g, o, gfo, ofo):
+    """Device reads g against oracle reads o, field by field over TrackCell: discrete values exactly, frame_timing to
+    1e-9, measurements to 1e-9 relative with the same NaNs, complex arrays to 1e-9 of the oracle array's largest
+    magnitude.  A field in no class fails, so that a new field of lcs_track_cell cannot go unchecked."""
     assert np.abs(gfo - ofo).max() < 1e-6
     assert len(g) == len(o)
     for a, b in zip(g, o):
-        for k in DISCRETE:
-            assert a[k] == b[k], k
-        assert abs(a["frame_timing"] - b["frame_timing"]) < 1e-9
-        for k in MEAS:
-            x, y = np.asarray(a[k], float), np.asarray(b[k], float)
-            assert np.array_equal(np.isnan(x), np.isnan(y)), k
-            m = ~np.isnan(y)
-            assert np.all(np.abs(x[m] - y[m]) <= 1e-9 * np.maximum(np.abs(y[m]), 1e-30)), k
-        for k in ("ce", "sync_ce"):
-            assert np.abs(a[k] - b[k]).max() <= 1e-9 * max(np.abs(b[k]).max(), 1e-30), k
+        for k, _ in TrackCell._fields_:
+            if k in DISCRETE:
+                assert a[k] == b[k], k
+            elif k == "frame_timing":
+                assert abs(a[k] - b[k]) < 1e-9, k
+            elif k in MEAS:
+                x, y = np.asarray(a[k], float), np.asarray(b[k], float)
+                assert np.array_equal(np.isnan(x), np.isnan(y)), k
+                m = ~np.isnan(y)
+                assert np.all(np.abs(x[m] - y[m]) <= 1e-9 * np.maximum(np.abs(y[m]), 1e-30)), k
+            elif k in COMPLEX:
+                assert np.abs(a[k] - b[k]).max() <= 1e-9 * max(np.abs(b[k]).max(), 1e-30), k
+            else:
+                pytest.fail(f"lcs_track_cell field {k} has no comparison class")
 
 
 def run_pair(lcs, ctx, cu8s, cells, fo0, step, fc=None, max_cells=4, fc_programmed=None, fs_programmed=1.92e6,
@@ -65,8 +78,7 @@ def run_pair(lcs, ctx, cu8s, cells, fo0, step, fc=None, max_cells=4, fc_programm
 def read_raw(read_fn, h, ch, m):
     """lcs_track_read / to_read with room for m cells."""
     import ctypes as C
-    import lcs_b200
-    out = (lcs_b200.TrackCell * m)()
+    out = (TrackCell * m)()
     n = C.c_uint32(0)
     assert read_fn(h, ch, out, m, C.byref(n)) == 0
     return [out[i].as_dict() for i in range(n.value)]
@@ -93,11 +105,24 @@ def tile():
 @pytest.mark.gpu
 @pytest.mark.parametrize("n_ports,cp_type,declared", [(1, 1, 1), (2, 1, 2), (2, 2, 2), (2, 1, 4), (4, 1, 4), (4, 2, 4)])
 def test_tracker_matches_oracle_synthetic(lcs, ctx, n_ports, cp_type, declared):
+    """Every autocorrelation lag ends non-zero; with 4 ports declared on a 2-port cell, ports 2 and 3 see no CRS and their
+    sp is clamped to 1e-5."""
     d = cell_dict(n_id_cell=277 if cp_type == 1 else 271, n_ports=n_ports, cp_type=cp_type)
     cu8 = S.synth_cu8(int(0.6 * FS), [d], f_true=3000.0, snr_db=10, seed=20 + n_ports + cp_type)
     (cells,), fo = run_pair(lcs, ctx, cu8[None], [[(lcs_cell(d, declared), d["t0"] - 2 + 0.6)]], 2700.0, 96000)
     if declared == n_ports:
         assert cells[0]["mib_successes"] == cells[0]["mib_attempts"] > 0
+    assert np.all(cells[0]["ac_td"] != 0) and np.all(cells[0]["ac_fd"] != 0)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("name", sorted(STREAMS))
+def test_ac_matches_oracle_multipath(lcs, ctx, name):
+    """The flat, two-path and Doppler streams of test_tracker_ac_oracle.py."""
+    d, seconds, seed = STREAMS[name]
+    cu8, ft, fo = stream(d, seconds, seed)
+    ((r,),), _ = run_pair(lcs, ctx, cu8[None], [[(lcs_cell(d), ft)]], fo, 192000)
+    assert r["mib_successes"] == r["mib_attempts"] > 0
 
 
 @pytest.mark.gpu
@@ -220,29 +245,37 @@ def test_tracker_drop_in_the_middle_then_reuse_slot(lcs, ctx, tile):
     g.close()
 
 
-@pytest.mark.gpu
-def test_tracker_real_capture(lcs, ctx, capbuf0000):
-    """The recording framed and searched as the searcher cycle does; its cells handed to a tracker of the same stream
-    before the first push, so that their frame timing refers to the tracker's own time stamps."""
+@pytest.fixture(scope="module")
+def real_capture_handover(lcs, ctx, capbuf0000):
+    """The recording framed and searched as the searcher cycle does; cells 277 and 271 with their frame timing in the
+    time stamps of a tracker that starts on the same stream.  (stream, cells, f_off, fc)."""
     fc, fs = capbuf0000["fc"], 1.92e6
     real = capbuf0000["cu8"]
     full, _ = ctx.cell_search(real, lcs.f_search_set(fc, 120.0), fc, fc, fs)
     f_off = float(np.round(full[0].freq_superfine))
     lead = np.random.default_rng(5).integers(100, 156, size=(19200 + 777, 2), dtype=np.uint8)
-    stream = np.concatenate([lead, real, lead])
+    st = np.concatenate([lead, real, lead])
     fr = lcs.Framer(fc, fc, fs, real.shape[0])
-    fr.push(stream[:500], f_off)
+    fr.push(st[:500], f_off)
     fr.request()
     got = None
-    for lo in range(500, stream.shape[0], 10000):
-        got = got or fr.push(stream[lo:lo + 10000], f_off)
+    for lo in range(500, st.shape[0], 10000):
+        got = got or fr.push(st[lo:lo + 10000], f_off)
     cap, late = got
     found = ctx.tracker_search_cu8(cap, f_off, fc, fc, fs, late)
     cells = [(c, ft % 19200) for c, ft in found if c.n_id_cell() in (277, 271)]
     assert sorted(c.n_id_cell() for c, _ in cells) == [271, 277]
-    (res,), _ = run_pair(lcs, ctx, stream[None], [cells], f_off, 10000, fc=[fc])
+    return st, cells, f_off, fc
+
+
+@pytest.mark.gpu
+def test_tracker_real_capture(lcs, ctx, real_capture_handover):
+    """The recording's cells handed to a tracker of the same stream before the first push."""
+    st, cells, f_off, fc = real_capture_handover
+    (res,), _ = run_pair(lcs, ctx, st[None], [cells], f_off, 10000, fc=[fc])
     assert [r["n_id_cell"] for r in res] == [c.n_id_cell() for c, _ in cells]
     assert all(r["mib_successes"] > 0 for r in res)
+    assert all(np.any(r["ac_fd"]) for r in res)
 
 
 @pytest.mark.gpu
@@ -297,9 +330,16 @@ def test_tracker_push_size_and_time_stamps(lcs, ctx):
 
 @pytest.mark.gpu
 def test_tracker_drop_matches_oracle(lcs, ctx):
+    """A cell on noise drops with a full CE history and non-zero autocorrelations.  A cell added into the freed slot
+    reads zero arrays, keeps ac_fd 0 until its first estimate and ac_td exactly 0 until its own 72nd (so no entry of the
+    old history is used)."""
     rng = np.random.default_rng(5)
+
+    def noise(n):
+        return np.clip(np.round(127 + 128 * 0.1 * rng.standard_normal((n, 2))), 0, 255).astype(np.uint8)
+
     n = int(16.4 * FS)
-    cu8 = np.clip(np.round(127 + 128 * 0.1 * rng.standard_normal((n, 2))), 0, 255).astype(np.uint8)
+    cu8 = noise(n)
     g = lcs.Tracker(ctx, FC, 0.0)
     g.add_cell(0, lcs_cell(cell_dict()), 100.0)
     o = TO.Tracker(FC, 0.0)
@@ -310,7 +350,29 @@ def test_tracker_drop_matches_oracle(lcs, ctx):
     gr, orr = g.read(0), o.read(0)
     compare(gr, orr, g.frequency_offset(), o.frequency_offset())
     assert gr[0]["dropped"] == 1 and gr[0]["mib_attempts"] == 1600
+    assert np.all(gr[0]["ac_td"] != 0) and np.all(gr[0]["ac_fd"] != 0)
     assert g.read(0) == []
+    for t in (g, o):
+        t.add_cell(0, lcs_cell(cell_dict(n_id_cell=11)), 5000.0)
+    (r,) = g.read(0)
+    compare([r], o.read(0), g.frequency_offset(), o.frequency_offset())
+    assert r["n_symbols"] == 0 and not np.any(r["ac_fd"]) and not np.any(r["ac_td"])
+    more = noise(int(0.2 * FS))
+    seen = set()
+    for i in range(0, more.shape[0], 10000):
+        g.push_cu8(more[i:i + 10000])
+        o.push_cu8(more[i:i + 10000])
+        (r,) = g.read(0)
+        compare([r], o.read(0), g.frequency_offset(), o.frequency_offset())
+        u = crs_estimates(r["n_symbols"]) - 71
+        seen.add(u > 0)
+        assert np.any(r["ac_fd"]) == (crs_estimates(r["n_symbols"]) > 0)   # the first symbols may come in later blocks
+        if u <= 0:
+            assert not np.any(r["ac_td"]), r["n_symbols"]
+        else:
+            assert np.all(r["ac_td"] != 0)
+    assert seen == {False, True}
+    g.close()
 
 
 @pytest.mark.gpu
@@ -341,26 +403,39 @@ def test_tracker_bad_arguments(lcs, ctx):
 @pytest.mark.gpu
 def test_stream_search_cli_tracks_cells(lcs, ctx, tmp_path):
     """`StreamSearch_b200 -t N`: kalibrate, then framer + searcher cycles + the cell tracker on one stream; the searcher
-    runs at the tracker's (moving) offset, the cell found is tracked with its MIB locked, and the offset stays on f_true."""
-    import re
-    import subprocess
+    runs at the tracker's (moving) offset, the cell found is tracked with its MIB locked, and the offset stays on f_true.
+    `-x` adds under each status line of cell 277 the UOS power, one SP/NP/SNR + coherence bandwidth line per port and
+    the PSS/SSS line, and changes nothing else."""
     host = os.path.join(ROOT, "lte-cell-scanner_b200", "host")
     subprocess.check_call(["make", "-C", host, "-s"])
     f_true, d = 3000.0, cell_dict()
     S.synth_cu8(int(2 * FS), [d], f_true=f_true, snr_db=10, seed=30).tofile(str(tmp_path / "stream.bin"))
-    out = subprocess.run([os.path.join(host, "StreamSearch_b200"), "-f", "739000000", "-n", "6", "-t", "50",
-                          str(tmp_path / "stream.bin")], capture_output=True, text=True, timeout=300)
-    assert out.returncode == 0, out.stderr + out.stdout
-    assert "Calibration succeeded!" in out.stdout
-    assert re.search(r"cycle 0: new cell 277 ", out.stdout)
-    searched = [float(v) for v in re.findall(r"searched at tracker offset ([-0-9.]+) Hz", out.stdout)]
+
+    def run(*opts):
+        r = subprocess.run([os.path.join(host, "StreamSearch_b200"), "-f", "739000000", "-n", "6", "-t", "50", *opts,
+                            str(tmp_path / "stream.bin")], capture_output=True, text=True, timeout=300)
+        assert r.returncode == 0, r.stderr + r.stdout
+        return r.stdout
+
+    out, expert = run(), run("-x")
+    assert "Calibration succeeded!" in out
+    assert re.search(r"cycle 0: new cell 277 ", out)
+    searched = [float(v) for v in re.findall(r"searched at tracker offset ([-0-9.]+) Hz", out)]
     assert len(searched) == 6 and len(set(searched)) == 6          # the offset moves with the tracker's FOE
-    status = [float(v) for v in re.findall(r"frequency offset ([-0-9.]+) Hz", out.stdout)]
+    status = [float(v) for v in re.findall(r"frequency offset ([-0-9.]+) Hz", out)]
     assert len(status) >= 3 and all(abs(f - f_true) < 5 for f in searched + status)
-    rows = re.findall(r"cell 277  ports 2 .* MIB (\d+)/(\d+)  failures ([0-9.]+)", out.stdout)
+    rows = re.findall(r"cell 277  ports 2 .* MIB (\d+)/(\d+)  failures ([0-9.]+)", out)
     # the cell starts at slot 0 symbol 0 of the block after its hand-over, so its first MIB windows can straddle two PBCH
     # periods (failures of 0.25 each, tracker_thread.cpp:727-733); once locked no attempt fails
     lost = [int(n) - int(ok) for ok, n, _ in rows]
     assert len(rows) >= 3 and lost[0] <= 3 and len(set(lost)) == 1 and int(rows[-1][0]) > 40
     assert all(float(f) == 0 for _, _, f in rows)
-    assert "new cell 277" not in out.stdout.split("cycle 1:", 1)[1]   # a tracked cell is on the skip list
+    assert "new cell 277" not in out.split("cycle 1:", 1)[1]   # a tracked cell is on the skip list
+    blocks = re.findall(r"  cell 277  ports 2 .*\n    UOS pwr +[-0-9.]+ dB\n((?:    P\d .*\n)+)    S  SP/NP/SNR .*\n",
+                        expert)
+    assert len(blocks) >= 3, expert
+    for b in blocks:
+        ports = re.findall(r"    P(\d) SP/NP/SNR +[-0-9.]+/ *[-0-9.]+/ *[-0-9.]+ dB  CB (\d+ kHz|>990 kHz)\n", b)
+        assert [p for p, _ in ports] == ["0", "1"], b
+    plain = [ln for ln in expert.splitlines() if not re.match(r"    (UOS pwr|P\d SP/NP/SNR|S  SP/NP/SNR) ", ln)]
+    assert plain == out.splitlines()
