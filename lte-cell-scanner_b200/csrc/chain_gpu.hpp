@@ -7,7 +7,6 @@ namespace lcs {
 
 struct ChainScratch {
   DevBuf<signed char> d_sss_tab;   // [168][3][2][62] +-1
-  bool getce_attr_set = false;
   DevBuf<double2> d_pss_fd;        // [3][62]
   DevBuf<int> d_starts;
   DevBuf<double> d_kseg;           // per-segment / per-cell frequency-shift constant
