@@ -11,6 +11,7 @@ sys.path.insert(0, os.path.join(ROOT, "track_oracle"))
 
 import lte_dl_synth as S  # noqa: E402
 from test_channelizer_host import auto_gain_oracle, chan_oracle, n_outputs, quantise  # noqa: E402
+from test_search_chain_gpu import same_cells  # noqa: E402
 
 N_CAP = 153600
 
@@ -301,9 +302,8 @@ def test_device_sweep_equals_host_sweep(lcs, ctx, synthetic_sweep):
     b = sw.search_cu8(host, fcs, s["f_set"], max_cells=16)
     sw.close()
     assert sum(len(x) for x in a) >= 2
-    def record(c):   # every field, doubles by their bits (NaN sentinels included); struct padding is not compared
-        return tuple(np.float64(v).tobytes() if isinstance(v, float) else v for v in c.as_dict().values())
-    assert [[record(c) for c in x] for x in a] == [[record(c) for c in x] for x in b]
+    for x, y in zip(a, b, strict=True):
+        same_cells(x, y)
 
 
 @pytest.mark.gpu

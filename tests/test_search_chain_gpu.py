@@ -14,25 +14,72 @@ every FOC phase that scales with fs*k is exercised with a factor that is not 1:
       different numbers of PSS positions.
   E   frame_start on each side of the -0.5 / 19199.5 wrap, and on each side of extract_tfg's one-frame step back.
 
-Tolerances are those of test_gpu_parity.py: ids, CP type, peak indices and MIB fields exact, FP64 stages to 1e-9 or better."""
+Found cells and peaks are compared field by field (compare_cells, used by the other search tests too), the FP64 stages'
+intermediates to 1e-8 of their largest magnitude or better."""
+import contextlib
+import ctypes as C
 import os
 import sys
 
 import numpy as np
 import pytest
 
+import lcs_b200
+import lcs_oracle
 from conftest import synth_cu8 as noise_cu8
 
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "track_oracle"))
 import lte_dl_synth as S  # noqa: E402
 
-pytestmark = pytest.mark.gpu
-
 FC = 739e6
 FS_LTE16 = 30720000.0 / 16
 TH2 = 3.0                  # THRESH2_N_SIGMA of CellSearch.cpp:528
-REL = 1e-6
-DISCRETE = ("n_id_1", "n_id_2", "cp_type", "ind", "n_ports", "n_rb_dl", "phich_duration", "phich_resource", "sfn")
+
+# Every field of lcs_cell is in exactly one of these classes: exact, within an absolute bound, or within a bound
+# relative to the oracle's value.
+EXACT = ("fc_requested", "fc_programmed", "freq", "ind", "n_id_1", "n_id_2", "cp_type", "n_ports", "n_rb_dl",
+         "phich_duration", "phich_resource", "sfn")
+ABS = {"frame_start": 1e-9, "freq_fine": 1e-6, "freq_superfine": 1e-6}
+REL = {"pss_pow": 1e-6}
+
+
+def bound(k, y):
+    """How far field k may lie from the oracle's value y.  A field in no class fails, so that a new field of lcs_cell
+    cannot go unchecked."""
+    if k in ABS:
+        return ABS[k]
+    if k in REL:
+        return REL[k] * abs(y)
+    if k not in EXACT:
+        pytest.fail(f"lcs_cell field {k} has no comparison class")
+    return 0
+
+
+def cell_fields(c):
+    """The field names of c's structure, those of its ctypes base classes first."""
+    return [k for t in reversed(type(c).__mro__) for k, _ in vars(t).get("_fields_", ())]
+
+
+def compare_cells(got, ref):
+    """Device cells or peaks against the oracle's: the same ones in the same order, then every field within its bound.
+    A double is NaN on both sides or on neither (peaks carry NaN frame_start and freq_*)."""
+    assert [(c.n_id_cell(), c.n_id_2, c.ind) for c in got] == [(c.n_id_cell(), c.n_id_2, c.ind) for c in ref]
+    for a, b in zip(got, ref):
+        for k in cell_fields(a):
+            x, y = getattr(a, k), getattr(b, k)
+            lim = bound(k, y)
+            if isinstance(y, float) and (np.isnan(x) or np.isnan(y)):
+                assert np.isnan(x) and np.isnan(y), k
+            else:
+                assert abs(x - y) <= lim, k
+
+
+def same_cells(a, b):
+    """Two device results bit for bit: every field, doubles by their bytes (NaNs included)."""
+    def record(c):
+        return tuple(np.float64(v).tobytes() if isinstance(v, float) else v for v in (getattr(c, k) for k in cell_fields(c)))
+    assert [record(c) for c in a] == [record(c) for c in b]
+
 
 A_CELL = dict(n_id_cell=137, n_ports=2, cp_type=1, n_rb_dl=50, phich_duration=1, phich_resource=2, t0=8900.0, sfn0=100)
 B_CELL = dict(n_id_cell=301, n_ports=4, cp_type=2, n_rb_dl=25, phich_duration=2, phich_resource=4, t0=12345.0, sfn0=7)
@@ -142,19 +189,37 @@ def scen(oracle):
     return Scenarios(oracle)
 
 
-def check_cells(got, ref):
-    assert [c.n_id_cell() for c in got] == [c.n_id_cell() for c in ref]
-    for a, b in zip(got, ref):
-        for k in DISCRETE:
-            assert getattr(a, k) == getattr(b, k), k
-        assert abs(a.frame_start - b.frame_start) < 1e-9
-        assert abs(a.freq_fine - b.freq_fine) < 1e-6 and abs(a.freq_superfine - b.freq_superfine) < 1e-6
+def test_compare_cells_classes():
+    """Every field of a cell and of a peak (NaN past n_id_2) moved just inside its bound passes compare_cells; moved just
+    past it, or NaN on one side only, it fails.  A field in no class fails with its name."""
+    assert lcs_b200.Cell._fields_ == lcs_oracle.Cell._fields_
+    cell = lcs_b200.Cell(fc_requested=FC, fc_programmed=FC - 3e3, pss_pow=2.5e3, ind=1410, freq=35e3, n_id_2=1, n_id_1=92,
+                         cp_type=1, frame_start=8898.62, freq_fine=35227.9, freq_superfine=35228.46, n_ports=2, n_rb_dl=50,
+                         phich_duration=1, phich_resource=2, sfn=100)
+    peak = lcs_b200.Cell(fc_requested=FC, fc_programmed=FC - 3e3, pss_pow=170.25, ind=6990, freq=-5e3, n_id_2=0, n_id_1=-1,
+                         frame_start=np.nan, freq_fine=np.nan, freq_superfine=np.nan, n_ports=-1, n_rb_dl=-1, sfn=-1)
+    ref = [cell, peak]
+    for i, c in enumerate(ref):
+        for k in cell_fields(c):
+            y = getattr(c, k)
+            if isinstance(y, int):
+                moves = [(y, True), (y + 1, False), (y - 1, False)]
+            elif np.isnan(y):
+                moves = [(y, True), (0.0, False)]
+            else:           # an exact double (bound 0) fails one ulp away
+                lim = bound(k, y)
+                moves = [(np.nan, False)] + [(y + s * 0.99 * lim, True) for s in (1, -1)]
+                moves += [(np.nextafter(y + s * 1.01 * lim, s * np.inf), False) for s in (1, -1)]
+            for v, ok in moves:
+                got = [type(x).from_buffer_copy(x) for x in ref]
+                setattr(got[i], k, v)
+                with contextlib.nullcontext() if ok else pytest.raises(AssertionError):
+                    compare_cells(got, ref)
 
-
-def check_peaks(got, ref):
-    assert [(p.n_id_2, p.ind, p.freq) for p in got] == [(p.n_id_2, p.ind, p.freq) for p in ref]
-    for a, b in zip(got, ref):
-        assert abs(a.pss_pow - b.pss_pow) < REL * b.pss_pow
+    class Wider(lcs_b200.Cell):
+        _fields_ = [("extra", C.c_int32)]
+    with pytest.raises(pytest.fail.Exception, match="field extra "):
+        compare_cells([Wider()], [Wider()])
 
 
 def check_stages(ctx, lcs, oracle, peak, cap, p):
@@ -217,6 +282,7 @@ def check_scenario_shape(name, peaks, cells, p, n_cap):
     return npss
 
 
+@pytest.mark.gpu
 @pytest.mark.parametrize("name", list(SCEN))
 def test_stages_per_peak(ctx, lcs, oracle, scen, name):
     """Every peak of the oracle's peak search through sss_detect, pss_sss_foe and extract_tfg on both sides."""
@@ -232,6 +298,7 @@ def test_stages_per_peak(ctx, lcs, oracle, scen, name):
         assert o.n_id_1 * 3 + o.n_id_2 == 137 and abs(o.frame_start - (t0 - 2) - 9600) < 2
 
 
+@pytest.mark.gpu
 @pytest.mark.parametrize("fmt", ["cu8", "c128"])
 @pytest.mark.parametrize("name", list(SCEN))
 def test_cell_search(ctx, scen, name, fmt):
@@ -240,10 +307,11 @@ def test_cell_search(ctx, scen, name, fmt):
     o_cells, o_peaks = scen.chain(name)
     buf = scen.cu8(name) if fmt == "cu8" else scen.cap(name)
     cells, peaks = ctx.cell_search(buf, p["f"], p["fcr"], p["fcp"], p["fs"])
-    check_peaks(peaks, o_peaks)
-    check_cells(cells, o_cells)
+    compare_cells(peaks, o_peaks)
+    compare_cells(cells, o_cells)
 
 
+@pytest.mark.gpu
 @pytest.mark.parametrize("name", ["B", "C_straddle", "D"])
 def test_cell_search_c128_not_8bit_exact(ctx, oracle, scen, name):
     """Samples scaled by 0.999 are no longer (u8-127)/128: the chain reads them as c128 and still equals the oracle."""
@@ -252,10 +320,11 @@ def test_cell_search_c128_not_8bit_exact(ctx, oracle, scen, name):
     o_cells, o_peaks = oracle.cell_search_one(cap, p["f"], p["fcr"], p["fcp"], p["fs"])
     assert sorted(c.n_id_cell() for c in o_cells) == p["ids"]
     cells, peaks = ctx.cell_search(cap, p["f"], p["fcr"], p["fcp"], p["fs"])
-    check_peaks(peaks, o_peaks)
-    check_cells(cells, o_cells)
+    compare_cells(peaks, o_peaks)
+    compare_cells(cells, o_cells)
 
 
+@pytest.mark.gpu
 def test_cell_search_batch_off_nominal_clock(ctx, lcs, oracle, scen):
     """lcs_cell_search_batch_cu8 with scenario B's clock: B between noise buffers, more buffers than one chunk."""
     p = scen.params("B")
@@ -269,7 +338,7 @@ def test_cell_search_batch_off_nominal_clock(ctx, lcs, oracle, scen):
     plan.close()
     for k, cells in zip(order, got):
         if k:
-            check_cells(cells, o_cells)
+            compare_cells(cells, o_cells)
         else:
             assert cells == []
 
@@ -286,6 +355,7 @@ def sweep_channels(scen):
                 fcp=np.array([p["fcp"], FC + 5e6, fc2 + 2000.0, fc2 + 1e6]), fs=p["fs"], f=p["f"], f_true=p["f_true"])
 
 
+@pytest.mark.gpu
 def test_sweep_search_off_nominal_clock(ctx, lcs, oracle, sweep_channels):
     """lcs_sweep_search_cu8 with fs_programmed and per-channel fc_programmed against the oracle's chain per channel."""
     ch = sweep_channels
@@ -295,11 +365,12 @@ def test_sweep_search_off_nominal_clock(ctx, lcs, oracle, sweep_channels):
     for i in range(len(ch["fcr"])):
         o_cells, _ = oracle.cell_search_one(S.to_c128(ch["iq"][i]), ch["f"], ch["fcr"][i], ch["fcp"][i], ch["fs"])
         assert [c.n_id_cell() for c in o_cells] == ([301] if i == 0 else [46] if i == 2 else [])
-        check_cells(got[i], o_cells)
+        compare_cells(got[i], o_cells)
         for a in got[i]:
             assert a.fc_requested == ch["fcr"][i] and a.fc_programmed == ch["fcp"][i]
 
 
+@pytest.mark.gpu
 def test_tracker_search_off_nominal_clock(ctx, lcs, oracle, sweep_channels):
     """lcs_tracker_search_cu8 and lcs_sweep_track_cu8 at the cells' offset (n_f = 1) against the oracle's chain at n_f = 1;
     frame_timing = frame_start*(FS_LTE/16)/(fs*k) + late with k = (fc_requested - offset)/fc_programmed."""
@@ -314,15 +385,15 @@ def test_tracker_search_off_nominal_clock(ctx, lcs, oracle, sweep_channels):
         o_cells, _ = oracle.cell_search_one(S.to_c128(ch["iq"][i]), np.array([off[i]]), fcr, fcp, fs)
         assert [c.n_id_cell() for c in o_cells] == ([301] if i == 0 else [46] if i == 2 else [])
         new = ctx.tracker_search_cu8(ch["iq"][i], off[i], fcr, fcp, fs, late[i])
-        check_cells([c for c, _ in new], o_cells)
+        compare_cells([c for c, _ in new], o_cells)
         k = (fcr - off[i]) / fcp
         for (c, ft), b in zip(new, o_cells):
             assert abs(ft - (b.frame_start * FS_LTE16 / (fs * k) + late[i])) < 1e-9
-        assert len(got[i]) == len(new)
-        for (a, fa), (b, fb) in zip(got[i], new):
-            assert a.as_dict() == b.as_dict() and fa == fb
+        same_cells([a for a, _ in got[i]], [b for b, _ in new])
+        assert [fa for _, fa in got[i]] == [fb for _, fb in new]
 
 
+@pytest.mark.gpu
 def test_grid_outside_the_buffer(ctx, lcs, oracle):
     """A buffer too short for one cell's 732-symbol extended-CP grid: that cell is dropped (extract_tfg raises), the other
     cell is still decoded and equals the oracle's chain, which is run only where its DFT windows lie inside the buffer."""
@@ -352,5 +423,5 @@ def test_grid_outside_the_buffer(ctx, lcs, oracle):
     assert dropped == [114] and [c.n_id_cell() for c in o_cells] == [250]
     for buf in (cu8, cap):
         got, peaks = ctx.cell_search(buf, p["f"], FC, FC, fs)
-        check_peaks(peaks, o_peaks)
-        check_cells(got, o_cells)
+        compare_cells(peaks, o_peaks)
+        compare_cells(got, o_cells)
