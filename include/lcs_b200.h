@@ -112,6 +112,9 @@ int lcs_xcorr_plan_kernel(const lcs_xcorr_plan* plan, int iq_format);   /* kerne
  *   d_pow           [batch][3][9600] double,  d_frq [batch][3][9600] int32   (row-major (t,idx))
  *   d_sp_incoherent [batch][9600] double
  *   d_incoherent_planar  optional [batch][3][n_f][9600] float (NULL = skip)
+ * Alignment (checked before any launch, LCS_ERR_ARG otherwise): d_iq to its sample size (2 bytes CU8, 8 CF32, 16 C128);
+ * d_single_planar, d_pow, d_frq and d_incoherent_planar to 16 bytes; d_sp_incoherent to 8 bytes.  cudaMalloc'd bases
+ * qualify; pointers into a tensor or buffer at other offsets may not.
  */
 lcs_status lcs_xcorr_pss_device(lcs_xcorr_plan* plan, const void* d_iq, int iq_format, uint32_t batch,
                                 float* d_single_planar, double* d_pow, int32_t* d_frq, double* d_sp_incoherent,

@@ -287,6 +287,13 @@ lcs_status planset_run(PlanSet& ps, int kernel, const void* d_iq, int iq_format,
   if (batch == 0) return fail(ctx, LCS_ERR_ARG, "xcorr_pss_device: empty batch");
   if (iq_format != LCS_IQ_CF32 && iq_format != LCS_IQ_CU8 && iq_format != LCS_IQ_C128)
     return fail(ctx, LCS_ERR_ARG, "xcorr_pss_device: bad iq_format");
+  // every kernel loads a whole sample at a time (uchar2 / float2 / double2); the epilogue reads `single` as float4 and
+  // writes incoherent / pow / frq as float4 / double2 / int4; sp_fold_kernel stores single doubles
+  if ((uintptr_t)d_iq % iq_sample_bytes(iq_format) != 0)
+    return fail(ctx, LCS_ERR_ARG, "xcorr_pss_device: IQ pointer not aligned to its sample size");
+  if ((((uintptr_t)d_single | (uintptr_t)d_pow | (uintptr_t)d_frq | (uintptr_t)d_inc) & 15) != 0)
+    return fail(ctx, LCS_ERR_ARG, "xcorr_pss_device: single, pow, frq and incoherent need 16-byte aligned pointers");
+  if (((uintptr_t)d_spi & 7) != 0) return fail(ctx, LCS_ERR_ARG, "xcorr_pss_device: sp_incoherent needs an 8-byte aligned pointer");
   int kern = planset_resolve_kernel(ps, kernel, iq_format);
   // the tensor-core kernel stages raw bytes with 16-byte bulk copies: an unaligned base pointer goes to the FP32 kernel
   if (kern == LCS_KERNEL_TC && kernel == LCS_KERNEL_AUTO && ((uintptr_t)d_iq & 15) != 0) kern = LCS_KERNEL_FP32;
