@@ -38,8 +38,10 @@ enum {
   LCS_ERR_STATE = 4
 };
 
-/* IQ sample formats accepted by the device / batch entry points */
-enum { LCS_IQ_CF32 = 0, LCS_IQ_CU8 = 1, LCS_IQ_C128 = 2 };
+/* IQ sample formats.  The correlator and search entry points take CF32, CU8 and C128 and reject CI16 and CS8 (LCS_ERR_ARG);
+ * CI16 (interleaved little-endian int16) and CS8 (int8) are input formats of lcs_chan_create_rational, which also takes
+ * CU8 and CF32. */
+enum { LCS_IQ_CF32 = 0, LCS_IQ_CU8 = 1, LCS_IQ_C128 = 2, LCS_IQ_CI16 = 3, LCS_IQ_CS8 = 4 };
 
 /* Which correlator kernel a plan uses.  AUTO picks the fastest one that is exact for the input
  * format (DESIGN.md "kernels"). */
@@ -360,6 +362,34 @@ lcs_status lcs_chan_push_ci16(lcs_chan* chan, const int16_t* iq_host, uint32_t n
 /* Summed device time of the channelizer kernel (CUDA events around each launch, ms) and the number of launches since
  * the last read; resets both. */
 lcs_status lcs_chan_timing_read(lcs_chan* chan, double* kernel_ms, uint64_t* launches);
+
+/* ---- rational resampling: any SDR rate, ci16 / cs8 / cu8 / cf32 input (DESIGN.md section 4.7) ------------------------ */
+/* The same lcs_chan, created at any allowed rate and sample format; lcs_chan_n_out, lcs_chan_gain, lcs_chan_timing_read
+ * and lcs_chan_destroy serve it unchanged.
+ *   fs_in  an integer number of Hz (within 1e-6), 1.92 MHz < fs_in <= 122.88 MHz, with fs_in / 1 920 000 = down / up in
+ *          lowest terms, up <= 128, down <= 640 (2.048, 2.4, 2.5, 6, 10, 12.5, 20, 25, 56, 100 Msps and every D * 1.92
+ *          MHz, D <= 64, are allowed); channels, offsets and gains as in section 4.6.  Anything else is LCS_ERR_ARG.
+ *   input  iq_format LCS_IQ_CI16: (I + jQ)/32768; LCS_IQ_CS8: (I + jQ)/128; LCS_IQ_CU8: ((I-127) + j(Q-127))/128;
+ *          LCS_IQ_CF32: I + jQ.  The mixer is that of section 4.6.
+ *   filter h: the section 4.6 design at F = up * fs_in (grid every F/(64L) or denser), DC gain up, so each of the up
+ *          polyphase branches has unit gain; at up = 1 exactly lcs_chan_design_taps(fs_in).
+ *   output y_c[n] = sum_i h[n*down - i*up + M] x~_c[i] over 0 <= n*down - i*up + M <= 2M (x~ = 0 before the stream
+ *          starts); output n belongs to input instant n*down/up and is emitted once input floor((n*down + M)/up) has
+ *          been pushed: after N samples there are max(0, floor((N*up - M - 1)/down) + 1) outputs.  Any sequence of
+ *          pushes gives bitwise the bytes of one push.  Bytes, clip counts, gain and auto gain as in section 4.6.
+ *   At up = 1 with CI16 the channelizer is lcs_chan_create's (the same bytes, clip counts and auto gain). */
+/* host only: fs_in / 1.92e6 = down / up in lowest terms and the prototype at up * fs_in (taps NULL: query *n_taps; on
+ * input, the capacity of taps) */
+lcs_status lcs_chan_design_rational(double fs_in, uint32_t* up, uint32_t* down, float* taps, uint32_t* n_taps);
+lcs_status lcs_chan_create_rational(lcs_ctx* ctx, double fs_in, int iq_format, double fc_in, uint32_t n_ch,
+                                    const double* fc_ch, const float* gain /*[n_ch] or NULL*/, lcs_chan** out);
+/* lcs_chan_push_ci16 / lcs_chan_auto_gain_ci16 with the samples in the channelizer's own format ([n][2] of int16, int8,
+ * uint8 or float); also valid on an lcs_chan_create channelizer (ci16).  lcs_chan_push_ci16 and lcs_chan_auto_gain_ci16
+ * on a channelizer whose format is not CI16 return LCS_ERR_ARG before any launch.  The device output feeds
+ * lcs_sweep_search_cu8_device unchanged. */
+lcs_status lcs_chan_push(lcs_chan* chan, const void* iq_host, uint32_t n_in, uint8_t* out, uint32_t out_capacity,
+                         int out_on_device, uint32_t* n_out, uint64_t* n_clipped);
+lcs_status lcs_chan_auto_gain(lcs_chan* chan, const void* iq_host, uint32_t n);
 
 /* lcs_sweep_search_cu8 on capture buffers already in device memory (e.g. a channelizer's output): d_iq is cu8
  * [n_ch][n_cap][2], 16-byte aligned, and is read in place (no copy).  Same arguments and results otherwise. */

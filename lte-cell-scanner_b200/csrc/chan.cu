@@ -8,9 +8,15 @@
 // read 32 consecutive words for every tap) and runs 32 channels over it: each warp 4 channels x 128 outputs, each lane 4
 // outputs x 4 channels in registers.  The epilogue applies the output rotation (FP64, exact integer phase), the gain, the
 // round-to-nearest-even quantisation and the clip count.
+//
+// rchan_kernel (DESIGN.md section 4.7) generalises this to rational resampling by up / down from any allowed integer-Hz
+// rate and to ci16, cs8, cu8 and cf32 input; lcs_chan_create_rational builds the same lcs_chan for it.
+#include <climits>
 #include <cmath>
+#include <complex>
 #include <cstring>
 #include <new>
+#include <numeric>
 #include <type_traits>
 #include <vector>
 
@@ -250,6 +256,290 @@ static bool decimation(double fs_in, int* D) {
   return true;
 }
 
+// ---- rational resampling: any integer-Hz rate, ci16 / cs8 / cu8 / cf32 input (DESIGN.md section 4.7) -----------------
+//
+// Output n sums h[n*down - i*up + M] x~[i]: with q = n*down + M, its newest input is i_hi = q / up and its taps are branch
+// phi = q mod up of the polyphase filter, g_phi[j] = h[phi + j*up] (zero past 2M), applied to x~[i_hi - j], j < J.  The
+// mixer folds into the taps as in chan_kernel, referred to the newest input: x~[i_hi - j] = exp(-j2pi p[i_hi]/fs) *
+// x[i_hi - j] exp(+j2pi (j*delta mod fs)/fs).  A CTA covers the outputs n0 + up*m + r of 32*RM consecutive m and every
+// r < up; a lane's register slot fixes (m / 32, r), so all 32 lanes of a warp use one branch (warp-uniform tap loads) and
+// read inputs `down` apart, which the tile staged in polyphase order modulo `down` turns into consecutive words.
+constexpr int RMAX_UP = 128, RMAX_DOWN = 640;
+constexpr int RMAX_TAPS = 16385;
+constexpr int RSMEM_CAP = 227 * 1024;    // the opt-in maximum of an H100 CTA; one fixed attribute for every channelizer
+
+struct RParams {
+  const unsigned char* in;     // samples in the input format; local sample 0 is stream sample i_hi(n0) - (J-1)
+  long long n_in;              // valid samples at `in` (later ones read as 0; no valid output uses them)
+  int up, down, J, RM, qlen;
+  long long q0;                // n0*down + M
+  int n_out;                   // outputs of this launch
+  long long n0;                // stream index of local output 0
+  int n_ch;
+  const float2* taps;          // [n_ch][up][J] complex branch taps g_phi[j] * exp(+j2pi (j*delta mod fs)/fs)
+  const double2* taps64;       // the same in double (power mode)
+  const long long* dmod;       // [n_ch] delta mod fs
+  long long fs;
+  const float* gain;           // [n_ch]
+  unsigned char* out;          // [n_ch] rows of out_stride bytes; column 2*i is local output i
+  size_t out_stride;
+  unsigned long long* clip;    // [n_ch]
+  double* pw;                  // power mode: [n_ch][gridDim.x] sum |y|^2 per tile
+};
+
+// sample g of the input, converted exactly to float: ci16 / 32768, cs8 / 128, (cu8 - 127) / 128, cf32 as is
+template <int FMT>
+__device__ __forceinline__ float2 load_iq(const unsigned char* p, long long g) {
+  if constexpr (FMT == LCS_IQ_CI16) {
+    const int w = __ldg(reinterpret_cast<const int*>(p) + g);
+    return make_float2((float)(short)(w & 0xffff) * (1.f / 32768.f), (float)(short)(w >> 16) * (1.f / 32768.f));
+  } else if constexpr (FMT == LCS_IQ_CS8) {
+    const unsigned short w = __ldg(reinterpret_cast<const unsigned short*>(p) + g);
+    return make_float2((float)(signed char)(w & 0xff) * (1.f / 128.f), (float)(signed char)(w >> 8) * (1.f / 128.f));
+  } else if constexpr (FMT == LCS_IQ_CU8) {
+    const unsigned short w = __ldg(reinterpret_cast<const unsigned short*>(p) + g);
+    return make_float2((float)((int)(w & 0xff) - 127) * (1.f / 128.f), (float)((int)(w >> 8) - 127) * (1.f / 128.f));
+  } else {
+    return __ldg(reinterpret_cast<const float2*>(p) + g);
+  }
+}
+
+template <int FMT, bool POWER>
+__global__ void __launch_bounds__(THREADS) rchan_kernel(RParams P) {
+  extern __shared__ float2 xs[];                     // [down][qlen]
+  const int tile = blockIdx.x;
+  const int mt = 32 * P.RM;                          // m values of the tile
+  const long long j0 = (long long)tile * mt * P.down;
+  const long long c0q = P.q0 / P.up;
+  const int c_last = (int)((P.q0 + (long long)(P.up - 1) * P.down) / P.up - c0q);
+  const int span = (mt - 1) * P.down + c_last + P.J;
+  for (int j = threadIdx.x; j < span; j += THREADS) {
+    const long long g = j0 + j;
+    xs[(j % P.down) * P.qlen + j / P.down] = g < P.n_in ? load_iq<FMT>(P.in, g) : make_float2(0.f, 0.f);
+  }
+  __syncthreads();
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int c0 = blockIdx.y * CH_CTA + warp * CW;
+  if (c0 >= P.n_ch) return;
+  using V = typename std::conditional<POWER, double2, float2>::type;
+  const V* tp[CW];
+#pragma unroll
+  for (int i = 0; i < CW; i++) {
+    const size_t off = (size_t)min(c0 + i, P.n_ch - 1) * P.up * P.J;
+    if constexpr (POWER) tp[i] = P.taps64 + off; else tp[i] = P.taps + off;
+  }
+  double pws[CW];
+  unsigned clipped[CW];
+#pragma unroll
+  for (int i = 0; i < CW; i++) { pws[i] = 0; clipped[i] = 0; }
+  const int nslot = P.RM * P.up;                     // slot s: m / 32 = s / up, r = s % up
+  for (int s0 = 0; s0 < nslot; s0 += R) {
+    int ph[R], row[R], toff[R], nl[R];
+#pragma unroll
+    for (int k = 0; k < R; k++) {
+      const int s = min(s0 + k, nslot - 1);
+      const int mm = s / P.up, r = s % P.up;
+      const long long qr = P.q0 + (long long)r * P.down;
+      // tap j = J-1 reads local sample (32 mm + lane) * down + (c_r - c_0): phase e mod down, row lane + e / down
+      const int e = 32 * mm * P.down + (int)(qr / P.up - c0q);
+      ph[k] = e % P.down;
+      row[k] = e / P.down;
+      toff[k] = (int)(qr % P.up) * P.J;
+      nl[k] = s0 + k < nslot ? P.up * (tile * mt + 32 * mm + lane) + r : INT_MAX;
+    }
+    V acc[CW][R];
+#pragma unroll
+    for (int i = 0; i < CW; i++)
+#pragma unroll
+      for (int k = 0; k < R; k++) acc[i][k].x = acc[i][k].y = 0;
+    for (int j = P.J - 1; j >= 0; j--) {             // oldest input first, as chan_kernel
+      float2 x[R];
+#pragma unroll
+      for (int k = 0; k < R; k++) x[k] = xs[ph[k] * P.qlen + row[k] + lane];
+#pragma unroll
+      for (int i = 0; i < CW; i++)
+#pragma unroll
+        for (int k = 0; k < R; k++) cmac(acc[i][k], __ldg(tp[i] + toff[k] + j), x[k]);
+#pragma unroll
+      for (int k = 0; k < R; k++)
+        if (++ph[k] == P.down) { ph[k] = 0; row[k]++; }
+    }
+#pragma unroll
+    for (int i = 0; i < CW; i++) {
+      const int c = c0 + i;
+      if (c >= P.n_ch) break;
+#pragma unroll
+      for (int k = 0; k < R; k++) {
+        if (nl[k] >= P.n_out) continue;
+        if (POWER) {
+          pws[i] += (double)acc[i][k].x * acc[i][k].x + (double)acc[i][k].y * acc[i][k].y;
+          continue;
+        }
+        const long long ih = (P.q0 + (long long)nl[k] * P.down) / P.up;   // newest input of the output
+        const long long p = ((ih % P.fs) * P.dmod[c]) % P.fs;              // its exact mixer phase, in cycles * fs
+        double sn, cs;
+        sincospi(-2.0 * (double)p / (double)P.fs, &sn, &cs);
+        const double yr = (double)acc[i][k].x * cs - (double)acc[i][k].y * sn;
+        const double yi = (double)acc[i][k].x * sn + (double)acc[i][k].y * cs;
+        const double gn = 128.0 * (double)P.gain[c];
+        double vr = rint(127.0 + gn * yr), vi = rint(127.0 + gn * yi);
+        clipped[i] += (vr < 0 || vr > 255) + (vi < 0 || vi > 255);
+        vr = fmin(fmax(vr, 0.0), 255.0);
+        vi = fmin(fmax(vi, 0.0), 255.0);
+        unsigned char* o = P.out + (size_t)c * P.out_stride + 2 * (size_t)nl[k];
+        o[0] = (unsigned char)vr;
+        o[1] = (unsigned char)vi;
+      }
+    }
+  }
+#pragma unroll
+  for (int i = 0; i < CW; i++) {
+    const int c = c0 + i;
+    if (c >= P.n_ch) break;
+    if (POWER) {
+      double s = pws[i];
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) s += __shfl_down_sync(0xffffffffu, s, o);
+      if (lane == 0) P.pw[(size_t)c * gridDim.x + tile] = s;
+    } else {
+      const unsigned n = __reduce_add_sync(0xffffffffu, clipped[i]);
+      if (lane == 0 && n) atomicAdd(P.clip + c, (unsigned long long)n);
+    }
+  }
+}
+
+// In-place radix-2 FFT of a power-of-two length (forward, unnormalised); w[k] = exp(-j2pi k/(2 * a.size())).
+static void fft(std::vector<std::complex<double>>& a, const std::vector<std::complex<double>>& w) {
+  const size_t n = a.size();
+  for (size_t i = 1, j = 0; i < n; i++) {
+    size_t bit = n >> 1;
+    for (; j & bit; bit >>= 1) j ^= bit;
+    j ^= bit;
+    if (i < j) std::swap(a[i], a[j]);
+  }
+  for (size_t len = 2; len <= n; len <<= 1) {
+    const size_t half = len / 2, stride = 2 * n / len;
+    for (size_t i = 0; i < n; i += len)
+      for (size_t k = 0; k < half; k++) {
+        const std::complex<double> t = w[k * stride] * a[i + k + half];
+        a[i + k + half] = a[i + k] - t;
+        a[i + k] = a[i + k] + t;
+      }
+  }
+}
+
+// |X[k]|, k = 0..N/2, of the N-point DFT of the real taps h zero-padded: one N/2-point complex FFT of the even and odd
+// samples packed as real and imaginary parts.
+static std::vector<double> dft_magnitude(const std::vector<float>& h, size_t N) {
+  const size_t n2 = N / 2;
+  std::vector<std::complex<double>> w(n2), z(n2);
+  for (size_t k = 0; k < n2; k++) w[k] = std::polar(1.0, -2 * M_PI * (double)k / (double)N);
+  for (size_t n = 0; n < h.size(); n++)
+    if (n % 2) z[n / 2].imag((double)h[n]); else z[n / 2].real((double)h[n]);
+  fft(z, w);
+  std::vector<double> m(n2 + 1);
+  for (size_t k = 0; k <= n2; k++) {
+    const std::complex<double> a = z[k % n2], b = std::conj(z[(n2 - k) % n2]);
+    const std::complex<double> e = 0.5 * (a + b), o = std::complex<double>(0, -0.5) * (a - b);
+    m[k] = std::abs(e + (k < n2 ? w[k] : std::complex<double>(-1, 0)) * o);
+  }
+  return m;
+}
+
+// The spec of meets_spec for taps of DC gain `gain` at the rate F, on the grid of an FFT of the zero-padded taps (every
+// F/N, N the power of two >= 64L) plus the band edges 0.70 and 1.22 MHz.
+static bool meets_spec_fft(const std::vector<float>& h, double F, double gain) {
+  const int L = (int)h.size(), M = (L - 1) / 2;
+  size_t N = 1;
+  while (N < 64 * (size_t)L) N <<= 1;
+  const std::vector<double> a = dft_magnitude(h, N);
+  auto pass_ok = [&](double m) { return std::fabs(20 * std::log10(m / gain)) <= kPassDb; };
+  auto stop_ok = [&](double m) { return 20 * std::log10(m / gain + 1e-300) <= -kStopDb; };
+  for (size_t k = 0; k <= N / 2; k++) {
+    const double f = (double)k * F / (double)N, m = a[k];
+    if (f <= kPass && !pass_ok(m)) return false;
+    if (f >= kStop && !stop_ok(m)) return false;
+  }
+  auto resp = [&](double f) {   // h[M] + 2 sum h[M+m] cos(m theta), as meets_spec
+    double s = h[M];
+    for (int m = 1; m <= M; m++) s += 2.0 * (double)h[M + m] * std::cos(2 * M_PI * f * m / F);
+    return std::fabs(s);
+  };
+  return pass_ok(resp(kPass)) && stop_ok(resp(kStop));
+}
+
+// Kaiser-windowed sinc of odd length L at the rate F with DC gain `gain` (the rounding of kaiser_sinc, scaled in double).
+static void kaiser_sinc_gain(int L, double F, double gain, std::vector<float>& out) {
+  const int M = (L - 1) / 2;
+  const double beta = kaiser_beta(), i0b = bessel_i0(beta), fcn = 2 * kCut / F;
+  std::vector<double> h(L);
+  double sum = 0;
+  for (int n = 0; n < L; n++) {
+    const int m = n - M;
+    const double a = L > 1 ? 2.0 * n / (L - 1) - 1.0 : 0.0;
+    const double w = bessel_i0(beta * std::sqrt(std::max(0.0, 1 - a * a))) / i0b;
+    const double s = m == 0 ? fcn : std::sin(M_PI * fcn * m) / (M_PI * m);
+    h[n] = s * w;
+    sum += h[n];
+  }
+  out.resize(L);
+  for (int n = 0; n < L; n++) out[n] = (float)(gain * h[n] / sum);
+}
+
+// The prototype for fs_in = 1.92 MHz * down / up at F = up * fs_in, DC gain up.  up = 1 is design() itself; otherwise the
+// shortest odd length about the Kaiser estimate that meets the spec on the FFT grid and whose length - 2 fails it,
+// found by doubling steps and bisection (the spec holds from some length on), so that L ~ 10 000 takes a few FFTs.
+static int design_rational(long long fs_in, int up, std::vector<float>& h) {
+  if (up == 1) return design((double)fs_in, h);
+  const double F = (double)up * (double)fs_in, gain = up;
+  auto ok = [&](int L, std::vector<float>& g) {
+    kaiser_sinc_gain(L, F, gain, g);
+    return meets_spec_fft(g, F, gain);
+  };
+  const double dw = 2 * M_PI * (kStop - kPass) / F;
+  int L = ((int)std::ceil((kStopDb - 8.0) / (2.285 * dw)) + 1) | 1;
+  const int first_step = std::max(2, L / 64 / 2 * 2);   // the estimate is within a few per cent
+  std::vector<float> g;
+  int lo, hi;   // lo fails (or is 1), hi meets and h holds it
+  if (ok(L, h)) {
+    hi = L;
+    for (int step = first_step;; step *= 2) {
+      lo = hi - step;
+      if (lo < 3) { lo = 1; break; }
+      if (!ok(lo, g)) break;
+      hi = lo;
+      h.swap(g);
+    }
+  } else {
+    lo = L;
+    for (int step = first_step;; step *= 2) {
+      hi = std::min(lo + step, RMAX_TAPS);
+      if (ok(hi, h)) break;
+      if (hi == RMAX_TAPS) return 0;
+      lo = hi;
+    }
+  }
+  while (hi - lo > 2) {
+    const int mid = lo + 2 * std::max(1, (hi - lo) / 4);
+    if (ok(mid, g)) { hi = mid; h.swap(g); } else lo = mid;
+  }
+  return hi;
+}
+
+// fs_in an integer number of Hz in (1.92 MHz, 122.88 MHz] with fs_in / 1.92 MHz = down / up in lowest terms,
+// up <= 128, down <= 640
+static bool rational_rate(double fs_in, long long* fs, int* up, int* down) {
+  if (!std::isfinite(fs_in)) return false;
+  const double r = std::round(fs_in);
+  if (std::fabs(fs_in - r) > 1e-6 || !(r > kFsCh) || r > 64 * kFsCh) return false;
+  const long long f = (long long)r, g = std::gcd(f, 1920000LL);
+  if (1920000LL / g > RMAX_UP || f / g > RMAX_DOWN) return false;
+  *fs = f;
+  *up = (int)(1920000LL / g);
+  *down = (int)(f / g);
+  return true;
+}
+
 }  // namespace chn
 }  // namespace lcs
 
@@ -275,6 +565,12 @@ struct lcs_chan {
   uint32_t chunk = TILE;                 // outputs per launch (bounds the device scratch)
   std::vector<int> carry;                // stream samples [n_out*D - M, n_in) (zeros before the stream starts)
   uint64_t n_in = 0, n_out = 0;
+  // rational channelizer (lcs_chan_create_rational other than up = 1 with ci16, which is an lcs_chan_create one): D is
+  // unused, taps are [n_ch][up][J], step holds delta mod fs, and the carry is raw samples of esz bytes
+  bool rat = false;
+  int fmt = LCS_IQ_CI16, esz = 4, up = 1, down = 0, J = 0, RM = 1;
+  std::vector<unsigned char> rcarry;     // stream samples [i_hi(n_out) - (J-1), n_in) (zeros before the stream starts)
+  DevBuf<unsigned char> d_rin;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   double kernel_ms = 0;
   uint64_t kernel_launches = 0;
@@ -361,6 +657,172 @@ lcs_status run(lcs_chan* c, const int* a, size_t na, const int* b, size_t nb, ui
 }
 
 lcs_status cfail(const lcs_chan* c, const char* msg) { return fail(c ? c->ctx : nullptr, LCS_ERR_ARG, msg); }
+
+// ---- rational channelizer ----
+// newest input of output n, and the first input the outputs from n on need
+long long r_ihi(const lcs_chan* c, uint64_t n) { return (long long)((n * c->down + c->M) / c->up); }
+long long r_first(const lcs_chan* c, uint64_t n) { return r_ihi(c, n) - (c->J - 1); }
+uint64_t r_outputs_after(const lcs_chan* c, uint64_t n) {
+  const uint64_t q = n * c->up;
+  return q >= (uint64_t)c->M + 1 ? (q - 1 - c->M) / c->down + 1 : 0;
+}
+uint64_t chan_outputs_after(const lcs_chan* c, uint64_t n) { return c->rat ? r_outputs_after(c, n) : outputs_after(c->D, c->M, n); }
+// n samples of value 0 in the channelizer's format (cu8 127)
+std::vector<unsigned char> r_zeros(const lcs_chan* c, size_t n) {
+  return std::vector<unsigned char>(n * c->esz, c->fmt == LCS_IQ_CU8 ? 127 : 0);
+}
+int r_outputs_per_tile(const lcs_chan* c) { return 32 * c->RM * c->up; }
+size_t r_smem(int up, int down, int J, int RM) {   // the tile: down rows of qlen samples
+  const size_t span_max = (size_t)32 * RM * down + J;
+  return (size_t)down * ((span_max + down - 1) / down) * sizeof(float2);
+}
+
+template <int FMT>
+void r_launch(bool power, dim3 grid, size_t smem, cudaStream_t st, const RParams& P) {
+  if (power)
+    rchan_kernel<FMT, true><<<grid, THREADS, smem, st>>>(P);
+  else
+    rchan_kernel<FMT, false><<<grid, THREADS, smem, st>>>(P);
+}
+
+template <int FMT>
+cudaError_t r_set_smem() {
+  cudaError_t e = cudaFuncSetAttribute(rchan_kernel<FMT, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, RSMEM_CAP);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(rchan_kernel<FMT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, RSMEM_CAP);
+  return e;
+}
+
+// run() for a rational channelizer: outputs [0, n_out) of the virtual input a ++ b (raw samples), whose sample 0 is the
+// first input of output 0 (stream output n_abs0).
+lcs_status run_r(lcs_chan* c, const unsigned char* a, size_t na, const unsigned char* b, size_t nb, uint64_t n_abs0,
+                 uint64_t n_out, bool power, unsigned char* out, size_t out_stride, bool out_dev, std::vector<double>* pw_sum) {
+  lcs_ctx* ctx = c->ctx;
+  cudaStream_t st = ctx->streams[0];
+  const int T = r_outputs_per_tile(c);
+  const size_t es = c->esz;
+  const size_t span_max = (size_t)c->chunk * c->down / c->up + c->J + 2;
+  LCS_CUDA(ctx, c->d_rin.ensure(span_max * es));
+  if (!power && !out_dev) LCS_CUDA(ctx, c->d_out.ensure((size_t)c->n_ch * c->chunk * 2));
+  if (power) LCS_CUDA(ctx, c->d_pw.ensure((size_t)c->n_ch * ((c->chunk + T - 1) / T)));
+  const size_t smem = r_smem(c->up, c->down, c->J, c->RM);
+  const long long base = r_first(c, n_abs0);
+  std::vector<double> pw;
+  for (uint64_t e0 = 0; e0 < n_out; e0 += c->chunk) {
+    const uint32_t ne = (uint32_t)std::min<uint64_t>(c->chunk, n_out - e0);
+    const uint64_t n0 = n_abs0 + e0;
+    const size_t lo = (size_t)(r_first(c, n0) - base);
+    const size_t hi = std::min((size_t)(r_ihi(c, n0 + ne - 1) + 1 - base), na + nb);
+    if (lo < na) LCS_CUDA(ctx, cudaMemcpyAsync(c->d_rin.p, a + lo * es, (std::min(hi, na) - lo) * es, cudaMemcpyHostToDevice, st));
+    if (hi > na) {
+      const size_t s = std::max(lo, na);
+      LCS_CUDA(ctx, cudaMemcpyAsync(c->d_rin.p + (s - lo) * es, b + (s - na) * es, (hi - s) * es, cudaMemcpyHostToDevice, st));
+    }
+    RParams P;
+    P.in = c->d_rin.p;
+    P.n_in = (long long)(hi - lo);
+    P.up = c->up;
+    P.down = c->down;
+    P.J = c->J;
+    P.RM = c->RM;
+    P.qlen = (int)(smem / sizeof(float2) / c->down);
+    P.q0 = (long long)(n0 * c->down + c->M);
+    P.n_out = (int)ne;
+    P.n0 = (long long)n0;
+    P.n_ch = (int)c->n_ch;
+    P.taps = c->d_taps.p;
+    P.taps64 = c->d_taps64.p;
+    P.dmod = c->d_step.p;
+    P.fs = c->fs;
+    P.gain = c->d_gain.p;
+    P.out = out_dev ? out + 2 * e0 : c->d_out.p;
+    P.out_stride = out_dev ? out_stride : (size_t)ne * 2;
+    P.clip = c->d_clip.p;
+    P.pw = c->d_pw.p;
+    const dim3 grid((ne + T - 1) / T, (c->n_ch + CH_CTA - 1) / CH_CTA);
+    LCS_CUDA(ctx, cudaEventRecord(c->ev0, st));
+    switch (c->fmt) {
+      case LCS_IQ_CI16: r_launch<LCS_IQ_CI16>(power, grid, smem, st, P); break;
+      case LCS_IQ_CS8: r_launch<LCS_IQ_CS8>(power, grid, smem, st, P); break;
+      case LCS_IQ_CU8: r_launch<LCS_IQ_CU8>(power, grid, smem, st, P); break;
+      default: r_launch<LCS_IQ_CF32>(power, grid, smem, st, P); break;
+    }
+    ctx->launches++;
+    LCS_CUDA(ctx, cudaGetLastError());
+    LCS_CUDA(ctx, cudaEventRecord(c->ev1, st));
+    if (power) {
+      pw.resize((size_t)c->n_ch * grid.x);
+      LCS_CUDA(ctx, cudaMemcpyAsync(pw.data(), c->d_pw.p, pw.size() * 8, cudaMemcpyDeviceToHost, st));
+    } else if (!out_dev) {
+      LCS_CUDA(ctx, cudaMemcpy2DAsync(out + 2 * e0, out_stride, c->d_out.p, (size_t)ne * 2, (size_t)ne * 2, c->n_ch,
+                                      cudaMemcpyDeviceToHost, st));
+    }
+    LCS_CUDA(ctx, cudaStreamSynchronize(st));
+    float ms = 0;
+    LCS_CUDA(ctx, cudaEventElapsedTime(&ms, c->ev0, c->ev1));
+    c->kernel_ms += ms;
+    c->kernel_launches++;
+    if (power)   // fixed order: tiles of a chunk, chunks in stream order
+      for (uint32_t ch = 0; ch < c->n_ch; ch++)
+        for (uint32_t t = 0; t < grid.x; t++) (*pw_sum)[ch] += pw[(size_t)ch * grid.x + t];
+  }
+  return LCS_OK;
+}
+
+lcs_status r_push(lcs_chan* c, const void* iq_host, uint32_t n_in, uint8_t* out, uint32_t out_capacity, int out_on_device,
+                  uint32_t* n_out, uint64_t* n_clipped) {
+  if ((!iq_host && n_in) || !n_out) return cfail(c, "lcs_chan_push: null pointer");
+  const uint64_t k = r_outputs_after(c, c->n_in + n_in) - c->n_out;
+  if (k > out_capacity) return cfail(c, "lcs_chan_push: out_capacity is smaller than the outputs of this push");
+  if (k && !out) return cfail(c, "lcs_chan_push: null output");
+  LCS_CUDA(c->ctx, cudaSetDevice(c->ctx->device));
+  LCS_CUDA(c->ctx, cudaMemsetAsync(c->d_clip.p, 0, c->n_ch * 8, c->ctx->streams[0]));
+  const unsigned char* b = static_cast<const unsigned char*>(iq_host);
+  const size_t es = c->esz, na = c->rcarry.size() / es;
+  if (k) {
+    lcs_status rc = run_r(c, c->rcarry.data(), na, b, n_in, c->n_out, k, false, out, (size_t)out_capacity * 2,
+                          out_on_device != 0, nullptr);
+    if (rc != LCS_OK) return rc;
+  }
+  // keep the samples from the first input of the next output on
+  const size_t drop = (size_t)(r_first(c, c->n_out + k) - r_first(c, c->n_out));
+  std::vector<unsigned char> nc;
+  nc.reserve((na + n_in - drop) * es);
+  if (drop < na) nc.insert(nc.end(), c->rcarry.begin() + drop * es, c->rcarry.end());
+  nc.insert(nc.end(), b + (drop > na ? drop - na : 0) * es, b + (size_t)n_in * es);
+  c->rcarry.swap(nc);
+  c->n_in += n_in;
+  c->n_out += k;
+  *n_out = (uint32_t)k;
+  if (n_clipped) {
+    if (k)
+      LCS_CUDA(c->ctx, cudaMemcpy(n_clipped, c->d_clip.p, c->n_ch * 8, cudaMemcpyDeviceToHost));
+    else
+      std::memset(n_clipped, 0, c->n_ch * 8);
+  }
+  return LCS_OK;
+}
+
+lcs_status r_auto_gain(lcs_chan* c, const void* iq_host, uint32_t n) {
+  if (!iq_host) return cfail(c, "lcs_chan_auto_gain: null samples");
+  const uint64_t n_out = r_outputs_after(c, n);           // what a fresh channelizer would produce
+  if (n_out == 0) return cfail(c, "lcs_chan_auto_gain: fewer samples than one output needs");
+  LCS_CUDA(c->ctx, cudaSetDevice(c->ctx->device));
+  const std::vector<unsigned char> zeros = r_zeros(c, (size_t)-r_first(c, 0));
+  std::vector<double> sum(c->n_ch, 0.0);
+  lcs_status rc = run_r(c, zeros.data(), zeros.size() / c->esz, static_cast<const unsigned char*>(iq_host), n, 0, n_out,
+                        true, nullptr, 0, false, &sum);
+  if (rc != LCS_OK) return rc;
+  for (uint32_t ch = 0; ch < c->n_ch; ch++) {
+    const double ms = sum[ch] / (double)n_out;
+    c->gain[ch] = ms > 0 ? (float)(0.25 / std::sqrt(ms)) : 1.0f;
+  }
+  LCS_CUDA(c->ctx, cudaMemcpy(c->d_gain.p, c->gain.data(), c->n_ch * 4, cudaMemcpyHostToDevice));
+  return LCS_OK;
+}
+
+size_t r_sample_bytes(int fmt) {
+  return fmt == LCS_IQ_CI16 ? 4 : fmt == LCS_IQ_CS8 || fmt == LCS_IQ_CU8 ? 2 : fmt == LCS_IQ_CF32 ? 8 : 0;
+}
 
 }  // namespace
 
@@ -456,6 +918,10 @@ void lcs_chan_destroy(lcs_chan* c) {
 
 lcs_status lcs_chan_auto_gain_ci16(lcs_chan* c, const int16_t* iq_host, uint32_t n) {
   if (!c) return LCS_ERR_ARG;
+  if (c->rat) {
+    if (c->fmt != LCS_IQ_CI16) return cfail(c, "lcs_chan_auto_gain_ci16: the channelizer's input format is not ci16");
+    return r_auto_gain(c, iq_host, n);
+  }
   if (!iq_host) return cfail(c, "lcs_chan_auto_gain_ci16: null samples");
   const uint64_t n_out = outputs_after(c->D, c->M, n);      // what a fresh channelizer would produce
   if (n_out == 0) return cfail(c, "lcs_chan_auto_gain_ci16: fewer samples than one output needs");
@@ -482,7 +948,7 @@ lcs_status lcs_chan_gain(const lcs_chan* c, float* gain) {
 lcs_status lcs_chan_n_out(const lcs_chan* c, uint64_t n_in, uint32_t* n_out) {
   if (!c) return LCS_ERR_ARG;
   if (!n_out) return cfail(c, "lcs_chan_n_out: null pointer");
-  const uint64_t k = outputs_after(c->D, c->M, c->n_in + n_in) - c->n_out;
+  const uint64_t k = chan_outputs_after(c, c->n_in + n_in) - c->n_out;
   if (k > UINT32_MAX) return cfail(c, "lcs_chan_n_out: push too long");
   *n_out = (uint32_t)k;
   return LCS_OK;
@@ -491,6 +957,10 @@ lcs_status lcs_chan_n_out(const lcs_chan* c, uint64_t n_in, uint32_t* n_out) {
 lcs_status lcs_chan_push_ci16(lcs_chan* c, const int16_t* iq_host, uint32_t n_in, uint8_t* out, uint32_t out_capacity,
                               int out_on_device, uint32_t* n_out, uint64_t* n_clipped) {
   if (!c) return LCS_ERR_ARG;
+  if (c->rat) {
+    if (c->fmt != LCS_IQ_CI16) return cfail(c, "lcs_chan_push_ci16: the channelizer's input format is not ci16");
+    return r_push(c, iq_host, n_in, out, out_capacity, out_on_device, n_out, n_clipped);
+  }
   if ((!iq_host && n_in) || !n_out) return cfail(c, "lcs_chan_push_ci16: null pointer");
   const uint64_t k = outputs_after(c->D, c->M, c->n_in + n_in) - c->n_out;
   if (k > out_capacity) return cfail(c, "lcs_chan_push_ci16: out_capacity is smaller than the outputs of this push");
@@ -520,6 +990,136 @@ lcs_status lcs_chan_push_ci16(lcs_chan* c, const int16_t* iq_host, uint32_t n_in
       std::memset(n_clipped, 0, c->n_ch * 8);
   }
   return LCS_OK;
+}
+
+lcs_status lcs_chan_design_rational(double fs_in, uint32_t* up, uint32_t* down, float* taps, uint32_t* n_taps) {
+  long long fs = 0;
+  int u = 0, d = 0;
+  if (!up || !down || !n_taps || !rational_rate(fs_in, &fs, &u, &d))
+    return fail(nullptr, LCS_ERR_ARG, "lcs_chan_design_rational: fs_in must be an integer number of Hz in (1.92, 122.88] MHz "
+                                      "with fs_in / 1.92 MHz = down / up, up <= 128, down <= 640");
+  std::vector<float> h;
+  const int L = design_rational(fs, u, h);
+  if (!L) return fail(nullptr, LCS_ERR_RANGE, "lcs_chan_design_rational: no filter up to the tap limit meets the spec");
+  if (taps) {
+    if (*n_taps < (uint32_t)L) return fail(nullptr, LCS_ERR_ARG, "lcs_chan_design_rational: taps array too short");
+    std::memcpy(taps, h.data(), L * sizeof(float));
+  }
+  *up = (uint32_t)u;
+  *down = (uint32_t)d;
+  *n_taps = (uint32_t)L;
+  return LCS_OK;
+}
+
+lcs_status lcs_chan_create_rational(lcs_ctx* ctx, double fs_in, int iq_format, double fc_in, uint32_t n_ch,
+                                    const double* fc_ch, const float* gain, lcs_chan** out) {
+  if (!ctx || !out || !fc_ch) return fail(ctx, LCS_ERR_ARG, "lcs_chan_create_rational: null argument");
+  long long fs = 0;
+  int up = 0, down = 0;
+  if (!rational_rate(fs_in, &fs, &up, &down))
+    return fail(ctx, LCS_ERR_ARG, "lcs_chan_create_rational: fs_in must be an integer number of Hz in (1.92, 122.88] MHz "
+                                  "with fs_in / 1.92 MHz = down / up, up <= 128, down <= 640");
+  const size_t esz = r_sample_bytes(iq_format);
+  if (!esz) return fail(ctx, LCS_ERR_ARG, "lcs_chan_create_rational: iq_format must be LCS_IQ_CI16, CS8, CU8 or CF32");
+  if (n_ch < 1 || n_ch > 1024) return fail(ctx, LCS_ERR_ARG, "lcs_chan_create_rational: n_ch must be in [1, 1024]");
+  if (!std::isfinite(fc_in)) return fail(ctx, LCS_ERR_ARG, "lcs_chan_create_rational: fc_in is not finite");
+  std::vector<long long> delta(n_ch);
+  for (uint32_t c = 0; c < n_ch; c++) {
+    const double d = fc_ch[c] - fc_in;
+    if (!std::isfinite(d) || std::fabs(d - std::round(d)) > 1e-6)
+      return fail(ctx, LCS_ERR_ARG, "lcs_chan_create_rational: channel offset fc_ch - fc_in is not an integer number of Hz");
+    delta[c] = (long long)std::llround(d);
+    if (2 * std::llabs(delta[c]) > fs - 1920000)
+      return fail(ctx, LCS_ERR_ARG, "lcs_chan_create_rational: channel band (+-0.96 MHz) outside the input band");
+    if (gain && !(std::isfinite(gain[c]) && gain[c] > 0))
+      return fail(ctx, LCS_ERR_ARG, "lcs_chan_create_rational: gain must be finite and > 0");
+  }
+  // D * 1.92 MHz ci16 is lcs_chan_create's channelizer, bytes, clip counts and auto gain included
+  if (up == 1 && iq_format == LCS_IQ_CI16) return lcs_chan_create(ctx, fs_in, fc_in, n_ch, fc_ch, gain, out);
+  lcs_chan* c = new (std::nothrow) lcs_chan();
+  if (!c) return fail(ctx, LCS_ERR_STATE, "lcs_chan_create_rational: out of memory");
+  c->ctx = ctx;
+  c->rat = true;
+  c->fmt = iq_format;
+  c->esz = (int)esz;
+  c->up = up;
+  c->down = down;
+  c->fs = fs;
+  c->n_ch = n_ch;
+  c->L = design_rational(fs, up, c->h);
+  if (!c->L) {
+    delete c;
+    return fail(ctx, LCS_ERR_RANGE, "lcs_chan_create_rational: no filter up to the tap limit meets the spec");
+  }
+  c->M = (c->L - 1) / 2;
+  c->J = 2 * c->M / up + 1;
+  c->RM = (R + up - 1) / up;                // the lane slots of a tile cover up * RM outputs per m
+  c->delta = delta;
+  c->gain.assign(n_ch, 1.0f);
+  if (gain) c->gain.assign(gain, gain + n_ch);
+  c->rcarry = r_zeros(c, (size_t)-r_first(c, 0));
+  if (r_smem(up, down, c->J, c->RM) > (size_t)RSMEM_CAP) {
+    delete c;
+    return fail(ctx, LCS_ERR_RANGE, "lcs_chan_create_rational: the input tile exceeds shared memory");
+  }
+  // outputs per launch, whole tiles: device output scratch <= 32 MB, input <= 64 MB
+  const uint64_t T = (uint64_t)r_outputs_per_tile(c);
+  const uint64_t by_out = (32ull << 20) / (2ull * n_ch), by_in = (64ull << 20) / esz * up / down;
+  c->chunk = (uint32_t)std::max<uint64_t>(T, std::min(by_out, by_in) / T * T);
+  const int J = c->J;
+  std::vector<float2> taps((size_t)n_ch * up * J);
+  std::vector<double2> taps64(taps.size());
+  c->step.resize(n_ch);
+  for (uint32_t ch = 0; ch < n_ch; ch++) {
+    c->step[ch] = (delta[ch] % fs + fs) % fs;
+    for (int j = 0; j < J; j++) {
+      const long long p = (((long long)j * delta[ch]) % fs + fs) % fs;
+      const double a = 2 * M_PI * (double)p / (double)fs, ca = std::cos(a), sa = std::sin(a);
+      for (int phi = 0; phi < up; phi++) {
+        const int k = phi + j * up;
+        const double hk = k <= 2 * c->M ? (double)c->h[k] : 0.0;
+        const size_t i = ((size_t)ch * up + phi) * J + j;
+        taps64[i] = make_double2(hk * ca, hk * sa);
+        taps[i] = make_float2((float)taps64[i].x, (float)taps64[i].y);
+      }
+    }
+  }
+  cudaError_t e = cudaSetDevice(ctx->device);
+  if (e == cudaSuccess) e = c->d_taps.alloc(taps.size());
+  if (e == cudaSuccess) e = c->d_taps64.alloc(taps64.size());
+  if (e == cudaSuccess) e = c->d_step.alloc(n_ch);
+  if (e == cudaSuccess) e = c->d_gain.alloc(n_ch);
+  if (e == cudaSuccess) e = c->d_clip.alloc(n_ch);
+  if (e == cudaSuccess) e = cudaMemcpy(c->d_taps.p, taps.data(), taps.size() * sizeof(float2), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = cudaMemcpy(c->d_taps64.p, taps64.data(), taps64.size() * sizeof(double2), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = cudaMemcpy(c->d_step.p, c->step.data(), n_ch * 8, cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = cudaMemcpy(c->d_gain.p, c->gain.data(), n_ch * 4, cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = cudaEventCreate(&c->ev0);
+  if (e == cudaSuccess) e = cudaEventCreate(&c->ev1);
+  if (e == cudaSuccess) e = r_set_smem<LCS_IQ_CI16>();
+  if (e == cudaSuccess) e = r_set_smem<LCS_IQ_CS8>();
+  if (e == cudaSuccess) e = r_set_smem<LCS_IQ_CU8>();
+  if (e == cudaSuccess) e = r_set_smem<LCS_IQ_CF32>();
+  if (e != cudaSuccess) {
+    delete c;
+    return fail(ctx, LCS_ERR_CUDA, std::string("lcs_chan_create_rational: ") + cudaGetErrorString(e));
+  }
+  *out = c;
+  return LCS_OK;
+}
+
+lcs_status lcs_chan_push(lcs_chan* c, const void* iq_host, uint32_t n_in, uint8_t* out, uint32_t out_capacity,
+                         int out_on_device, uint32_t* n_out, uint64_t* n_clipped) {
+  if (!c) return LCS_ERR_ARG;
+  if (!c->rat)
+    return lcs_chan_push_ci16(c, static_cast<const int16_t*>(iq_host), n_in, out, out_capacity, out_on_device, n_out, n_clipped);
+  return r_push(c, iq_host, n_in, out, out_capacity, out_on_device, n_out, n_clipped);
+}
+
+lcs_status lcs_chan_auto_gain(lcs_chan* c, const void* iq_host, uint32_t n) {
+  if (!c) return LCS_ERR_ARG;
+  if (!c->rat) return lcs_chan_auto_gain_ci16(c, static_cast<const int16_t*>(iq_host), n);
+  return r_auto_gain(c, iq_host, n);
 }
 
 lcs_status lcs_chan_timing_read(lcs_chan* c, double* kernel_ms, uint64_t* launches) {

@@ -42,6 +42,11 @@ static void print_usage() {
   cout << "                                 little-endian int16 I/Q (ci16, no header), channelized on the GPU" << endl;
   cout << "     --fs-in FS                  with --wideband: the recording's sample rate, D * 1.92 MHz with D in [2, 64]" << endl;
   cout << "     --fc-in FC                  with --wideband: the recording's centre frequency" << endl;
+  cout << "     --resample                  with --wideband: resample by up/down to 1.92 Msps, so that --fs-in may be any" << endl;
+  cout << "                                 integer number of Hz in (1.92, 122.88] MHz with fs-in/1.92 MHz = down/up," << endl;
+  cout << "                                 up <= 128, down <= 640 (e.g. 2.048, 2.4, 2.5, 6, 10, 20, 25, 56, 100 Msps)" << endl;
+  cout << "     --format F                  with --resample: the recording's sample format, ci16 (default), cs8 (HackRF)," << endl;
+  cout << "                                 cu8 (rtl_sdr) or cf32 (GNU Radio, SigMF cf32_le)" << endl;
   cout << "  -r --record / -i --device-index need a live rtl-sdr dongle: not supported by this build" << endl;
 }
 
@@ -59,14 +64,16 @@ static string freq_formatter(const double& freq) {   // CellSearch.cpp:322-341
 int main(int argc, char* const argv[]) {
   double freq_start = -1, freq_end = -1, ppm = 120, correction = 1;
   bool save_cap = false, use_recorded_data = false, raw = false, batched = false;
-  string data_dir = ".", wideband;
+  string data_dir = ".", wideband, format = "ci16";
   double fs_in = -1, fc_in = -1;
+  bool resample = false;
   static struct option long_options[] = {
       {"help", no_argument, 0, 'h'},          {"verbose", no_argument, 0, 'v'},       {"brief", no_argument, 0, 'b'},
       {"freq-start", required_argument, 0, 's'}, {"freq-end", required_argument, 0, 'e'}, {"ppm", required_argument, 0, 'p'},
       {"correction", required_argument, 0, 'c'}, {"record", no_argument, 0, 'r'},        {"load", no_argument, 0, 'l'},
       {"data-dir", required_argument, 0, 'd'},   {"device-index", required_argument, 0, 'i'}, {"raw", no_argument, 0, 'R'}, {"sweep", no_argument, 0, 'W'},
       {"wideband", required_argument, 0, 'B'},   {"fs-in", required_argument, 0, 'F'},   {"fc-in", required_argument, 0, 'C'},
+      {"resample", no_argument, 0, 'S'},         {"format", required_argument, 0, 'T'},
       {0, 0, 0, 0}};
   for (;;) {
     int idx = 0;
@@ -89,6 +96,8 @@ int main(int argc, char* const argv[]) {
       case 'B': wideband = optarg; break;
       case 'F': fs_in = strtod(optarg, &endp); if (optarg == endp || *endp) { cerr << "Error: could not parse --fs-in" << endl; return -1; } break;
       case 'C': fc_in = strtod(optarg, &endp); if (optarg == endp || *endp) { cerr << "Error: could not parse --fc-in" << endl; return -1; } break;
+      case 'S': resample = true; break;
+      case 'T': format = optarg; break;
       case 'i': break;
       default: return -1;
     }
@@ -115,17 +124,32 @@ int main(int argc, char* const argv[]) {
     return -1;
   }
   // wideband recording: every argument and the file length are checked before any device work
-  vector<int16_t> wide_iq;
+  vector<unsigned char> wide_iq;
   uint32_t wide_n = 0;
+  int wide_format = LCS_IQ_CI16;
+  size_t wide_bytes = 4;   // per sample
   if (wide) {
     if (use_recorded_data || batched) { cerr << "Error: --wideband cannot be combined with -l or --sweep" << endl; return -1; }
     if (fc_in <= 0) { cerr << "Error: --wideband needs --fc-in" << endl; return -1; }
-    uint32_t n_taps = 0;
-    if (lcs_chan_design_taps(fs_in, nullptr, &n_taps) != LCS_OK) {
-      cerr << "Error: --fs-in must be D * 1.92 MHz with an integer D in [2, 64]" << endl;
+    if (format == "cs8") { wide_format = LCS_IQ_CS8; wide_bytes = 2; }
+    else if (format == "cu8") { wide_format = LCS_IQ_CU8; wide_bytes = 2; }
+    else if (format == "cf32") { wide_format = LCS_IQ_CF32; wide_bytes = 8; }
+    else if (format != "ci16") { cerr << "Error: --format must be ci16, cs8, cu8 or cf32" << endl; return -1; }
+    if (!resample && format != "ci16") { cerr << "Error: --format needs --resample" << endl; return -1; }
+    uint32_t n_taps = 0, up = 1, down = 1;
+    if (resample) {
+      if (lcs_chan_design_rational(fs_in, &up, &down, nullptr, &n_taps) != LCS_OK) {
+        cerr << "Error: --fs-in must be an integer number of Hz in (1.92, 122.88] MHz with fs-in / 1.92 MHz = down / up, "
+                "up <= 128 and down <= 640" << endl;
+        return -1;
+      }
+    } else if (lcs_chan_design_taps(fs_in, nullptr, &n_taps) != LCS_OK) {
+      cerr << "Error: --fs-in must be D * 1.92 MHz with an integer D in [2, 64] (other rates: --resample)" << endl;
       return -1;
+    } else {
+      down = (uint32_t)std::lround(fs_in / 1.92e6);
     }
-    const int D = (int)std::lround(fs_in / 1.92e6), M = (int)(n_taps - 1) / 2;
+    const uint64_t M = (n_taps - 1) / 2;
     const int n_fc = (int)floor((freq_end - freq_start) / 100e3) + 1;                     // the raster of the search loop
     for (int fci = 0; fci < n_fc; fci++) {
       const double fc = freq_start + fci * 100e3, d = fc - fc_in;
@@ -135,15 +159,16 @@ int main(int argc, char* const argv[]) {
         return -1;
       }
     }
-    wide_n = 153599u * D + M + 1;   // 153 600 outputs per channel
+    wide_n = (uint32_t)((153599ull * down + M + 1 + up - 1) / up);   // 153 600 outputs per channel
     // only the prefix the search uses is read (a recording may be far longer)
     FILE* f = std::fopen(wideband.c_str(), "rb");
     if (!f) { cerr << "Error: cannot read " << wideband << endl; return -1; }
-    wide_iq.resize((size_t)wide_n * 2);
-    const size_t got = std::fread(wide_iq.data(), 4, wide_n, f);
+    wide_iq.resize((size_t)wide_n * wide_bytes);
+    const size_t got = std::fread(wide_iq.data(), wide_bytes, wide_n, f);
     std::fclose(f);
     if (got < wide_n) {
-      cerr << "Error: " << wideband << " holds " << got << " ci16 samples; 153600 outputs per channel need " << wide_n << endl;
+      cerr << "Error: " << wideband << " holds " << got << " " << format << " samples; 153600 outputs per channel need "
+           << wide_n << endl;
       return -1;
     }
   }
@@ -175,7 +200,12 @@ int main(int argc, char* const argv[]) {
       vector<double> fcs;
       for (int fci = 0; fci < n_fc; fci++) fcs.push_back(freq_start + fci * 100e3);
       if (verbosity >= 1) cout << "Channelizing and examining " << n_fc << " center frequencies of one wideband recording ..." << endl;
-      wideband_search_ci16(wide_iq.data(), wide_n, fs_in, fc_in, fcs, f_search_set, fs_programmed, detected_cells);
+      if (resample)
+        wideband_search_rational(wide_iq.data(), wide_format, wide_n, fs_in, fc_in, fcs, f_search_set, fs_programmed,
+                                 detected_cells);
+      else
+        wideband_search_ci16(reinterpret_cast<const int16_t*>(wide_iq.data()), wide_n, fs_in, fc_in, fcs, f_search_set,
+                             fs_programmed, detected_cells);
     }
     if (batched) {
       // every centre frequency of the sweep in one call: the raw byte dumps are concatenated and handed to the batched

@@ -82,8 +82,10 @@ void sweep_search_cu8(const std::vector<unsigned char>& iq, uint32_t n_cap, cons
     for (uint32_t k = 0; k < n[c] && k < max_cells; k++) detected_cells[c].push_back(from_pod(cells[(size_t)c * max_cells + k]));
 }
 
-void wideband_search_ci16(const int16_t* iq, uint32_t n, double fs_in, double fc_in, const std::vector<double>& fc_requested,
-                          const vec& f_search_set, const double& fs_programmed, std::vector<std::list<Cell> >& detected_cells) {
+// iq_format < 0: lcs_chan_create (ci16 at D * 1.92 MHz); otherwise lcs_chan_create_rational with that format
+static void wideband_search(const void* iq, int iq_format, uint32_t n, double fs_in, double fc_in,
+                            const std::vector<double>& fc_requested, const vec& f_search_set, const double& fs_programmed,
+                            std::vector<std::list<Cell> >& detected_cells) {
   const uint32_t n_ch = (uint32_t)fc_requested.size(), max_cells = 16, n_cap = 153600;
   lcs_ctx* ctx = lcs_dropin_ctx();
   lcs_chan* ch = nullptr;
@@ -92,16 +94,23 @@ void wideband_search_ci16(const int16_t* iq, uint32_t n, double fs_in, double fc
   std::vector<lcs_cell> cells((size_t)n_ch * max_cells);
   std::vector<uint32_t> found(n_ch, 0);
   uint32_t n_out = 0;
-  lcs_status rc = lcs_chan_create(ctx, fs_in, fc_in, n_ch, fc_requested.data(), nullptr, &ch);
-  const char* where = "lcs_chan_create";
-  if (rc == LCS_OK) { rc = lcs_chan_auto_gain_ci16(ch, iq, n); where = "lcs_chan_auto_gain_ci16"; }
+  lcs_status rc;
+  const char* where;
+  if (iq_format < 0) {
+    rc = lcs_chan_create(ctx, fs_in, fc_in, n_ch, fc_requested.data(), nullptr, &ch);
+    where = "lcs_chan_create";
+  } else {
+    rc = lcs_chan_create_rational(ctx, fs_in, iq_format, fc_in, n_ch, fc_requested.data(), nullptr, &ch);
+    where = "lcs_chan_create_rational";
+  }
+  if (rc == LCS_OK) { rc = lcs_chan_auto_gain(ch, iq, n); where = "lcs_chan_auto_gain"; }
   if (rc == LCS_OK && cudaMalloc((void**)&d_iq, (size_t)n_ch * n_cap * 2) != cudaSuccess) {
     d_iq = nullptr;
     rc = LCS_ERR_CUDA;
     where = "cudaMalloc";
   }
-  if (rc == LCS_OK) { rc = lcs_chan_push_ci16(ch, iq, n, d_iq, n_cap, 1, &n_out, nullptr); where = "lcs_chan_push_ci16"; }
-  if (rc == LCS_OK && n_out != n_cap) { rc = LCS_ERR_ARG; where = "lcs_chan_push_ci16 (recording too short)"; }
+  if (rc == LCS_OK) { rc = lcs_chan_push(ch, iq, n, d_iq, n_cap, 1, &n_out, nullptr); where = "lcs_chan_push"; }
+  if (rc == LCS_OK && n_out != n_cap) { rc = LCS_ERR_ARG; where = "lcs_chan_push (recording too short)"; }
   if (rc == LCS_OK) { rc = lcs_sweep_create(ctx, n_cap, &sw); where = "lcs_sweep_create"; }
   if (rc == LCS_OK) {
     rc = lcs_sweep_search_cu8_device(sw, d_iq, n_ch, fc_requested.data(), nullptr, fs_programmed, f_search_set._data(),
@@ -115,6 +124,17 @@ void wideband_search_ci16(const int16_t* iq, uint32_t n, double fs_in, double fc
   detected_cells.assign(n_ch, std::list<Cell>());
   for (uint32_t c = 0; c < n_ch; c++)
     for (uint32_t k = 0; k < found[c] && k < max_cells; k++) detected_cells[c].push_back(from_pod(cells[(size_t)c * max_cells + k]));
+}
+
+void wideband_search_ci16(const int16_t* iq, uint32_t n, double fs_in, double fc_in, const std::vector<double>& fc_requested,
+                          const vec& f_search_set, const double& fs_programmed, std::vector<std::list<Cell> >& detected_cells) {
+  wideband_search(iq, -1, n, fs_in, fc_in, fc_requested, f_search_set, fs_programmed, detected_cells);
+}
+
+void wideband_search_rational(const void* iq, int iq_format, uint32_t n, double fs_in, double fc_in,
+                              const std::vector<double>& fc_requested, const vec& f_search_set,
+                              const double& fs_programmed, std::vector<std::list<Cell> >& detected_cells) {
+  wideband_search(iq, iq_format, n, fs_in, fc_in, fc_requested, f_search_set, fs_programmed, detected_cells);
 }
 
 // ---- searcher.h:22-41 ----

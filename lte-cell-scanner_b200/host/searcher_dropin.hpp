@@ -100,4 +100,8 @@ void sweep_search_cu8(const std::vector<unsigned char>& iq, uint32_t n_cap, cons
 // channel channelized into device memory (153 600 samples each), then lcs_sweep_search_cu8_device.
 void wideband_search_ci16(const int16_t* iq, uint32_t n, double fs_in, double fc_in, const std::vector<double>& fc_requested,
                           const itpp::vec& f_search_set, const double& fs_programmed, std::vector<std::list<Cell> >& detected_cells);
+// The same at any rate lcs_chan_create_rational allows, iq [n][2] in iq_format (LCS_IQ_CI16, CS8, CU8 or CF32).
+void wideband_search_rational(const void* iq, int iq_format, uint32_t n, double fs_in, double fc_in,
+                              const std::vector<double>& fc_requested, const itpp::vec& f_search_set,
+                              const double& fs_programmed, std::vector<std::list<Cell> >& detected_cells);
    // skip the 136 MB `xc`/`sp`/`xc_incoherent` debug outputs (CLI does)

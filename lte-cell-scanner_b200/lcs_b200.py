@@ -15,7 +15,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("LCS_B200_LIB") or os.path.join(HERE, "liblcs_b200.so")
 HEADER = os.path.join(HERE, "..", "include", "lcs_b200.h")
 
-IQ_CF32, IQ_CU8, IQ_C128 = 0, 1, 2
+IQ_CF32, IQ_CU8, IQ_C128, IQ_CI16, IQ_CS8 = 0, 1, 2, 3, 4
 KERNEL_AUTO, KERNEL_FP32, KERNEL_TC = 0, 1, 2
 N_FOLD = 9600
 
@@ -100,6 +100,12 @@ def lib():
         _lib.lcs_chan_push_ci16.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_int, C.c_void_p,
                                             C.c_void_p]
         _lib.lcs_chan_timing_read.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+        _lib.lcs_chan_design_rational.argtypes = [C.c_double, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        _lib.lcs_chan_create_rational.argtypes = [C.c_void_p, C.c_double, C.c_int, C.c_double, C.c_uint32, C.c_void_p,
+                                                  C.c_void_p, C.c_void_p]
+        _lib.lcs_chan_push.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_int, C.c_void_p,
+                                       C.c_void_p]
+        _lib.lcs_chan_auto_gain.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
     return _lib
 
 
@@ -677,6 +683,109 @@ class Channelizer:
         got = C.c_uint32(0)
         _chk(lib().lcs_chan_push_ci16(self._h, _p(iq), C.c_uint32(iq.shape[0]), C.c_void_p(out.data_ptr()),
                                       C.c_uint32(cap), 1, C.byref(got), _p(clip)), self.ctx._h)
+        return got.value, clip
+
+    def timing_read(self):
+        """(kernel ms, launches) since the last read, from CUDA events around each launch."""
+        ms = C.c_double(0); n = C.c_uint64(0)
+        _chk(lib().lcs_chan_timing_read(self._h, C.byref(ms), C.byref(n)), self.ctx._h)
+        return ms.value, n.value
+
+    def close(self):
+        if self._h:
+            lib().lcs_chan_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def chan_design_rational(fs_in):
+    """fs_in / 1.92 MHz = down / up in lowest terms and the prototype low-pass at up * fs_in, DC gain up (host only):
+    (up, down, float32 [L])."""
+    up, down, n = C.c_uint32(0), C.c_uint32(0), C.c_uint32(0)
+    _chk(lib().lcs_chan_design_rational(C.c_double(fs_in), C.byref(up), C.byref(down), None, C.byref(n)))
+    h = np.zeros(n.value, np.float32)
+    _chk(lib().lcs_chan_design_rational(C.c_double(fs_in), C.byref(up), C.byref(down), _p(h), C.byref(n)))
+    return up.value, down.value, h
+
+
+# sample format name -> (lcs format, numpy dtype of the [n][2] components)
+CHAN_FORMATS = {"ci16": (IQ_CI16, np.int16), "cs8": (IQ_CS8, np.int8), "cu8": (IQ_CU8, np.uint8),
+                "cf32": (IQ_CF32, np.float32)}
+
+
+class RationalChannelizer:
+    """lcs_chan at any allowed SDR rate: a wideband ci16 / cs8 / cu8 / cf32 recording -> one 1.92 Msps cu8 stream per LTE
+    raster channel, resampled by up / down (DESIGN.md section 4.7)."""
+
+    def __init__(self, ctx, fs_in, fc_in, fc_ch, fmt="ci16", gain=None):
+        if fmt not in CHAN_FORMATS:
+            raise ValueError("fmt must be one of %s" % ", ".join(CHAN_FORMATS))
+        self.ctx = ctx
+        self.fmt = fmt
+        self._iq_format, self._dtype = CHAN_FORMATS[fmt]
+        fc = np.ascontiguousarray(np.atleast_1d(fc_ch), np.float64)
+        self.n_ch = fc.size
+        self.fc_ch = fc
+        g = None if gain is None else np.ascontiguousarray(np.broadcast_to(np.asarray(gain, np.float32), (self.n_ch,)))
+        self._h = C.c_void_p()
+        _chk(lib().lcs_chan_create_rational(ctx._h, C.c_double(fs_in), self._iq_format, C.c_double(fc_in),
+                                            C.c_uint32(self.n_ch), _p(fc), _p(g), C.byref(self._h)), ctx._h)
+        self.up, self.down, self.taps = chan_design_rational(fs_in)
+        self.M = (self.taps.size - 1) // 2
+
+    def _samples(self, iq):
+        """iq as a contiguous [n][2] array of the format's dtype (complex64 [n] is accepted for cf32)."""
+        iq = np.asarray(iq)
+        if self.fmt == "cf32" and iq.dtype == np.complex64 and iq.ndim == 1:
+            iq = iq.view(np.float32).reshape(-1, 2)
+        if iq.dtype != self._dtype or iq.ndim != 2 or iq.shape[1] != 2:
+            raise ValueError("expected %s samples: %s [n][2]" % (self.fmt, np.dtype(self._dtype).name))
+        return np.ascontiguousarray(iq)
+
+    def auto_gain(self, iq):
+        """Set every channel's gain to 0.25 / RMS of its output over these samples (the stream is not touched)."""
+        iq = self._samples(iq)
+        _chk(lib().lcs_chan_auto_gain(self._h, _p(iq), C.c_uint32(iq.shape[0])), self.ctx._h)
+        return self.gain
+
+    @property
+    def gain(self):
+        g = np.zeros(self.n_ch, np.float32)
+        _chk(lib().lcs_chan_gain(self._h, _p(g)), self.ctx._h)
+        return g
+
+    def n_out(self, n_in):
+        k = C.c_uint32(0)
+        _chk(lib().lcs_chan_n_out(self._h, C.c_uint64(n_in), C.byref(k)), self.ctx._h)
+        return k.value
+
+    def push(self, iq):
+        """Push [n][2] samples.  Returns (cu8 [n_ch][n_out][2], n_clipped [n_ch])."""
+        iq = self._samples(iq)
+        k = self.n_out(iq.shape[0])
+        out = np.zeros((self.n_ch, k, 2), np.uint8)
+        clip = np.zeros(self.n_ch, np.uint64)
+        got = C.c_uint32(0)
+        _chk(lib().lcs_chan_push(self._h, _p(iq), C.c_uint32(iq.shape[0]), _p(out), C.c_uint32(k), 0, C.byref(got),
+                                 _p(clip)), self.ctx._h)
+        return out, clip
+
+    def push_device(self, iq, out):
+        """Push [n][2] samples, writing the bytes into the uint8 CUDA tensor out [n_ch][capacity][2] from column 0 on.
+        Returns (n_out, n_clipped [n_ch])."""
+        iq = self._samples(iq)
+        if not (out.is_cuda and out.is_contiguous() and str(out.dtype) == "torch.uint8" and out.dim() == 3 and
+                out.shape[0] == self.n_ch and out.shape[2] == 2):
+            raise ValueError("push_device: expected a contiguous uint8 CUDA tensor [n_ch][capacity][2]")
+        clip = np.zeros(self.n_ch, np.uint64)
+        got = C.c_uint32(0)
+        _chk(lib().lcs_chan_push(self._h, _p(iq), C.c_uint32(iq.shape[0]), C.c_void_p(out.data_ptr()),
+                                 C.c_uint32(out.shape[1]), 1, C.byref(got), _p(clip)), self.ctx._h)
         return got.value, clip
 
     def timing_read(self):

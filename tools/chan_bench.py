@@ -9,7 +9,11 @@ from a synthetic ci16 recording (complex noise, 2 LTE carriers).  One JSON line 
     lcs_sweep_search_cu8 on the same channelized bytes from host memory;
   - the card name and power limit, read in the same run.
 
-Usage: python tools/chan_bench.py [--d 16 32] [--reps 10]
+With --fs-in FS:FMT ... (e.g. 2.4e6:cu8 20e6:cs8 25e6:ci16) it first reports the same device time per 80 ms and
+real-time factor for the resampling channelizer (lcs_chan_create_rational) at each rate and sample format, every raster
+channel, then the --d runs as usual.
+
+Usage: python tools/chan_bench.py [--d 16 32] [--reps 10] [--fs-in FS:FMT ...]
 """
 import argparse
 import json
@@ -103,14 +107,63 @@ def run(D, reps, ctx):
     }
 
 
+def run_rational(fs_in, fmt, reps, ctx):
+    """Device time per 80 ms of a continuing stream of fs_in fmt samples, every raster channel, into device memory."""
+    import torch
+    edge = fs_in / 2 - 960e3
+    fcs = FC_IN + 100e3 * np.arange(-int(edge // 100e3), int(edge // 100e3) + 1)
+    up, down, h = L.chan_design_rational(fs_in)
+    n80 = N_CAP * down // up                # 80 ms of input
+    off = round(fs_in / 6 / 100e3) * 100e3
+    cell = dict(n_id_cell=277, n_ports=2, cp_type=1, n_rb_dl=6, phich_duration=1, phich_resource=3, t0=1234.0, sfn0=0)
+    iq16 = S.synth_wide_ci16(n80, fs_in, FC_IN, [(FC_IN - off, [cell], 1.0)], snr_db=10, seed=1, scale=2048.0)
+    if fmt == "cf32":
+        iq = (iq16 / 32768).astype(np.float32)
+    elif fmt in ("cs8", "cu8"):
+        v = np.clip(np.round(iq16 * (20 / np.sqrt(np.mean(iq16.astype(np.float64) ** 2)))), -127, 127)
+        iq = v.astype(np.int8) if fmt == "cs8" else (v + 127).astype(np.uint8)
+    else:
+        iq = iq16
+    out = torch.empty((fcs.size, N_CAP + 1, 2), dtype=torch.uint8, device="cuda")
+    ch = L.RationalChannelizer(ctx, fs_in, FC_IN, fcs, fmt=fmt)
+    ch.auto_gain(iq)
+    ch.push_device(iq, out)                 # warm-up
+    ch.timing_read()
+    host = []
+    for r in range(reps):
+        t0 = time.perf_counter()
+        ch.push_device(iq, out)
+        host.append(time.perf_counter() - t0)
+    kernel_ms, launches = ch.timing_read()
+    ch.close()
+    per80 = kernel_ms / reps
+    taps_per_out = -(-h.size // up)
+    return {
+        "fs_in_msps": fs_in / 1e6, "format": fmt, "up": up, "down": down, "channels": int(fcs.size), "taps": int(h.size),
+        "taps_per_output": taps_per_out,
+        "chan_kernel_ms_per_80ms": per80,
+        "chan_launches_per_push": launches / reps,
+        "chan_input_msamp_s": n80 / (per80 / 1e3) / 1e6,
+        "chan_realtime_factor": 80.0 / per80,
+        "chan_tflops": 8.0 * taps_per_out * N_CAP * fcs.size / (per80 / 1e3) / 1e12,
+        "chan_push_ms_mean": 1e3 * float(np.mean(host)),
+    }
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--d", type=int, nargs="+", default=[16, 32])
     ap.add_argument("--reps", type=int, default=10)
+    ap.add_argument("--fs-in", nargs="*", default=[], metavar="FS:FMT")
     a = ap.parse_args()
     ctx = L.Context(0)
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
-                       text=True).stdout.strip().splitlines()
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"],
+                       capture_output=True, text=True).stdout.strip().splitlines()
+    for spec in a.fs_in:
+        fs, fmt = spec.split(":")
+        r = run_rational(float(fs), fmt, a.reps, ctx)
+        r["gpu"] = q[0] if q else "unknown"
+        print(json.dumps(r), flush=True)
     for D in a.d:
         r = run(D, a.reps, ctx)
         r["gpu"] = q[0] if q else "unknown"
