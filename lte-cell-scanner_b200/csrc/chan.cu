@@ -10,7 +10,9 @@
 // round-to-nearest-even quantisation and the clip count.
 //
 // rchan_kernel (DESIGN.md section 4.7) generalises this to rational resampling by up / down from any allowed integer-Hz
-// rate and to ci16, cs8, cu8 and cf32 input; lcs_chan_create_rational builds the same lcs_chan for it.
+// rate and to ci16, cs8, cu8 and cf32 input.  Decimation by D is up = 1, down = D, so one host path (create, push, auto
+// gain, the chunked launch loop) drives both kernels; chan_kernel runs for ci16 at up = 1 and rchan_kernel for everything
+// else, and only the tap table and the launch know which.
 #include <climits>
 #include <cmath>
 #include <complex>
@@ -36,24 +38,50 @@ constexpr double kCut = 960000.0;        // prototype cutoff
 constexpr double kPass = 700000.0, kStop = 1220000.0;
 constexpr double kPassDb = 0.01, kStopDb = 70.0;
 constexpr int MAX_TAPS = 4097;
-// Dynamic shared memory of a launch: the input tile, D rows of TILE + 2M/D + 1 samples.  The largest any channelizer can
-// ask for (D = 64, L = MAX_TAPS) is the kernels' attribute, set identically by every lcs_chan_create: the attribute is one
-// value per function for the whole process, so a per-channelizer value would cap the launches of channelizers created
-// earlier with a larger D.
-constexpr int smem_bytes(int D, int M) { return D * (TILE + (2 * M) / D + 1) * (int)sizeof(float2); }
-constexpr int SMEM_CAP = smem_bytes(64, (MAX_TAPS - 1) / 2);   // 98 816 bytes
-static_assert(SMEM_CAP <= 227 * 1024, "input tile exceeds the shared memory of an SM");
+constexpr int RMAX_UP = 128, RMAX_DOWN = 640;
+constexpr int RMAX_TAPS = 16385;
+// Dynamic shared memory of a launch: the input tile, `down` rows of qlen samples, covering the 32 * RM * down + J inputs
+// of a tile's outputs (at up = 1, RM = 4: D rows of TILE + 2M/D + 1).  The kernels' attribute is one value per function
+// for the whole process, so a per-channelizer value would cap the launches of channelizers created earlier with a larger
+// tile; every create sets the same fixed caps: for chan_kernel the largest tile it can be asked for (D = 64, L = MAX_TAPS),
+// for rchan_kernel the opt-in maximum of an H100 CTA.
+constexpr int tile_qlen(int down, int J, int RM) { return (32 * RM * down + J + down - 1) / down; }
+constexpr size_t tile_smem(int down, int J, int RM) { return (size_t)down * tile_qlen(down, J, RM) * sizeof(float2); }
+constexpr int SMEM_CAP = (int)tile_smem(64, MAX_TAPS, R);   // 98 816 bytes
+constexpr int RSMEM_CAP = 227 * 1024;
+static_assert(SMEM_CAP <= RSMEM_CAP, "input tile exceeds the shared memory of an SM");
 
-struct Params {
-  const int* in;               // packed ci16 (I low, Q high); local sample 0 is the first input of local output 0 (n0*D-M)
+// The parameters of a launch.  The two kernels share every field but the tile geometry (run() assigns the shared ones in
+// one place); each keeps the layout it was compiled and measured with, which ptxas's register allocation depends on.
+struct Params {                // chan_kernel (up = 1: down = D)
+  const unsigned char* in;     // packed ci16 (I low, Q high); local sample 0 is the first input of local output 0 (n0*D-M)
   long long n_in;              // valid samples at `in` (later ones read as 0; no valid output uses them)
-  int D, L, M, qlen;
+  int down, L, M, qlen;
   int n_out;                   // outputs of this launch
   long long n0;                // stream index of local output 0
   int n_ch;
   const float2* taps;          // [n_ch][L] complex taps h[t] * exp(+j2pi ((t-M)*delta mod fs)/fs)
   const double2* taps64;       // the same in double (power mode)
   const long long* step;       // [n_ch] (D*delta) mod fs
+  long long fs;
+  const float* gain;           // [n_ch]
+  unsigned char* out;          // [n_ch] rows of out_stride bytes; column 2*i is local output i
+  size_t out_stride;
+  unsigned long long* clip;    // [n_ch]
+  double* pw;                  // power mode: [n_ch][gridDim.x] sum |y|^2 per tile
+};
+
+struct RParams {               // rchan_kernel
+  const unsigned char* in;     // samples in the input format; local sample 0 is stream sample i_hi(n0) - (J-1)
+  long long n_in;              // valid samples at `in` (later ones read as 0; no valid output uses them)
+  int up, down, J, RM, qlen;
+  long long q0;                // n0*down + M
+  int n_out;                   // outputs of this launch
+  long long n0;                // stream index of local output 0
+  int n_ch;
+  const float2* taps;          // [n_ch][up][J] complex branch taps g_phi[j] * exp(+j2pi (j*delta mod fs)/fs)
+  const double2* taps64;       // the same in double (power mode)
+  const long long* step;       // [n_ch] delta mod fs
   long long fs;
   const float* gain;           // [n_ch]
   unsigned char* out;          // [n_ch] rows of out_stride bytes; column 2*i is local output i
@@ -76,21 +104,57 @@ __device__ __forceinline__ void cmac(double2& a, double2 g, float2 x) {
   a.y = __fma_rn(g.y, (double)x.x, a.y);
 }
 
+// sample g of the input, converted exactly to float: ci16 / 32768, cs8 / 128, (cu8 - 127) / 128, cf32 as is
+template <int FMT>
+__device__ __forceinline__ float2 load_iq(const unsigned char* p, long long g) {
+  if constexpr (FMT == LCS_IQ_CI16) {
+    const int w = __ldg(reinterpret_cast<const int*>(p) + g);
+    return make_float2((float)(short)(w & 0xffff) * (1.f / 32768.f), (float)(short)(w >> 16) * (1.f / 32768.f));
+  } else if constexpr (FMT == LCS_IQ_CS8) {
+    const unsigned short w = __ldg(reinterpret_cast<const unsigned short*>(p) + g);
+    return make_float2((float)(signed char)(w & 0xff) * (1.f / 128.f), (float)(signed char)(w >> 8) * (1.f / 128.f));
+  } else if constexpr (FMT == LCS_IQ_CU8) {
+    const unsigned short w = __ldg(reinterpret_cast<const unsigned short*>(p) + g);
+    return make_float2((float)((int)(w & 0xff) - 127) * (1.f / 128.f), (float)((int)(w >> 8) - 127) * (1.f / 128.f));
+  } else {
+    return __ldg(reinterpret_cast<const float2*>(p) + g);
+  }
+}
+
+// One output: rotate the accumulator by the exact mixer phase p (cycles * fs) in FP64, scale by gn = 128 * gain, round to
+// nearest even about 127 and store the two clamped bytes at o.  Returns how many of the two were clamped.
+template <class V>
+__device__ __forceinline__ int rotate_quantise(V acc, long long p, long long fs, double gn, unsigned char* o) {
+  double sn, cs;
+  sincospi(-2.0 * (double)p / (double)fs, &sn, &cs);
+  const double yr = (double)acc.x * cs - (double)acc.y * sn;
+  const double yi = (double)acc.x * sn + (double)acc.y * cs;
+  double vr = rint(127.0 + gn * yr), vi = rint(127.0 + gn * yi);
+  const int clipped = (vr < 0 || vr > 255) + (vi < 0 || vi > 255);
+  vr = fmin(fmax(vr, 0.0), 255.0);
+  vi = fmin(fmax(vi, 0.0), 255.0);
+  o[0] = (unsigned char)vr;
+  o[1] = (unsigned char)vi;
+  return clipped;
+}
+
+// the warp's sum of s, in lane 0
+__device__ __forceinline__ double warp_sum(double s) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_down_sync(0xffffffffu, s, o);
+  return s;
+}
+
 template <bool POWER>
 __global__ void __launch_bounds__(THREADS) chan_kernel(Params P) {
   extern __shared__ float2 xs[];                     // [D][qlen]
   const int tile = blockIdx.x;
   const int nl0 = tile * TILE;
-  const long long j0 = (long long)nl0 * P.D;
-  const int span = (TILE - 1) * P.D + 2 * P.M + 1;
+  const long long j0 = (long long)nl0 * P.down;
+  const int span = (TILE - 1) * P.down + 2 * P.M + 1;
   for (int j = threadIdx.x; j < span; j += THREADS) {
     const long long g = j0 + j;
-    float2 v = make_float2(0.f, 0.f);
-    if (g < P.n_in) {
-      const int w = __ldg(P.in + g);
-      v = make_float2((float)(short)(w & 0xffff) * (1.f / 32768.f), (float)(short)(w >> 16) * (1.f / 32768.f));
-    }
-    xs[(j % P.D) * P.qlen + j / P.D] = v;
+    xs[(j % P.down) * P.qlen + j / P.down] = g < P.n_in ? load_iq<LCS_IQ_CI16>(P.in, g) : make_float2(0.f, 0.f);
   }
   __syncthreads();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -124,7 +188,7 @@ __global__ void __launch_bounds__(THREADS) chan_kernel(Params P) {
 #pragma unroll
       for (int r = 0; r < R; r++) cmac(acc[i][r], g, x[r]);
     }
-    if (++ph == P.D) { ph = 0; row++; }
+    if (++ph == P.down) { ph = 0; row++; }
   }
 #pragma unroll
   for (int i = 0; i < CW; i++) {
@@ -135,8 +199,7 @@ __global__ void __launch_bounds__(THREADS) chan_kernel(Params P) {
 #pragma unroll
       for (int r = 0; r < R; r++)
         if (nl0 + lane + 32 * r < P.n_out) s += (double)acc[i][r].x * acc[i][r].x + (double)acc[i][r].y * acc[i][r].y;
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) s += __shfl_down_sync(0xffffffffu, s, o);
+      s = warp_sum(s);
       if (lane == 0) P.pw[(size_t)c * gridDim.x + tile] = s;
     } else {
       const long long st = P.step[c];
@@ -148,17 +211,8 @@ __global__ void __launch_bounds__(THREADS) chan_kernel(Params P) {
         if (nl >= P.n_out) continue;
         const long long n = P.n0 + nl;
         const long long p = ((n % P.fs) * st) % P.fs;            // exact phase of output n, in cycles * fs
-        double sn, cs;
-        sincospi(-2.0 * (double)p / (double)P.fs, &sn, &cs);
-        const double yr = (double)acc[i][r].x * cs - (double)acc[i][r].y * sn;
-        const double yi = (double)acc[i][r].x * sn + (double)acc[i][r].y * cs;
-        double vr = rint(127.0 + gn * yr), vi = rint(127.0 + gn * yi);
-        clipped += (vr < 0 || vr > 255) + (vi < 0 || vi > 255);
-        vr = fmin(fmax(vr, 0.0), 255.0);
-        vi = fmin(fmax(vi, 0.0), 255.0);
-        unsigned char* o = P.out + (size_t)c * P.out_stride + 2 * (size_t)nl;
-        o[0] = (unsigned char)vr;
-        o[1] = (unsigned char)vi;
+        clipped += rotate_quantise(acc[i][r], p, P.fs, gn,
+                                   P.out + (size_t)c * P.out_stride + 2 * (size_t)nl);
       }
       clipped = __reduce_add_sync(0xffffffffu, clipped);
       if (lane == 0 && clipped) atomicAdd(P.clip + c, (unsigned long long)clipped);
@@ -180,10 +234,10 @@ static double bessel_i0(double x) {
 
 double kaiser_beta() { return 0.1102 * (kStopDb - 8.7); }
 
-// Kaiser-windowed sinc of odd length L, cutoff 0.96 MHz at fs, DC gain 1, rounded to float.
-static void kaiser_sinc(int L, double fs, std::vector<float>& out) {
+// Kaiser-windowed sinc of odd length L, cutoff 0.96 MHz at the rate F, DC gain `gain`, rounded to float.
+static void kaiser_sinc(int L, double F, double gain, std::vector<float>& out) {
   const int M = (L - 1) / 2;
-  const double beta = kaiser_beta(), i0b = bessel_i0(beta), fcn = 2 * kCut / fs;
+  const double beta = kaiser_beta(), i0b = bessel_i0(beta), fcn = 2 * kCut / F;
   std::vector<double> h(L);
   double sum = 0;
   for (int n = 0; n < L; n++) {
@@ -195,7 +249,7 @@ static void kaiser_sinc(int L, double fs, std::vector<float>& out) {
     sum += h[n];
   }
   out.resize(L);
-  for (int n = 0; n < L; n++) out[n] = (float)(h[n] / sum);
+  for (int n = 0; n < L; n++) out[n] = (float)(gain * h[n] / sum);
 }
 
 // Response of the (symmetric) float taps on the grid of lcs_chan_design_taps: every fs/(64L) from 0 to 0.70 MHz and from
@@ -229,11 +283,11 @@ static int design(double fs, std::vector<float>& h) {
   const double dw = 2 * M_PI * (kStop - kPass) / fs;
   int L = (int)std::ceil((kStopDb - 8.0) / (2.285 * dw)) + 1;
   L |= 1;
-  kaiser_sinc(L, fs, h);
+  kaiser_sinc(L, fs, 1.0, h);
   if (meets_spec(h, fs)) {
     std::vector<float> g;
     while (L >= 5) {
-      kaiser_sinc(L - 2, fs, g);
+      kaiser_sinc(L - 2, fs, 1.0, g);
       if (!meets_spec(g, fs)) break;
       L -= 2;
       h.swap(g);
@@ -242,7 +296,7 @@ static int design(double fs, std::vector<float>& h) {
   }
   while (L < MAX_TAPS) {
     L += 2;
-    kaiser_sinc(L, fs, h);
+    kaiser_sinc(L, fs, 1.0, h);
     if (meets_spec(h, fs)) return L;
   }
   return 0;
@@ -264,46 +318,6 @@ static bool decimation(double fs_in, int* D) {
 // x[i_hi - j] exp(+j2pi (j*delta mod fs)/fs).  A CTA covers the outputs n0 + up*m + r of 32*RM consecutive m and every
 // r < up; a lane's register slot fixes (m / 32, r), so all 32 lanes of a warp use one branch (warp-uniform tap loads) and
 // read inputs `down` apart, which the tile staged in polyphase order modulo `down` turns into consecutive words.
-constexpr int RMAX_UP = 128, RMAX_DOWN = 640;
-constexpr int RMAX_TAPS = 16385;
-constexpr int RSMEM_CAP = 227 * 1024;    // the opt-in maximum of an H100 CTA; one fixed attribute for every channelizer
-
-struct RParams {
-  const unsigned char* in;     // samples in the input format; local sample 0 is stream sample i_hi(n0) - (J-1)
-  long long n_in;              // valid samples at `in` (later ones read as 0; no valid output uses them)
-  int up, down, J, RM, qlen;
-  long long q0;                // n0*down + M
-  int n_out;                   // outputs of this launch
-  long long n0;                // stream index of local output 0
-  int n_ch;
-  const float2* taps;          // [n_ch][up][J] complex branch taps g_phi[j] * exp(+j2pi (j*delta mod fs)/fs)
-  const double2* taps64;       // the same in double (power mode)
-  const long long* dmod;       // [n_ch] delta mod fs
-  long long fs;
-  const float* gain;           // [n_ch]
-  unsigned char* out;          // [n_ch] rows of out_stride bytes; column 2*i is local output i
-  size_t out_stride;
-  unsigned long long* clip;    // [n_ch]
-  double* pw;                  // power mode: [n_ch][gridDim.x] sum |y|^2 per tile
-};
-
-// sample g of the input, converted exactly to float: ci16 / 32768, cs8 / 128, (cu8 - 127) / 128, cf32 as is
-template <int FMT>
-__device__ __forceinline__ float2 load_iq(const unsigned char* p, long long g) {
-  if constexpr (FMT == LCS_IQ_CI16) {
-    const int w = __ldg(reinterpret_cast<const int*>(p) + g);
-    return make_float2((float)(short)(w & 0xffff) * (1.f / 32768.f), (float)(short)(w >> 16) * (1.f / 32768.f));
-  } else if constexpr (FMT == LCS_IQ_CS8) {
-    const unsigned short w = __ldg(reinterpret_cast<const unsigned short*>(p) + g);
-    return make_float2((float)(signed char)(w & 0xff) * (1.f / 128.f), (float)(signed char)(w >> 8) * (1.f / 128.f));
-  } else if constexpr (FMT == LCS_IQ_CU8) {
-    const unsigned short w = __ldg(reinterpret_cast<const unsigned short*>(p) + g);
-    return make_float2((float)((int)(w & 0xff) - 127) * (1.f / 128.f), (float)((int)(w >> 8) - 127) * (1.f / 128.f));
-  } else {
-    return __ldg(reinterpret_cast<const float2*>(p) + g);
-  }
-}
-
 template <int FMT, bool POWER>
 __global__ void __launch_bounds__(THREADS) rchan_kernel(RParams P) {
   extern __shared__ float2 xs[];                     // [down][qlen]
@@ -376,19 +390,9 @@ __global__ void __launch_bounds__(THREADS) rchan_kernel(RParams P) {
           continue;
         }
         const long long ih = (P.q0 + (long long)nl[k] * P.down) / P.up;   // newest input of the output
-        const long long p = ((ih % P.fs) * P.dmod[c]) % P.fs;              // its exact mixer phase, in cycles * fs
-        double sn, cs;
-        sincospi(-2.0 * (double)p / (double)P.fs, &sn, &cs);
-        const double yr = (double)acc[i][k].x * cs - (double)acc[i][k].y * sn;
-        const double yi = (double)acc[i][k].x * sn + (double)acc[i][k].y * cs;
-        const double gn = 128.0 * (double)P.gain[c];
-        double vr = rint(127.0 + gn * yr), vi = rint(127.0 + gn * yi);
-        clipped[i] += (vr < 0 || vr > 255) + (vi < 0 || vi > 255);
-        vr = fmin(fmax(vr, 0.0), 255.0);
-        vi = fmin(fmax(vi, 0.0), 255.0);
-        unsigned char* o = P.out + (size_t)c * P.out_stride + 2 * (size_t)nl[k];
-        o[0] = (unsigned char)vr;
-        o[1] = (unsigned char)vi;
+        const long long p = ((ih % P.fs) * P.step[c]) % P.fs;              // its exact mixer phase, in cycles * fs
+        clipped[i] += rotate_quantise(acc[i][k], p, P.fs, 128.0 * (double)P.gain[c],
+                                      P.out + (size_t)c * P.out_stride + 2 * (size_t)nl[k]);
       }
     }
   }
@@ -397,9 +401,7 @@ __global__ void __launch_bounds__(THREADS) rchan_kernel(RParams P) {
     const int c = c0 + i;
     if (c >= P.n_ch) break;
     if (POWER) {
-      double s = pws[i];
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) s += __shfl_down_sync(0xffffffffu, s, o);
+      const double s = warp_sum(pws[i]);
       if (lane == 0) P.pw[(size_t)c * gridDim.x + tile] = s;
     } else {
       const unsigned n = __reduce_add_sync(0xffffffffu, clipped[i]);
@@ -468,24 +470,6 @@ static bool meets_spec_fft(const std::vector<float>& h, double F, double gain) {
   return pass_ok(resp(kPass)) && stop_ok(resp(kStop));
 }
 
-// Kaiser-windowed sinc of odd length L at the rate F with DC gain `gain` (the rounding of kaiser_sinc, scaled in double).
-static void kaiser_sinc_gain(int L, double F, double gain, std::vector<float>& out) {
-  const int M = (L - 1) / 2;
-  const double beta = kaiser_beta(), i0b = bessel_i0(beta), fcn = 2 * kCut / F;
-  std::vector<double> h(L);
-  double sum = 0;
-  for (int n = 0; n < L; n++) {
-    const int m = n - M;
-    const double a = L > 1 ? 2.0 * n / (L - 1) - 1.0 : 0.0;
-    const double w = bessel_i0(beta * std::sqrt(std::max(0.0, 1 - a * a))) / i0b;
-    const double s = m == 0 ? fcn : std::sin(M_PI * fcn * m) / (M_PI * m);
-    h[n] = s * w;
-    sum += h[n];
-  }
-  out.resize(L);
-  for (int n = 0; n < L; n++) out[n] = (float)(gain * h[n] / sum);
-}
-
 // The prototype for fs_in = 1.92 MHz * down / up at F = up * fs_in, DC gain up.  up = 1 is design() itself; otherwise the
 // shortest odd length about the Kaiser estimate that meets the spec on the FFT grid and whose length - 2 fails it,
 // found by doubling steps and bisection (the spec holds from some length on), so that L ~ 10 000 takes a few FFTs.
@@ -493,7 +477,7 @@ static int design_rational(long long fs_in, int up, std::vector<float>& h) {
   if (up == 1) return design((double)fs_in, h);
   const double F = (double)up * (double)fs_in, gain = up;
   auto ok = [&](int L, std::vector<float>& g) {
-    kaiser_sinc_gain(L, F, gain, g);
+    kaiser_sinc(L, F, gain, g);
     return meets_spec_fft(g, F, gain);
   };
   const double dw = 2 * M_PI * (kStop - kPass) / F;
@@ -548,7 +532,9 @@ using namespace lcs::chn;
 
 struct lcs_chan {
   lcs_ctx* ctx = nullptr;
-  int D = 0, L = 0, M = 0;
+  // fs / 1.92 MHz = down / up in lowest terms (decimation by D: up = 1, down = D); samples of esz bytes in format fmt;
+  // L = 2M + 1 prototype taps, J = 2M / up + 1 of them per output; a tile is 32 * RM * up outputs
+  int fmt = LCS_IQ_CI16, esz = 4, up = 1, down = 0, L = 0, M = 0, J = 0, RM = 1;
   long long fs = 0;
   uint32_t n_ch = 0;
   std::vector<float> h;
@@ -558,19 +544,13 @@ struct lcs_chan {
   DevBuf<double2> d_taps64;
   DevBuf<long long> d_step;
   DevBuf<float> d_gain;
-  DevBuf<int> d_in;
+  DevBuf<unsigned char> d_in;
   DevBuf<unsigned char> d_out;
   DevBuf<unsigned long long> d_clip;
   DevBuf<double> d_pw;
   uint32_t chunk = TILE;                 // outputs per launch (bounds the device scratch)
-  std::vector<int> carry;                // stream samples [n_out*D - M, n_in) (zeros before the stream starts)
+  std::vector<unsigned char> carry;      // stream samples [i_hi(n_out) - (J-1), n_in) (zeros before the stream starts)
   uint64_t n_in = 0, n_out = 0;
-  // rational channelizer (lcs_chan_create_rational other than up = 1 with ci16, which is an lcs_chan_create one): D is
-  // unused, taps are [n_ch][up][J], step holds delta mod fs, and the carry is raw samples of esz bytes
-  bool rat = false;
-  int fmt = LCS_IQ_CI16, esz = 4, up = 1, down = 0, J = 0, RM = 1;
-  std::vector<unsigned char> rcarry;     // stream samples [i_hi(n_out) - (J-1), n_in) (zeros before the stream starts)
-  DevBuf<unsigned char> d_rin;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   double kernel_ms = 0;
   uint64_t kernel_launches = 0;
@@ -582,170 +562,156 @@ struct lcs_chan {
 
 namespace {
 
-// outputs after n input samples of a stream
-uint64_t outputs_after(int D, int M, uint64_t n) { return n >= (uint64_t)M + 1 ? (n - 1 - M) / D + 1 : 0; }
-
-// Outputs [0, n_out) of the virtual input a (na samples) ++ b (nb samples), whose sample 0 is the first input of output 0
-// (stream output n_abs0).  power: per-channel sums of |y|^2 are added to pw_sum; otherwise bytes go to out (row stride
-// out_stride, on the device or the host) and clip counts to d_clip.
-lcs_status run(lcs_chan* c, const int* a, size_t na, const int* b, size_t nb, uint64_t n_abs0, uint64_t n_out, bool power,
-               unsigned char* out, size_t out_stride, bool out_dev, std::vector<double>* pw_sum) {
-  lcs_ctx* ctx = c->ctx;
-  cudaStream_t st = ctx->streams[0];
-  const size_t span_max = (size_t)(c->chunk - 1) * c->D + 2 * c->M + 1;
-  LCS_CUDA(ctx, c->d_in.ensure(span_max + (size_t)TILE * c->D));
-  if (!power && !out_dev) LCS_CUDA(ctx, c->d_out.ensure((size_t)c->n_ch * c->chunk * 2));
-  if (power) LCS_CUDA(ctx, c->d_pw.ensure((size_t)c->n_ch * (c->chunk / TILE)));
-  const int qlen = TILE + (2 * c->M) / c->D + 1;
-  const size_t smem = (size_t)smem_bytes(c->D, c->M);
-  std::vector<double> pw;
-  for (uint64_t e0 = 0; e0 < n_out; e0 += c->chunk) {
-    const uint32_t ne = (uint32_t)std::min<uint64_t>(c->chunk, n_out - e0);
-    const size_t lo = (size_t)e0 * c->D;
-    const size_t hi = std::min(lo + (size_t)(ne - 1) * c->D + 2 * c->M + 1, na + nb);
-    // samples [lo, hi) of a ++ b
-    if (lo < na) LCS_CUDA(ctx, cudaMemcpyAsync(c->d_in.p, a + lo, (std::min(hi, na) - lo) * 4, cudaMemcpyHostToDevice, st));
-    if (hi > na) {
-      const size_t s = std::max(lo, na);
-      LCS_CUDA(ctx, cudaMemcpyAsync(c->d_in.p + (s - lo), b + (s - na), (hi - s) * 4, cudaMemcpyHostToDevice, st));
-    }
-    Params P;
-    P.in = c->d_in.p;
-    P.n_in = (long long)(hi - lo);
-    P.D = c->D;
-    P.L = c->L;
-    P.M = c->M;
-    P.qlen = qlen;
-    P.n_out = (int)ne;
-    P.n0 = (long long)(n_abs0 + e0);
-    P.n_ch = (int)c->n_ch;
-    P.taps = c->d_taps.p;
-    P.taps64 = c->d_taps64.p;
-    P.step = c->d_step.p;
-    P.fs = c->fs;
-    P.gain = c->d_gain.p;
-    P.out = out_dev ? out + 2 * e0 : c->d_out.p;
-    P.out_stride = out_dev ? out_stride : (size_t)ne * 2;
-    P.clip = c->d_clip.p;
-    P.pw = c->d_pw.p;
-    const dim3 grid((ne + TILE - 1) / TILE, (c->n_ch + CH_CTA - 1) / CH_CTA);
-    LCS_CUDA(ctx, cudaEventRecord(c->ev0, st));
-    if (power)
-      chan_kernel<true><<<grid, THREADS, smem, st>>>(P);
-    else
-      chan_kernel<false><<<grid, THREADS, smem, st>>>(P);
-    ctx->launches++;
-    LCS_CUDA(ctx, cudaGetLastError());
-    LCS_CUDA(ctx, cudaEventRecord(c->ev1, st));
-    if (power) {
-      pw.resize((size_t)c->n_ch * grid.x);
-      LCS_CUDA(ctx, cudaMemcpyAsync(pw.data(), c->d_pw.p, pw.size() * 8, cudaMemcpyDeviceToHost, st));
-    } else if (!out_dev) {
-      LCS_CUDA(ctx, cudaMemcpy2DAsync(out + 2 * e0, out_stride, c->d_out.p, (size_t)ne * 2, (size_t)ne * 2, c->n_ch,
-                                      cudaMemcpyDeviceToHost, st));
-    }
-    LCS_CUDA(ctx, cudaStreamSynchronize(st));
-    float ms = 0;
-    LCS_CUDA(ctx, cudaEventElapsedTime(&ms, c->ev0, c->ev1));
-    c->kernel_ms += ms;
-    c->kernel_launches++;
-    if (power)   // fixed order: tiles of a chunk, chunks in stream order
-      for (uint32_t ch = 0; ch < c->n_ch; ch++)
-        for (uint32_t t = 0; t < grid.x; t++) (*pw_sum)[ch] += pw[(size_t)ch * grid.x + t];
-  }
-  return LCS_OK;
-}
-
 lcs_status cfail(const lcs_chan* c, const char* msg) { return fail(c ? c->ctx : nullptr, LCS_ERR_ARG, msg); }
 
-// ---- rational channelizer ----
+// chan_kernel (the faster one, with its own tap table) serves ci16 at D * 1.92 MHz, rchan_kernel everything else
+bool decimating_kernel(const lcs_chan* c) { return c->up == 1 && c->fmt == LCS_IQ_CI16; }
+
 // newest input of output n, and the first input the outputs from n on need
-long long r_ihi(const lcs_chan* c, uint64_t n) { return (long long)((n * c->down + c->M) / c->up); }
-long long r_first(const lcs_chan* c, uint64_t n) { return r_ihi(c, n) - (c->J - 1); }
-uint64_t r_outputs_after(const lcs_chan* c, uint64_t n) {
+long long newest_input(const lcs_chan* c, uint64_t n) { return (long long)((n * c->down + c->M) / c->up); }
+long long first_input(const lcs_chan* c, uint64_t n) { return newest_input(c, n) - (c->J - 1); }
+// outputs after n input samples of a stream
+uint64_t outputs_after(const lcs_chan* c, uint64_t n) {
   const uint64_t q = n * c->up;
   return q >= (uint64_t)c->M + 1 ? (q - 1 - c->M) / c->down + 1 : 0;
 }
-uint64_t chan_outputs_after(const lcs_chan* c, uint64_t n) { return c->rat ? r_outputs_after(c, n) : outputs_after(c->D, c->M, n); }
 // n samples of value 0 in the channelizer's format (cu8 127)
-std::vector<unsigned char> r_zeros(const lcs_chan* c, size_t n) {
+std::vector<unsigned char> zero_samples(const lcs_chan* c, size_t n) {
   return std::vector<unsigned char>(n * c->esz, c->fmt == LCS_IQ_CU8 ? 127 : 0);
 }
-int r_outputs_per_tile(const lcs_chan* c) { return 32 * c->RM * c->up; }
-size_t r_smem(int up, int down, int J, int RM) {   // the tile: down rows of qlen samples
-  const size_t span_max = (size_t)32 * RM * down + J;
-  return (size_t)down * ((span_max + down - 1) / down) * sizeof(float2);
+int outputs_per_tile(const lcs_chan* c) { return 32 * c->RM * c->up; }
+size_t sample_bytes(int fmt) {
+  return fmt == LCS_IQ_CI16 ? 4 : fmt == LCS_IQ_CS8 || fmt == LCS_IQ_CU8 ? 2 : fmt == LCS_IQ_CF32 ? 8 : 0;
 }
 
 template <int FMT>
-void r_launch(bool power, dim3 grid, size_t smem, cudaStream_t st, const RParams& P) {
+void launch_rchan(bool power, dim3 grid, size_t smem, cudaStream_t st, const RParams& P) {
   if (power)
     rchan_kernel<FMT, true><<<grid, THREADS, smem, st>>>(P);
   else
     rchan_kernel<FMT, false><<<grid, THREADS, smem, st>>>(P);
 }
 
+// One launch of the channelizer's kernel: `shared` assigns the fields both kernels read, the rest is the kernel's own.
+template <class F>
+void launch(const lcs_chan* c, bool power, dim3 grid, size_t smem, cudaStream_t st, F shared) {
+  if (decimating_kernel(c)) {
+    Params P;
+    shared(P);
+    P.L = c->L;
+    P.M = c->M;
+    if (power)
+      chan_kernel<true><<<grid, THREADS, smem, st>>>(P);
+    else
+      chan_kernel<false><<<grid, THREADS, smem, st>>>(P);
+    return;
+  }
+  RParams P;
+  shared(P);
+  P.up = c->up;
+  P.J = c->J;
+  P.RM = c->RM;
+  P.q0 = P.n0 * c->down + c->M;
+  switch (c->fmt) {
+    case LCS_IQ_CI16: launch_rchan<LCS_IQ_CI16>(power, grid, smem, st, P); break;
+    case LCS_IQ_CS8: launch_rchan<LCS_IQ_CS8>(power, grid, smem, st, P); break;
+    case LCS_IQ_CU8: launch_rchan<LCS_IQ_CU8>(power, grid, smem, st, P); break;
+    default: launch_rchan<LCS_IQ_CF32>(power, grid, smem, st, P); break;
+  }
+}
+
 template <int FMT>
-cudaError_t r_set_smem() {
+cudaError_t set_rchan_smem() {
   cudaError_t e = cudaFuncSetAttribute(rchan_kernel<FMT, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, RSMEM_CAP);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(rchan_kernel<FMT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, RSMEM_CAP);
   return e;
 }
 
-// run() for a rational channelizer: outputs [0, n_out) of the virtual input a ++ b (raw samples), whose sample 0 is the
-// first input of output 0 (stream output n_abs0).
-lcs_status run_r(lcs_chan* c, const unsigned char* a, size_t na, const unsigned char* b, size_t nb, uint64_t n_abs0,
-                 uint64_t n_out, bool power, unsigned char* out, size_t out_stride, bool out_dev, std::vector<double>* pw_sum) {
+// The per-channel complex taps (float and double) and epilogue phase step in the format of the channelizer's kernel.
+void build_taps(lcs_chan* c, std::vector<float2>& taps, std::vector<double2>& taps64) {
+  const long long fs = c->fs;
+  const int up = c->up, J = c->J;
+  const bool centre = decimating_kernel(c);
+  taps.resize((size_t)c->n_ch * (centre ? c->L : up * J));
+  taps64.resize(taps.size());
+  c->step.resize(c->n_ch);
+  for (uint32_t ch = 0; ch < c->n_ch; ch++) {
+    const long long delta = c->delta[ch];
+    if (centre) {   // referred to the centre tap, [n_ch][L]; the phase advances by D * delta per output
+      c->step[ch] = (((long long)c->down * delta) % fs + fs) % fs;
+      for (int t = 0; t < c->L; t++) {
+        const long long p = (((long long)(t - c->M) * delta) % fs + fs) % fs;
+        const double a = 2 * M_PI * (double)p / (double)fs;
+        const double2 g = make_double2((double)c->h[t] * std::cos(a), (double)c->h[t] * std::sin(a));
+        taps64[(size_t)ch * c->L + t] = g;
+        taps[(size_t)ch * c->L + t] = make_float2((float)g.x, (float)g.y);
+      }
+      continue;
+    }
+    // referred to the newest input, one branch per output phase, [n_ch][up][J]; the phase advances by delta per input
+    c->step[ch] = (delta % fs + fs) % fs;
+    for (int j = 0; j < J; j++) {
+      const long long p = (((long long)j * delta) % fs + fs) % fs;
+      const double a = 2 * M_PI * (double)p / (double)fs, ca = std::cos(a), sa = std::sin(a);
+      for (int phi = 0; phi < up; phi++) {
+        const int k = phi + j * up;
+        const double hk = k <= 2 * c->M ? (double)c->h[k] : 0.0;
+        const size_t i = ((size_t)ch * up + phi) * J + j;
+        taps64[i] = make_double2(hk * ca, hk * sa);
+        taps[i] = make_float2((float)taps64[i].x, (float)taps64[i].y);
+      }
+    }
+  }
+}
+
+// Outputs [0, n_out) of the virtual input a (na samples) ++ b (nb samples) in the channelizer's format, whose sample 0 is
+// the first input of output 0 (stream output n_abs0).  power: per-channel sums of |y|^2 are added to pw_sum; otherwise
+// bytes go to out (row stride out_stride, on the device or the host) and clip counts to d_clip.
+lcs_status run(lcs_chan* c, const unsigned char* a, size_t na, const unsigned char* b, size_t nb, uint64_t n_abs0,
+               uint64_t n_out, bool power, unsigned char* out, size_t out_stride, bool out_dev, std::vector<double>* pw_sum) {
   lcs_ctx* ctx = c->ctx;
   cudaStream_t st = ctx->streams[0];
-  const int T = r_outputs_per_tile(c);
+  const int T = outputs_per_tile(c);
   const size_t es = c->esz;
   const size_t span_max = (size_t)c->chunk * c->down / c->up + c->J + 2;
-  LCS_CUDA(ctx, c->d_rin.ensure(span_max * es));
+  LCS_CUDA(ctx, c->d_in.ensure(span_max * es));
   if (!power && !out_dev) LCS_CUDA(ctx, c->d_out.ensure((size_t)c->n_ch * c->chunk * 2));
   if (power) LCS_CUDA(ctx, c->d_pw.ensure((size_t)c->n_ch * ((c->chunk + T - 1) / T)));
-  const size_t smem = r_smem(c->up, c->down, c->J, c->RM);
-  const long long base = r_first(c, n_abs0);
+  const size_t smem = tile_smem(c->down, c->J, c->RM);
+  const long long base = first_input(c, n_abs0);
   std::vector<double> pw;
   for (uint64_t e0 = 0; e0 < n_out; e0 += c->chunk) {
     const uint32_t ne = (uint32_t)std::min<uint64_t>(c->chunk, n_out - e0);
     const uint64_t n0 = n_abs0 + e0;
-    const size_t lo = (size_t)(r_first(c, n0) - base);
-    const size_t hi = std::min((size_t)(r_ihi(c, n0 + ne - 1) + 1 - base), na + nb);
-    if (lo < na) LCS_CUDA(ctx, cudaMemcpyAsync(c->d_rin.p, a + lo * es, (std::min(hi, na) - lo) * es, cudaMemcpyHostToDevice, st));
+    // samples [lo, hi) of a ++ b
+    const size_t lo = (size_t)(first_input(c, n0) - base);
+    const size_t hi = std::min((size_t)(newest_input(c, n0 + ne - 1) + 1 - base), na + nb);
+    if (lo < na) LCS_CUDA(ctx, cudaMemcpyAsync(c->d_in.p, a + lo * es, (std::min(hi, na) - lo) * es, cudaMemcpyHostToDevice, st));
     if (hi > na) {
       const size_t s = std::max(lo, na);
-      LCS_CUDA(ctx, cudaMemcpyAsync(c->d_rin.p + (s - lo) * es, b + (s - na) * es, (hi - s) * es, cudaMemcpyHostToDevice, st));
+      LCS_CUDA(ctx, cudaMemcpyAsync(c->d_in.p + (s - lo) * es, b + (s - na) * es, (hi - s) * es, cudaMemcpyHostToDevice, st));
     }
-    RParams P;
-    P.in = c->d_rin.p;
-    P.n_in = (long long)(hi - lo);
-    P.up = c->up;
-    P.down = c->down;
-    P.J = c->J;
-    P.RM = c->RM;
-    P.qlen = (int)(smem / sizeof(float2) / c->down);
-    P.q0 = (long long)(n0 * c->down + c->M);
-    P.n_out = (int)ne;
-    P.n0 = (long long)n0;
-    P.n_ch = (int)c->n_ch;
-    P.taps = c->d_taps.p;
-    P.taps64 = c->d_taps64.p;
-    P.dmod = c->d_step.p;
-    P.fs = c->fs;
-    P.gain = c->d_gain.p;
-    P.out = out_dev ? out + 2 * e0 : c->d_out.p;
-    P.out_stride = out_dev ? out_stride : (size_t)ne * 2;
-    P.clip = c->d_clip.p;
-    P.pw = c->d_pw.p;
+    auto shared = [&](auto& P) {
+      P.in = c->d_in.p;
+      P.n_in = (long long)(hi - lo);
+      P.down = c->down;
+      P.qlen = tile_qlen(c->down, c->J, c->RM);
+      P.n_out = (int)ne;
+      P.n0 = (long long)n0;
+      P.n_ch = (int)c->n_ch;
+      P.taps = c->d_taps.p;
+      P.taps64 = c->d_taps64.p;
+      P.step = c->d_step.p;
+      P.fs = c->fs;
+      P.gain = c->d_gain.p;
+      P.out = out_dev ? out + 2 * e0 : c->d_out.p;
+      P.out_stride = out_dev ? out_stride : (size_t)ne * 2;
+      P.clip = c->d_clip.p;
+      P.pw = c->d_pw.p;
+    };
     const dim3 grid((ne + T - 1) / T, (c->n_ch + CH_CTA - 1) / CH_CTA);
     LCS_CUDA(ctx, cudaEventRecord(c->ev0, st));
-    switch (c->fmt) {
-      case LCS_IQ_CI16: r_launch<LCS_IQ_CI16>(power, grid, smem, st, P); break;
-      case LCS_IQ_CS8: r_launch<LCS_IQ_CS8>(power, grid, smem, st, P); break;
-      case LCS_IQ_CU8: r_launch<LCS_IQ_CU8>(power, grid, smem, st, P); break;
-      default: r_launch<LCS_IQ_CF32>(power, grid, smem, st, P); break;
-    }
+    launch(c, power, grid, smem, st, shared);
     ctx->launches++;
     LCS_CUDA(ctx, cudaGetLastError());
     LCS_CUDA(ctx, cudaEventRecord(c->ev1, st));
@@ -768,60 +734,78 @@ lcs_status run_r(lcs_chan* c, const unsigned char* a, size_t na, const unsigned 
   return LCS_OK;
 }
 
-lcs_status r_push(lcs_chan* c, const void* iq_host, uint32_t n_in, uint8_t* out, uint32_t out_capacity, int out_on_device,
-                  uint32_t* n_out, uint64_t* n_clipped) {
-  if ((!iq_host && n_in) || !n_out) return cfail(c, "lcs_chan_push: null pointer");
-  const uint64_t k = r_outputs_after(c, c->n_in + n_in) - c->n_out;
-  if (k > out_capacity) return cfail(c, "lcs_chan_push: out_capacity is smaller than the outputs of this push");
-  if (k && !out) return cfail(c, "lcs_chan_push: null output");
-  LCS_CUDA(c->ctx, cudaSetDevice(c->ctx->device));
-  LCS_CUDA(c->ctx, cudaMemsetAsync(c->d_clip.p, 0, c->n_ch * 8, c->ctx->streams[0]));
-  const unsigned char* b = static_cast<const unsigned char*>(iq_host);
-  const size_t es = c->esz, na = c->rcarry.size() / es;
-  if (k) {
-    lcs_status rc = run_r(c, c->rcarry.data(), na, b, n_in, c->n_out, k, false, out, (size_t)out_capacity * 2,
-                          out_on_device != 0, nullptr);
-    if (rc != LCS_OK) return rc;
+// What lcs_chan_create and lcs_chan_create_rational share once the rate and format are known to be allowed: `who` is the
+// caller's name in the error texts.
+lcs_status create(lcs_ctx* ctx, const std::string& who, long long fs, int up, int down, int fmt, double fc_in,
+                  uint32_t n_ch, const double* fc_ch, const float* gain, lcs_chan** out) {
+  if (n_ch < 1 || n_ch > 1024) return fail(ctx, LCS_ERR_ARG, who + ": n_ch must be in [1, 1024]");
+  if (!std::isfinite(fc_in)) return fail(ctx, LCS_ERR_ARG, who + ": fc_in is not finite");
+  std::vector<long long> delta(n_ch);
+  for (uint32_t c = 0; c < n_ch; c++) {
+    const double d = fc_ch[c] - fc_in;
+    if (!std::isfinite(d) || std::fabs(d - std::round(d)) > 1e-6)
+      return fail(ctx, LCS_ERR_ARG, who + ": channel offset fc_ch - fc_in is not an integer number of Hz");
+    delta[c] = (long long)std::llround(d);
+    if (2 * std::llabs(delta[c]) > fs - 1920000)
+      return fail(ctx, LCS_ERR_ARG, who + ": channel band (+-0.96 MHz) outside the input band");
+    if (gain && !(std::isfinite(gain[c]) && gain[c] > 0)) return fail(ctx, LCS_ERR_ARG, who + ": gain must be finite and > 0");
   }
-  // keep the samples from the first input of the next output on
-  const size_t drop = (size_t)(r_first(c, c->n_out + k) - r_first(c, c->n_out));
-  std::vector<unsigned char> nc;
-  nc.reserve((na + n_in - drop) * es);
-  if (drop < na) nc.insert(nc.end(), c->rcarry.begin() + drop * es, c->rcarry.end());
-  nc.insert(nc.end(), b + (drop > na ? drop - na : 0) * es, b + (size_t)n_in * es);
-  c->rcarry.swap(nc);
-  c->n_in += n_in;
-  c->n_out += k;
-  *n_out = (uint32_t)k;
-  if (n_clipped) {
-    if (k)
-      LCS_CUDA(c->ctx, cudaMemcpy(n_clipped, c->d_clip.p, c->n_ch * 8, cudaMemcpyDeviceToHost));
-    else
-      std::memset(n_clipped, 0, c->n_ch * 8);
+  lcs_chan* c = new (std::nothrow) lcs_chan();
+  if (!c) return fail(ctx, LCS_ERR_STATE, who + ": out of memory");
+  c->ctx = ctx;
+  c->fmt = fmt;
+  c->esz = (int)sample_bytes(fmt);
+  c->up = up;
+  c->down = down;
+  c->fs = fs;
+  c->n_ch = n_ch;
+  c->L = design_rational(fs, up, c->h);
+  if (!c->L) {
+    delete c;
+    return fail(ctx, LCS_ERR_RANGE, who + ": no filter up to the tap limit meets the spec");
   }
+  c->M = (c->L - 1) / 2;
+  c->J = 2 * c->M / up + 1;
+  c->RM = (R + up - 1) / up;                // the lane slots of a tile cover up * RM outputs per m
+  c->delta = delta;
+  c->gain.assign(n_ch, 1.0f);
+  if (gain) c->gain.assign(gain, gain + n_ch);
+  c->carry = zero_samples(c, (size_t)-first_input(c, 0));
+  if (tile_smem(down, c->J, c->RM) > (size_t)RSMEM_CAP) {
+    delete c;
+    return fail(ctx, LCS_ERR_RANGE, who + ": the input tile exceeds shared memory");
+  }
+  // outputs per launch, whole tiles: device output scratch <= 32 MB, input <= 64 MB
+  const uint64_t T = (uint64_t)outputs_per_tile(c);
+  const uint64_t by_out = (32ull << 20) / (2ull * n_ch), by_in = (64ull << 20) / c->esz * up / down;
+  c->chunk = (uint32_t)std::max<uint64_t>(T, std::min(by_out, by_in) / T * T);
+  std::vector<float2> taps;
+  std::vector<double2> taps64;
+  build_taps(c, taps, taps64);
+  cudaError_t e = cudaSetDevice(ctx->device);
+  if (e == cudaSuccess) e = c->d_taps.alloc(taps.size());
+  if (e == cudaSuccess) e = c->d_taps64.alloc(taps64.size());
+  if (e == cudaSuccess) e = c->d_step.alloc(n_ch);
+  if (e == cudaSuccess) e = c->d_gain.alloc(n_ch);
+  if (e == cudaSuccess) e = c->d_clip.alloc(n_ch);
+  if (e == cudaSuccess) e = cudaMemcpy(c->d_taps.p, taps.data(), taps.size() * sizeof(float2), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = cudaMemcpy(c->d_taps64.p, taps64.data(), taps64.size() * sizeof(double2), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = cudaMemcpy(c->d_step.p, c->step.data(), n_ch * 8, cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = cudaMemcpy(c->d_gain.p, c->gain.data(), n_ch * 4, cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = cudaEventCreate(&c->ev0);
+  if (e == cudaSuccess) e = cudaEventCreate(&c->ev1);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(chan_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_CAP);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(chan_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_CAP);
+  if (e == cudaSuccess) e = set_rchan_smem<LCS_IQ_CI16>();
+  if (e == cudaSuccess) e = set_rchan_smem<LCS_IQ_CS8>();
+  if (e == cudaSuccess) e = set_rchan_smem<LCS_IQ_CU8>();
+  if (e == cudaSuccess) e = set_rchan_smem<LCS_IQ_CF32>();
+  if (e != cudaSuccess) {
+    delete c;
+    return fail(ctx, LCS_ERR_CUDA, who + ": " + cudaGetErrorString(e));
+  }
+  *out = c;
   return LCS_OK;
-}
-
-lcs_status r_auto_gain(lcs_chan* c, const void* iq_host, uint32_t n) {
-  if (!iq_host) return cfail(c, "lcs_chan_auto_gain: null samples");
-  const uint64_t n_out = r_outputs_after(c, n);           // what a fresh channelizer would produce
-  if (n_out == 0) return cfail(c, "lcs_chan_auto_gain: fewer samples than one output needs");
-  LCS_CUDA(c->ctx, cudaSetDevice(c->ctx->device));
-  const std::vector<unsigned char> zeros = r_zeros(c, (size_t)-r_first(c, 0));
-  std::vector<double> sum(c->n_ch, 0.0);
-  lcs_status rc = run_r(c, zeros.data(), zeros.size() / c->esz, static_cast<const unsigned char*>(iq_host), n, 0, n_out,
-                        true, nullptr, 0, false, &sum);
-  if (rc != LCS_OK) return rc;
-  for (uint32_t ch = 0; ch < c->n_ch; ch++) {
-    const double ms = sum[ch] / (double)n_out;
-    c->gain[ch] = ms > 0 ? (float)(0.25 / std::sqrt(ms)) : 1.0f;
-  }
-  LCS_CUDA(c->ctx, cudaMemcpy(c->d_gain.p, c->gain.data(), c->n_ch * 4, cudaMemcpyHostToDevice));
-  return LCS_OK;
-}
-
-size_t r_sample_bytes(int fmt) {
-  return fmt == LCS_IQ_CI16 ? 4 : fmt == LCS_IQ_CS8 || fmt == LCS_IQ_CU8 ? 2 : fmt == LCS_IQ_CF32 ? 8 : 0;
 }
 
 }  // namespace
@@ -839,156 +823,6 @@ lcs_status lcs_chan_design_taps(double fs_in, float* taps, uint32_t* n_taps) {
     std::memcpy(taps, h.data(), L * sizeof(float));
   }
   *n_taps = (uint32_t)L;
-  return LCS_OK;
-}
-
-lcs_status lcs_chan_create(lcs_ctx* ctx, double fs_in, double fc_in, uint32_t n_ch, const double* fc_ch, const float* gain,
-                           lcs_chan** out) {
-  if (!ctx || !out || !fc_ch) return fail(ctx, LCS_ERR_ARG, "lcs_chan_create: null argument");
-  int D = 0;
-  if (!decimation(fs_in, &D)) return fail(ctx, LCS_ERR_ARG, "lcs_chan_create: fs_in must be D * 1.92 MHz, D in [2, 64]");
-  if (n_ch < 1 || n_ch > 1024) return fail(ctx, LCS_ERR_ARG, "lcs_chan_create: n_ch must be in [1, 1024]");
-  if (!std::isfinite(fc_in)) return fail(ctx, LCS_ERR_ARG, "lcs_chan_create: fc_in is not finite");
-  const long long fs = (long long)D * 1920000LL;
-  std::vector<long long> delta(n_ch);
-  for (uint32_t c = 0; c < n_ch; c++) {
-    const double d = fc_ch[c] - fc_in;
-    if (!std::isfinite(d) || std::fabs(d - std::round(d)) > 1e-6)
-      return fail(ctx, LCS_ERR_ARG, "lcs_chan_create: channel offset fc_ch - fc_in is not an integer number of Hz");
-    delta[c] = (long long)std::llround(d);
-    if (std::llabs(delta[c]) > fs / 2 - 960000)
-      return fail(ctx, LCS_ERR_ARG, "lcs_chan_create: channel band (+-0.96 MHz) outside the input band");
-    if (gain && !(std::isfinite(gain[c]) && gain[c] > 0)) return fail(ctx, LCS_ERR_ARG, "lcs_chan_create: gain must be finite and > 0");
-  }
-  lcs_chan* c = new (std::nothrow) lcs_chan();
-  if (!c) return fail(ctx, LCS_ERR_STATE, "lcs_chan_create: out of memory");
-  c->ctx = ctx;
-  c->D = D;
-  c->fs = fs;
-  c->n_ch = n_ch;
-  c->L = design(D * kFsCh, c->h);
-  c->M = (c->L - 1) / 2;
-  c->delta = delta;
-  c->gain.assign(n_ch, 1.0f);
-  if (gain) c->gain.assign(gain, gain + n_ch);
-  c->carry.assign(c->M, 0);
-  // outputs per launch: device output scratch <= 32 MB, input tile <= 64 MB
-  const uint64_t by_out = (32ull << 20) / (2ull * n_ch), by_in = (64ull << 20) / (4ull * D);
-  c->chunk = (uint32_t)std::max<uint64_t>(TILE, std::min(by_out, by_in) / TILE * TILE);
-  std::vector<float2> taps((size_t)n_ch * c->L);
-  std::vector<double2> taps64((size_t)n_ch * c->L);
-  c->step.resize(n_ch);
-  for (uint32_t ch = 0; ch < n_ch; ch++) {
-    c->step[ch] = (((long long)D * delta[ch]) % fs + fs) % fs;
-    for (int t = 0; t < c->L; t++) {
-      const long long p = (((long long)(t - c->M) * delta[ch]) % fs + fs) % fs;
-      const double a = 2 * M_PI * (double)p / (double)fs;
-      const double2 g = make_double2((double)c->h[t] * std::cos(a), (double)c->h[t] * std::sin(a));
-      taps64[(size_t)ch * c->L + t] = g;
-      taps[(size_t)ch * c->L + t] = make_float2((float)g.x, (float)g.y);
-    }
-  }
-  cudaError_t e = cudaSetDevice(ctx->device);
-  if (e == cudaSuccess) e = c->d_taps.alloc(taps.size());
-  if (e == cudaSuccess) e = c->d_taps64.alloc(taps64.size());
-  if (e == cudaSuccess) e = c->d_step.alloc(n_ch);
-  if (e == cudaSuccess) e = c->d_gain.alloc(n_ch);
-  if (e == cudaSuccess) e = c->d_clip.alloc(n_ch);
-  if (e == cudaSuccess) e = cudaMemcpy(c->d_taps.p, taps.data(), taps.size() * sizeof(float2), cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) e = cudaMemcpy(c->d_taps64.p, taps64.data(), taps64.size() * sizeof(double2), cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) e = cudaMemcpy(c->d_step.p, c->step.data(), n_ch * 8, cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) e = cudaMemcpy(c->d_gain.p, c->gain.data(), n_ch * 4, cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) e = cudaEventCreate(&c->ev0);
-  if (e == cudaSuccess) e = cudaEventCreate(&c->ev1);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(chan_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_CAP);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(chan_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_CAP);
-  if (e != cudaSuccess) {
-    delete c;
-    return fail(ctx, LCS_ERR_CUDA, std::string("lcs_chan_create: ") + cudaGetErrorString(e));
-  }
-  *out = c;
-  return LCS_OK;
-}
-
-void lcs_chan_destroy(lcs_chan* c) {
-  if (!c) return;
-  cudaSetDevice(c->ctx->device);             // its buffers and events belong to the context's device
-  delete c;
-}
-
-lcs_status lcs_chan_auto_gain_ci16(lcs_chan* c, const int16_t* iq_host, uint32_t n) {
-  if (!c) return LCS_ERR_ARG;
-  if (c->rat) {
-    if (c->fmt != LCS_IQ_CI16) return cfail(c, "lcs_chan_auto_gain_ci16: the channelizer's input format is not ci16");
-    return r_auto_gain(c, iq_host, n);
-  }
-  if (!iq_host) return cfail(c, "lcs_chan_auto_gain_ci16: null samples");
-  const uint64_t n_out = outputs_after(c->D, c->M, n);      // what a fresh channelizer would produce
-  if (n_out == 0) return cfail(c, "lcs_chan_auto_gain_ci16: fewer samples than one output needs");
-  LCS_CUDA(c->ctx, cudaSetDevice(c->ctx->device));
-  const std::vector<int> zeros(c->M, 0);
-  std::vector<double> sum(c->n_ch, 0.0);
-  lcs_status rc = run(c, zeros.data(), zeros.size(), reinterpret_cast<const int*>(iq_host), n, 0, n_out, true, nullptr, 0, false, &sum);
-  if (rc != LCS_OK) return rc;
-  for (uint32_t ch = 0; ch < c->n_ch; ch++) {
-    const double ms = sum[ch] / (double)n_out;
-    c->gain[ch] = ms > 0 ? (float)(0.25 / std::sqrt(ms)) : 1.0f;
-  }
-  LCS_CUDA(c->ctx, cudaMemcpy(c->d_gain.p, c->gain.data(), c->n_ch * 4, cudaMemcpyHostToDevice));
-  return LCS_OK;
-}
-
-lcs_status lcs_chan_gain(const lcs_chan* c, float* gain) {
-  if (!c) return LCS_ERR_ARG;
-  if (!gain) return cfail(c, "lcs_chan_gain: null pointer");
-  std::memcpy(gain, c->gain.data(), c->n_ch * sizeof(float));
-  return LCS_OK;
-}
-
-lcs_status lcs_chan_n_out(const lcs_chan* c, uint64_t n_in, uint32_t* n_out) {
-  if (!c) return LCS_ERR_ARG;
-  if (!n_out) return cfail(c, "lcs_chan_n_out: null pointer");
-  const uint64_t k = chan_outputs_after(c, c->n_in + n_in) - c->n_out;
-  if (k > UINT32_MAX) return cfail(c, "lcs_chan_n_out: push too long");
-  *n_out = (uint32_t)k;
-  return LCS_OK;
-}
-
-lcs_status lcs_chan_push_ci16(lcs_chan* c, const int16_t* iq_host, uint32_t n_in, uint8_t* out, uint32_t out_capacity,
-                              int out_on_device, uint32_t* n_out, uint64_t* n_clipped) {
-  if (!c) return LCS_ERR_ARG;
-  if (c->rat) {
-    if (c->fmt != LCS_IQ_CI16) return cfail(c, "lcs_chan_push_ci16: the channelizer's input format is not ci16");
-    return r_push(c, iq_host, n_in, out, out_capacity, out_on_device, n_out, n_clipped);
-  }
-  if ((!iq_host && n_in) || !n_out) return cfail(c, "lcs_chan_push_ci16: null pointer");
-  const uint64_t k = outputs_after(c->D, c->M, c->n_in + n_in) - c->n_out;
-  if (k > out_capacity) return cfail(c, "lcs_chan_push_ci16: out_capacity is smaller than the outputs of this push");
-  if (k && !out) return cfail(c, "lcs_chan_push_ci16: null output");
-  LCS_CUDA(c->ctx, cudaSetDevice(c->ctx->device));
-  LCS_CUDA(c->ctx, cudaMemsetAsync(c->d_clip.p, 0, c->n_ch * 8, c->ctx->streams[0]));
-  const int* b = reinterpret_cast<const int*>(iq_host);
-  if (k) {
-    lcs_status rc = run(c, c->carry.data(), c->carry.size(), b, n_in, c->n_out, k, false, out, (size_t)out_capacity * 2,
-                        out_on_device != 0, nullptr);
-    if (rc != LCS_OK) return rc;
-  }
-  // keep the samples from the first input of the next output on
-  const size_t drop = (size_t)k * c->D, na = c->carry.size();
-  std::vector<int> nc;
-  nc.reserve(na + n_in - drop);
-  if (drop < na) nc.insert(nc.end(), c->carry.begin() + drop, c->carry.end());
-  nc.insert(nc.end(), b + (drop > na ? drop - na : 0), b + n_in);
-  c->carry.swap(nc);
-  c->n_in += n_in;
-  c->n_out += k;
-  *n_out = (uint32_t)k;
-  if (n_clipped) {
-    if (k)
-      LCS_CUDA(c->ctx, cudaMemcpy(n_clipped, c->d_clip.p, c->n_ch * 8, cudaMemcpyDeviceToHost));
-    else
-      std::memset(n_clipped, 0, c->n_ch * 8);
-  }
   return LCS_OK;
 }
 
@@ -1011,6 +845,14 @@ lcs_status lcs_chan_design_rational(double fs_in, uint32_t* up, uint32_t* down, 
   return LCS_OK;
 }
 
+lcs_status lcs_chan_create(lcs_ctx* ctx, double fs_in, double fc_in, uint32_t n_ch, const double* fc_ch, const float* gain,
+                           lcs_chan** out) {
+  if (!ctx || !out || !fc_ch) return fail(ctx, LCS_ERR_ARG, "lcs_chan_create: null argument");
+  int D = 0;
+  if (!decimation(fs_in, &D)) return fail(ctx, LCS_ERR_ARG, "lcs_chan_create: fs_in must be D * 1.92 MHz, D in [2, 64]");
+  return create(ctx, "lcs_chan_create", (long long)D * 1920000LL, 1, D, LCS_IQ_CI16, fc_in, n_ch, fc_ch, gain, out);
+}
+
 lcs_status lcs_chan_create_rational(lcs_ctx* ctx, double fs_in, int iq_format, double fc_in, uint32_t n_ch,
                                     const double* fc_ch, const float* gain, lcs_chan** out) {
   if (!ctx || !out || !fc_ch) return fail(ctx, LCS_ERR_ARG, "lcs_chan_create_rational: null argument");
@@ -1019,107 +861,98 @@ lcs_status lcs_chan_create_rational(lcs_ctx* ctx, double fs_in, int iq_format, d
   if (!rational_rate(fs_in, &fs, &up, &down))
     return fail(ctx, LCS_ERR_ARG, "lcs_chan_create_rational: fs_in must be an integer number of Hz in (1.92, 122.88] MHz "
                                   "with fs_in / 1.92 MHz = down / up, up <= 128, down <= 640");
-  const size_t esz = r_sample_bytes(iq_format);
-  if (!esz) return fail(ctx, LCS_ERR_ARG, "lcs_chan_create_rational: iq_format must be LCS_IQ_CI16, CS8, CU8 or CF32");
-  if (n_ch < 1 || n_ch > 1024) return fail(ctx, LCS_ERR_ARG, "lcs_chan_create_rational: n_ch must be in [1, 1024]");
-  if (!std::isfinite(fc_in)) return fail(ctx, LCS_ERR_ARG, "lcs_chan_create_rational: fc_in is not finite");
-  std::vector<long long> delta(n_ch);
-  for (uint32_t c = 0; c < n_ch; c++) {
-    const double d = fc_ch[c] - fc_in;
-    if (!std::isfinite(d) || std::fabs(d - std::round(d)) > 1e-6)
-      return fail(ctx, LCS_ERR_ARG, "lcs_chan_create_rational: channel offset fc_ch - fc_in is not an integer number of Hz");
-    delta[c] = (long long)std::llround(d);
-    if (2 * std::llabs(delta[c]) > fs - 1920000)
-      return fail(ctx, LCS_ERR_ARG, "lcs_chan_create_rational: channel band (+-0.96 MHz) outside the input band");
-    if (gain && !(std::isfinite(gain[c]) && gain[c] > 0))
-      return fail(ctx, LCS_ERR_ARG, "lcs_chan_create_rational: gain must be finite and > 0");
+  if (!sample_bytes(iq_format))
+    return fail(ctx, LCS_ERR_ARG, "lcs_chan_create_rational: iq_format must be LCS_IQ_CI16, CS8, CU8 or CF32");
+  return create(ctx, "lcs_chan_create_rational", fs, up, down, iq_format, fc_in, n_ch, fc_ch, gain, out);
+}
+
+void lcs_chan_destroy(lcs_chan* c) {
+  if (!c) return;
+  cudaSetDevice(c->ctx->device);             // its buffers and events belong to the context's device
+  delete c;
+}
+
+lcs_status lcs_chan_auto_gain(lcs_chan* c, const void* iq_host, uint32_t n) {
+  if (!c) return LCS_ERR_ARG;
+  if (!iq_host) return cfail(c, "lcs_chan_auto_gain: null samples");
+  const uint64_t n_out = outputs_after(c, n);             // what a fresh channelizer would produce
+  if (n_out == 0) return cfail(c, "lcs_chan_auto_gain: fewer samples than one output needs");
+  LCS_CUDA(c->ctx, cudaSetDevice(c->ctx->device));
+  const std::vector<unsigned char> zeros = zero_samples(c, (size_t)-first_input(c, 0));
+  std::vector<double> sum(c->n_ch, 0.0);
+  lcs_status rc = run(c, zeros.data(), zeros.size() / c->esz, static_cast<const unsigned char*>(iq_host), n, 0, n_out,
+                      true, nullptr, 0, false, &sum);
+  if (rc != LCS_OK) return rc;
+  for (uint32_t ch = 0; ch < c->n_ch; ch++) {
+    const double ms = sum[ch] / (double)n_out;
+    c->gain[ch] = ms > 0 ? (float)(0.25 / std::sqrt(ms)) : 1.0f;
   }
-  // D * 1.92 MHz ci16 is lcs_chan_create's channelizer, bytes, clip counts and auto gain included
-  if (up == 1 && iq_format == LCS_IQ_CI16) return lcs_chan_create(ctx, fs_in, fc_in, n_ch, fc_ch, gain, out);
-  lcs_chan* c = new (std::nothrow) lcs_chan();
-  if (!c) return fail(ctx, LCS_ERR_STATE, "lcs_chan_create_rational: out of memory");
-  c->ctx = ctx;
-  c->rat = true;
-  c->fmt = iq_format;
-  c->esz = (int)esz;
-  c->up = up;
-  c->down = down;
-  c->fs = fs;
-  c->n_ch = n_ch;
-  c->L = design_rational(fs, up, c->h);
-  if (!c->L) {
-    delete c;
-    return fail(ctx, LCS_ERR_RANGE, "lcs_chan_create_rational: no filter up to the tap limit meets the spec");
-  }
-  c->M = (c->L - 1) / 2;
-  c->J = 2 * c->M / up + 1;
-  c->RM = (R + up - 1) / up;                // the lane slots of a tile cover up * RM outputs per m
-  c->delta = delta;
-  c->gain.assign(n_ch, 1.0f);
-  if (gain) c->gain.assign(gain, gain + n_ch);
-  c->rcarry = r_zeros(c, (size_t)-r_first(c, 0));
-  if (r_smem(up, down, c->J, c->RM) > (size_t)RSMEM_CAP) {
-    delete c;
-    return fail(ctx, LCS_ERR_RANGE, "lcs_chan_create_rational: the input tile exceeds shared memory");
-  }
-  // outputs per launch, whole tiles: device output scratch <= 32 MB, input <= 64 MB
-  const uint64_t T = (uint64_t)r_outputs_per_tile(c);
-  const uint64_t by_out = (32ull << 20) / (2ull * n_ch), by_in = (64ull << 20) / esz * up / down;
-  c->chunk = (uint32_t)std::max<uint64_t>(T, std::min(by_out, by_in) / T * T);
-  const int J = c->J;
-  std::vector<float2> taps((size_t)n_ch * up * J);
-  std::vector<double2> taps64(taps.size());
-  c->step.resize(n_ch);
-  for (uint32_t ch = 0; ch < n_ch; ch++) {
-    c->step[ch] = (delta[ch] % fs + fs) % fs;
-    for (int j = 0; j < J; j++) {
-      const long long p = (((long long)j * delta[ch]) % fs + fs) % fs;
-      const double a = 2 * M_PI * (double)p / (double)fs, ca = std::cos(a), sa = std::sin(a);
-      for (int phi = 0; phi < up; phi++) {
-        const int k = phi + j * up;
-        const double hk = k <= 2 * c->M ? (double)c->h[k] : 0.0;
-        const size_t i = ((size_t)ch * up + phi) * J + j;
-        taps64[i] = make_double2(hk * ca, hk * sa);
-        taps[i] = make_float2((float)taps64[i].x, (float)taps64[i].y);
-      }
-    }
-  }
-  cudaError_t e = cudaSetDevice(ctx->device);
-  if (e == cudaSuccess) e = c->d_taps.alloc(taps.size());
-  if (e == cudaSuccess) e = c->d_taps64.alloc(taps64.size());
-  if (e == cudaSuccess) e = c->d_step.alloc(n_ch);
-  if (e == cudaSuccess) e = c->d_gain.alloc(n_ch);
-  if (e == cudaSuccess) e = c->d_clip.alloc(n_ch);
-  if (e == cudaSuccess) e = cudaMemcpy(c->d_taps.p, taps.data(), taps.size() * sizeof(float2), cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) e = cudaMemcpy(c->d_taps64.p, taps64.data(), taps64.size() * sizeof(double2), cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) e = cudaMemcpy(c->d_step.p, c->step.data(), n_ch * 8, cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) e = cudaMemcpy(c->d_gain.p, c->gain.data(), n_ch * 4, cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) e = cudaEventCreate(&c->ev0);
-  if (e == cudaSuccess) e = cudaEventCreate(&c->ev1);
-  if (e == cudaSuccess) e = r_set_smem<LCS_IQ_CI16>();
-  if (e == cudaSuccess) e = r_set_smem<LCS_IQ_CS8>();
-  if (e == cudaSuccess) e = r_set_smem<LCS_IQ_CU8>();
-  if (e == cudaSuccess) e = r_set_smem<LCS_IQ_CF32>();
-  if (e != cudaSuccess) {
-    delete c;
-    return fail(ctx, LCS_ERR_CUDA, std::string("lcs_chan_create_rational: ") + cudaGetErrorString(e));
-  }
-  *out = c;
+  LCS_CUDA(c->ctx, cudaMemcpy(c->d_gain.p, c->gain.data(), c->n_ch * 4, cudaMemcpyHostToDevice));
+  return LCS_OK;
+}
+
+lcs_status lcs_chan_auto_gain_ci16(lcs_chan* c, const int16_t* iq_host, uint32_t n) {
+  if (!c) return LCS_ERR_ARG;
+  if (c->fmt != LCS_IQ_CI16) return cfail(c, "lcs_chan_auto_gain_ci16: the channelizer's input format is not ci16");
+  return lcs_chan_auto_gain(c, iq_host, n);
+}
+
+lcs_status lcs_chan_gain(const lcs_chan* c, float* gain) {
+  if (!c) return LCS_ERR_ARG;
+  if (!gain) return cfail(c, "lcs_chan_gain: null pointer");
+  std::memcpy(gain, c->gain.data(), c->n_ch * sizeof(float));
+  return LCS_OK;
+}
+
+lcs_status lcs_chan_n_out(const lcs_chan* c, uint64_t n_in, uint32_t* n_out) {
+  if (!c) return LCS_ERR_ARG;
+  if (!n_out) return cfail(c, "lcs_chan_n_out: null pointer");
+  const uint64_t k = outputs_after(c, c->n_in + n_in) - c->n_out;
+  if (k > UINT32_MAX) return cfail(c, "lcs_chan_n_out: push too long");
+  *n_out = (uint32_t)k;
   return LCS_OK;
 }
 
 lcs_status lcs_chan_push(lcs_chan* c, const void* iq_host, uint32_t n_in, uint8_t* out, uint32_t out_capacity,
                          int out_on_device, uint32_t* n_out, uint64_t* n_clipped) {
   if (!c) return LCS_ERR_ARG;
-  if (!c->rat)
-    return lcs_chan_push_ci16(c, static_cast<const int16_t*>(iq_host), n_in, out, out_capacity, out_on_device, n_out, n_clipped);
-  return r_push(c, iq_host, n_in, out, out_capacity, out_on_device, n_out, n_clipped);
+  if ((!iq_host && n_in) || !n_out) return cfail(c, "lcs_chan_push: null pointer");
+  const uint64_t k = outputs_after(c, c->n_in + n_in) - c->n_out;
+  if (k > out_capacity) return cfail(c, "lcs_chan_push: out_capacity is smaller than the outputs of this push");
+  if (k && !out) return cfail(c, "lcs_chan_push: null output");
+  LCS_CUDA(c->ctx, cudaSetDevice(c->ctx->device));
+  LCS_CUDA(c->ctx, cudaMemsetAsync(c->d_clip.p, 0, c->n_ch * 8, c->ctx->streams[0]));
+  const unsigned char* b = static_cast<const unsigned char*>(iq_host);
+  const size_t es = c->esz, na = c->carry.size() / es;
+  if (k) {
+    lcs_status rc = run(c, c->carry.data(), na, b, n_in, c->n_out, k, false, out, (size_t)out_capacity * 2,
+                        out_on_device != 0, nullptr);
+    if (rc != LCS_OK) return rc;
+  }
+  // keep the samples from the first input of the next output on
+  const size_t drop = (size_t)(first_input(c, c->n_out + k) - first_input(c, c->n_out));
+  std::vector<unsigned char> nc;
+  nc.reserve((na + n_in - drop) * es);
+  if (drop < na) nc.insert(nc.end(), c->carry.begin() + drop * es, c->carry.end());
+  nc.insert(nc.end(), b + (drop > na ? drop - na : 0) * es, b + (size_t)n_in * es);
+  c->carry.swap(nc);
+  c->n_in += n_in;
+  c->n_out += k;
+  *n_out = (uint32_t)k;
+  if (n_clipped) {
+    if (k)
+      LCS_CUDA(c->ctx, cudaMemcpy(n_clipped, c->d_clip.p, c->n_ch * 8, cudaMemcpyDeviceToHost));
+    else
+      std::memset(n_clipped, 0, c->n_ch * 8);
+  }
+  return LCS_OK;
 }
 
-lcs_status lcs_chan_auto_gain(lcs_chan* c, const void* iq_host, uint32_t n) {
+lcs_status lcs_chan_push_ci16(lcs_chan* c, const int16_t* iq_host, uint32_t n_in, uint8_t* out, uint32_t out_capacity,
+                              int out_on_device, uint32_t* n_out, uint64_t* n_clipped) {
   if (!c) return LCS_ERR_ARG;
-  if (!c->rat) return lcs_chan_auto_gain_ci16(c, static_cast<const int16_t*>(iq_host), n);
-  return r_auto_gain(c, iq_host, n);
+  if (c->fmt != LCS_IQ_CI16) return cfail(c, "lcs_chan_push_ci16: the channelizer's input format is not ci16");
+  return lcs_chan_push(c, iq_host, n_in, out, out_capacity, out_on_device, n_out, n_clipped);
 }
 
 lcs_status lcs_chan_timing_read(lcs_chan* c, double* kernel_ms, uint64_t* launches) {

@@ -620,89 +620,6 @@ def chan_design_taps(fs_in):
     return h
 
 
-def _ci16(iq):
-    iq = np.ascontiguousarray(iq, np.int16)
-    if iq.ndim != 2 or iq.shape[1] != 2:
-        raise ValueError("expected ci16 samples [n][2]")
-    return iq
-
-
-class Channelizer:
-    """lcs_chan: wideband ci16 recording -> one 1.92 Msps cu8 stream per LTE raster channel (DESIGN.md section 4.6)."""
-
-    def __init__(self, ctx, fs_in, fc_in, fc_ch, gain=None):
-        self.ctx = ctx
-        fc = np.ascontiguousarray(np.atleast_1d(fc_ch), np.float64)
-        self.n_ch = fc.size
-        self.fc_ch = fc
-        g = None if gain is None else np.ascontiguousarray(np.broadcast_to(np.asarray(gain, np.float32), (self.n_ch,)))
-        self.taps = chan_design_taps(fs_in)
-        self.M = (self.taps.size - 1) // 2
-        self.D = int(round(fs_in / 1.92e6))
-        self._h = C.c_void_p()
-        _chk(lib().lcs_chan_create(ctx._h, C.c_double(fs_in), C.c_double(fc_in), C.c_uint32(self.n_ch), _p(fc), _p(g),
-                                   C.byref(self._h)), ctx._h)
-
-    def auto_gain(self, iq):
-        """Set every channel's gain to 0.25 / RMS of its output over these samples (the stream is not touched)."""
-        iq = _ci16(iq)
-        _chk(lib().lcs_chan_auto_gain_ci16(self._h, _p(iq), C.c_uint32(iq.shape[0])), self.ctx._h)
-        return self.gain
-
-    @property
-    def gain(self):
-        g = np.zeros(self.n_ch, np.float32)
-        _chk(lib().lcs_chan_gain(self._h, _p(g)), self.ctx._h)
-        return g
-
-    def n_out(self, n_in):
-        k = C.c_uint32(0)
-        _chk(lib().lcs_chan_n_out(self._h, C.c_uint64(n_in), C.byref(k)), self.ctx._h)
-        return k.value
-
-    def push_ci16(self, iq):
-        """Push ci16 [n][2] samples.  Returns (cu8 [n_ch][n_out][2], n_clipped [n_ch])."""
-        iq = _ci16(iq)
-        k = self.n_out(iq.shape[0])
-        out = np.zeros((self.n_ch, k, 2), np.uint8)
-        clip = np.zeros(self.n_ch, np.uint64)
-        got = C.c_uint32(0)
-        _chk(lib().lcs_chan_push_ci16(self._h, _p(iq), C.c_uint32(iq.shape[0]), _p(out), C.c_uint32(k), 0, C.byref(got),
-                                      _p(clip)), self.ctx._h)
-        return out, clip
-
-    def push_ci16_device(self, iq, out):
-        """Push ci16 [n][2] samples, writing the bytes into the uint8 CUDA tensor out [n_ch][capacity][2] from column 0
-        on.  Returns (n_out, n_clipped [n_ch])."""
-        iq = _ci16(iq)
-        if not (out.is_cuda and out.is_contiguous() and str(out.dtype) == "torch.uint8" and out.dim() == 3 and
-                out.shape[0] == self.n_ch and out.shape[2] == 2):
-            raise ValueError("push_ci16_device: expected a contiguous uint8 CUDA tensor [n_ch][capacity][2]")
-        cap = out.shape[1]
-        clip = np.zeros(self.n_ch, np.uint64)
-        got = C.c_uint32(0)
-        _chk(lib().lcs_chan_push_ci16(self._h, _p(iq), C.c_uint32(iq.shape[0]), C.c_void_p(out.data_ptr()),
-                                      C.c_uint32(cap), 1, C.byref(got), _p(clip)), self.ctx._h)
-        return got.value, clip
-
-    def timing_read(self):
-        """(kernel ms, launches) since the last read, from CUDA events around each launch."""
-        ms = C.c_double(0); n = C.c_uint64(0)
-        _chk(lib().lcs_chan_timing_read(self._h, C.byref(ms), C.byref(n)), self.ctx._h)
-        return ms.value, n.value
-
-    def close(self):
-        if self._h:
-            lib().lcs_chan_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-
 def chan_design_rational(fs_in):
     """fs_in / 1.92 MHz = down / up in lowest terms and the prototype low-pass at up * fs_in, DC gain up (host only):
     (up, down, float32 [L])."""
@@ -720,7 +637,7 @@ CHAN_FORMATS = {"ci16": (IQ_CI16, np.int16), "cs8": (IQ_CS8, np.int8), "cu8": (I
 
 class RationalChannelizer:
     """lcs_chan at any allowed SDR rate: a wideband ci16 / cs8 / cu8 / cf32 recording -> one 1.92 Msps cu8 stream per LTE
-    raster channel, resampled by up / down (DESIGN.md section 4.7)."""
+    raster channel, resampled by up / down (DESIGN.md sections 4.6 and 4.7)."""
 
     def __init__(self, ctx, fs_in, fc_in, fc_ch, fmt="ci16", gain=None):
         if fmt not in CHAN_FORMATS:
@@ -733,10 +650,13 @@ class RationalChannelizer:
         self.fc_ch = fc
         g = None if gain is None else np.ascontiguousarray(np.broadcast_to(np.asarray(gain, np.float32), (self.n_ch,)))
         self._h = C.c_void_p()
-        _chk(lib().lcs_chan_create_rational(ctx._h, C.c_double(fs_in), self._iq_format, C.c_double(fc_in),
-                                            C.c_uint32(self.n_ch), _p(fc), _p(g), C.byref(self._h)), ctx._h)
+        _chk(self._create(fs_in, fc_in, fc, g), ctx._h)
         self.up, self.down, self.taps = chan_design_rational(fs_in)
         self.M = (self.taps.size - 1) // 2
+
+    def _create(self, fs_in, fc_in, fc, g):
+        return lib().lcs_chan_create_rational(self.ctx._h, C.c_double(fs_in), self._iq_format, C.c_double(fc_in),
+                                              C.c_uint32(self.n_ch), _p(fc), _p(g), C.byref(self._h))
 
     def _samples(self, iq):
         """iq as a contiguous [n][2] array of the format's dtype (complex64 [n] is accepted for cf32)."""
@@ -804,6 +724,28 @@ class RationalChannelizer:
             self.close()
         except Exception:
             pass
+
+
+class Channelizer(RationalChannelizer):
+    """The ci16 channelizer of DESIGN.md section 4.6, made by lcs_chan_create: fs_in must be D * 1.92 MHz."""
+
+    def __init__(self, ctx, fs_in, fc_in, fc_ch, gain=None):
+        super().__init__(ctx, fs_in, fc_in, fc_ch, "ci16", gain)
+        self.D = self.down
+
+    def _create(self, fs_in, fc_in, fc, g):
+        return lib().lcs_chan_create(self.ctx._h, C.c_double(fs_in), C.c_double(fc_in), C.c_uint32(self.n_ch), _p(fc),
+                                     _p(g), C.byref(self._h))
+
+    def _samples(self, iq):
+        """iq as contiguous int16 [n][2], cast from other integer types."""
+        iq = np.ascontiguousarray(iq, np.int16)
+        if iq.ndim != 2 or iq.shape[1] != 2:
+            raise ValueError("expected ci16 samples [n][2]")
+        return iq
+
+    push_ci16 = RationalChannelizer.push
+    push_ci16_device = RationalChannelizer.push_device
 
 
 def declared_symbols():
