@@ -2,7 +2,7 @@
 // at once (one per centre frequency of a sweep, one per tracked channel) and kept resident in HBM.
 //
 //   host   integer geometry: k_factor fold offsets round_i(m*.005*k_factor*fs) (searcher.cpp:298), their range check,
-//          per-pass minima / spreads of the tensor-core correlator, tile geometry of the FP32 correlator
+//          per-pass staging starts / column offsets of the tensor-core correlator, tile geometry of the FP32 correlator
 //   device plan_build_kernel: the pre-rotated templates conj(fshift(pss_td[t], f_off, fs*k_factor))/137
 //          (searcher.cpp:145-151 with dsp.h:40-53) in double precision, rounded once to FP32 for the CUDA-core
 //          correlator and to 24-bit fixed point, split in three balanced int8 digit planes in wgmma core-matrix order,
@@ -198,24 +198,36 @@ lcs_status planset_build(lcs_ctx* ctx, PlanSet& ps, uint32_t n_cap, uint8_t arm,
         h_smin[((size_t)p * M + m) * g.n_fchunk + ch] = lo;
         max_spread = std::max(max_spread, (uint32_t)(hi - lo));
       }
-    // tensor-core correlator: per pass minimum and per-column offsets
+    // tensor-core correlator: per pass staging start smin[m] and per-column offsets dsh = offset - smin[m].  The kernel
+    // adds half frame m of a fold position in tile (position - run start + dsh) / 256 of its run, half frames of one tile
+    // in order.  smin[m] advances by the smallest step of the pass' offsets from half frame m - 1 to m, so dsh is
+    // non-decreasing in m for every column: the half frames of a position are then added in ascending m, whatever tile
+    // phase its run starts at (so at every batch size and SM count).  smin[m] <= every offset of half frame m, so dsh >= 0.
     for (uint32_t ps_i = 0; ps_i < n_pass && ps.tc_ready; ps_i++) {
       tc::PassGeo& pg = h_geo[(size_t)p * n_pass + ps_i];
       const uint32_t f0 = ps_i * hpp, f1 = std::min(n_f, f0 + hpp);
       pg.f0 = (int)f0;
       pg.n_f = f1 > f0 ? (int)(f1 - f0) : 0;
       int16_t* dsh = h_dsh + ((size_t)p * n_pass + ps_i) * tc::M_MAX * npad;
+      int start = 0;
       for (uint32_t m = 0; m < M; m++) {
-        int lo = INT32_MAX, hi = INT32_MIN;
+        int lo = INT32_MAX, hi = INT32_MIN, step = INT32_MAX;
         for (uint32_t f = f0; f < f1; f++) {
-          lo = std::min(lo, so[(size_t)m * n_f_stride + f]);
-          hi = std::max(hi, so[(size_t)m * n_f_stride + f]);
+          const int s = so[(size_t)m * n_f_stride + f];
+          lo = std::min(lo, s);
+          hi = std::max(hi, s);
+          if (m > 0) step = std::min(step, s - so[(size_t)(m - 1) * n_f_stride + f]);
         }
-        if (f1 <= f0) { lo = hi = so[(size_t)m * n_f_stride + n_f - 1]; }
-        pg.smin[m] = lo;
-        if (hi - lo > tc::HALO) { ps.tc_ready = false; ps.tc_why = "frequency grid too sparse for the tensor-core tiling (fold-offset spread > 32)"; break; }
+        if (f1 <= f0) start = hi = so[(size_t)m * n_f_stride + n_f - 1];     // an empty pass: no column to order
+        else start = m == 0 ? lo : start + step;
+        pg.smin[m] = start;
+        if (hi - start > tc::HALO) {
+          ps.tc_ready = false;
+          ps.tc_why = "frequency grid too sparse for the tensor-core tiling (fold offsets more than 32 samples above the staging start)";
+          break;
+        }
         for (uint32_t f = f0; f < f1; f++)
-          for (int t = 0; t < 3; t++) dsh[(size_t)m * npad + (f - f0) * 3 + t] = (int16_t)(so[(size_t)m * n_f_stride + f] - lo);
+          for (int t = 0; t < 3; t++) dsh[(size_t)m * npad + (f - f0) * 3 + t] = (int16_t)(so[(size_t)m * n_f_stride + f] - start);
       }
     }
   }

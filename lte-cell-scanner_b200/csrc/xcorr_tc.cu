@@ -51,7 +51,7 @@ struct TcParams {
   const uint8_t* b_img;       // [plan][pass][b_bytes] digit planes in core-matrix order
   const float* corr;          // [plan][pass][2][npad] (C_re row, C_im row), MAGIC_VAL already subtracted
   const tc::PassGeo* geo;     // [plan][pass]
-  const int16_t* dsh;         // [plan][pass][M_MAX][npad] fold offset of the column minus the pass minimum
+  const int16_t* dsh;         // [plan][pass][M_MAX][npad] fold offset of the column minus the pass' staging start smin
   float* single_planar;       // [batch][3][n_f_stride][9600]
   uint32_t n_cap, n_f_stride, n_comb, batch, n_pass;
   uint32_t tu, t_cta;         // tiles per unit / tiles per CTA
@@ -399,7 +399,7 @@ __global__ void __launch_bounds__(128 + 128 * J, 1) xcorr_fold_tc_kernel(const _
 #pragma unroll
             for (int v = 0; v < NV; v++) rr[v] = __fmaf_rn(x[v], x[v], rr[v]);
             // fold into the sliding window: lag q*64 + row of the tile lands at window index lag + HALO - dsh; all loads
-            // of the read-modify-write first, then add + store.  d = -4 * (fold offset of the column - pass minimum),
+            // of the read-modify-write first, then add + store.  d = -4 * (fold offset of the column - staging start),
             // bytes, for the C/4 columns of this thread, read per sub-tile to keep it out of the registers the MMAs overlap.
             int d[CG][2];
 #pragma unroll

@@ -199,11 +199,16 @@ def test_tc_integer_formulation_numpy(oracle):
     S = 2.0 ** e
     assert maxabs * S <= limit
     lags = np.random.default_rng(1).integers(0, n_cap - 136, 150)
+    # the bit-exact model of the kernel (xcorr_tc_model) builds the same integer templates with the library's pss_td
+    from xcorr_tc_model import TcModel
+    model = TcModel(n_cap, f, fc, fc, fs)
+    assert model.S == S
     worst = 0.0
     for fi in range(f.size):
         for t in range(3):
             wr, wi = np.rint(w[fi, t].real * S).astype(np.int64), np.rint(w[fi, t].imag * S).astype(np.int64)
             a = np.empty(274, np.int64); a[0::2] = wr; a[1::2] = -wi
+            assert np.array_equal(model.a[fi, t], a)
             d2 = ((a + 128) % 256) - 128; r1 = (a - d2) // 256
             d1 = ((r1 + 128) % 256) - 128; d0 = (r1 - d1) // 256
             assert np.array_equal((d0 * 256 + d1) * 256 + d2, a)
@@ -223,43 +228,20 @@ def test_tc_integer_formulation_numpy(oracle):
 def test_tc_run_decomposition_covers_every_position_once():
     """The tensor-core correlator distributes work in tile space (xcorr_tc.cu: launch_xcorr_fold_tc / TcRunIter): CTA i takes
     tiles [i*t_cta, (i+1)*t_cta) of the sequence [unit][tu]; a run of T tiles yields 256*T - 32 fold positions.  Restated
-    here: for many (units, SMs) every position 0..9599 of every unit is produced by exactly one run, and no run needs more
-    tiles than it was given."""
-    NT, HALO, NF = 256, 32, 9600
+    in xcorr_tc_model (which the bit-exact model's fold order uses too): for many (units, SMs) every position 0..9599 of
+    every unit is produced by exactly one run, and no run needs more tiles than it was given."""
+    from xcorr_tc_model import HALO, N_FOLD, NT, tc_plan, tc_runs
 
-    def plan(n_units, n_sm):
-        tu = (NF + HALO + NT - 1) // NT
-        while True:
-            t_cta = (n_units * tu + n_sm - 1) // n_sm
-            runs = (tu + t_cta - 1) // t_cta + 1
-            if NT * tu - HALO * runs >= NF:
-                return tu, t_cta
-            tu += 1
-
-    for n_units, n_sm in [(1, 132), (2, 132), (3, 7), (8, 132), (32, 132), (64, 132), (128, 132), (384, 132), (768, 132), (5, 1), (37, 13)]:
-        tu, t_cta = plan(n_units, n_sm)
-        total = n_units * tu
-        cover = np.zeros((n_units, NF), np.int32)
-        grid = (total + t_cta - 1) // t_cta
+    for n_units, n_sm in [(1, 132), (2, 132), (3, 7), (8, 132), (32, 132), (64, 132), (128, 132), (384, 132), (768, 132), (5, 1), (37, 13),
+                          (3, 114), (128, 114), (6, 78)]:
+        tu, t_cta = tc_plan(n_units, n_sm)
+        cover = np.zeros((n_units, N_FOLD), np.int32)
+        grid = (n_units * tu + t_cta - 1) // t_cta
         assert grid <= max(n_sm, 1) or t_cta == 1
-        for cta in range(grid):
-            t, t_end = cta * t_cta, min((cta + 1) * t_cta, total)
-            while t < t_end:
-                u = t // tu
-                base = u * tu
-                a = t - base
-                e = min(t_end, base + tu)
-                bb = e - base
-                nb = (base + a) // t_cta - base // t_cta
-                t = e
-                p0 = NT * a - HALO * nb
-                if p0 >= NF:
-                    continue
-                p1 = min(NT * bb - HALO * (nb + 1), NF)
-                assert p1 > p0
-                n_tiles = min(bb - a, (p1 - p0 + HALO + NT - 1) // NT)
-                assert NT * n_tiles - HALO >= p1 - p0          # the run's tiles suffice for its positions
-                cover[u, p0:p1] += 1
+        for cta, u, p0, p1, n_tiles, given in tc_runs(n_units, n_sm):
+            assert cta < grid and p1 > p0
+            assert n_tiles <= given and NT * n_tiles - HALO >= p1 - p0          # the run's tiles suffice for its positions
+            cover[u, p0:p1] += 1
         assert (cover == 1).all(), (n_units, n_sm, tu, t_cta)
 
 
