@@ -72,7 +72,7 @@ typedef struct lcs_xcorr_plan lcs_xcorr_plan;
 /* ---- library / context ------------------------------------------------------------------ */
 const char* lcs_version(void);
 /* Create a context on CUDA device `device` (one per process per GPU).  Fails with LCS_ERR_CUDA
- * when the device is absent or is not compute capability 10.x. */
+ * when the device is absent or is not compute capability 9.0 (the kernels are built for sm_90a only). */
 lcs_status lcs_ctx_create(int device, lcs_ctx** ctx);
 void lcs_ctx_destroy(lcs_ctx* ctx);
 const char* lcs_last_error(const lcs_ctx* ctx);   /* ctx may be NULL: last global error */

@@ -1,12 +1,14 @@
 """ctypes binding of liblcs_b200.so - the C ABI declared in include/lcs_b200.h.
 
 This module is plumbing for tests/, bench.py and __graft_entry__.py: every call goes through the
-same `extern "C"` entry points a C++/IT++ host would bind (INTEGRATION.md).  There is no CPU
-fallback: importing works anywhere (the symbols are checked), but every compute call needs an
-H100 and raises LcsError otherwise.
+same `extern "C"` entry points a C++/IT++ host would bind (INTEGRATION.md).  lib() gives every
+function of the header its ctypes prototype, read from the header itself, so a call with a missing
+or mistyped argument raises before it reaches the library.  There is no CPU fallback: importing
+works anywhere, but every compute call needs an H100 and raises LcsError otherwise.
 """
 import ctypes as C
 import os
+import re
 import subprocess
 
 import numpy as np
@@ -42,12 +44,46 @@ class Cell(C.Structure):
 
 
 def build(force=False):
-    """Compile the CUDA library in-tree (nvcc cross-compiles sm_90a without a GPU)."""
-    if force or not os.path.exists(LIB_PATH):
-        subprocess.check_call(["make", "-C", HERE, "-s", "-j8"])
-    else:
-        subprocess.check_call(["make", "-C", HERE, "-s", "-j8"])  # make is incremental
+    """Compile the CUDA library in-tree (nvcc cross-compiles sm_90a without a GPU).  make is incremental, so it rebuilds
+    what changed whether or not `force` is set."""
+    subprocess.check_call(["make", "-C", HERE, "-s", "-j8"])
     return LIB_PATH
+
+
+# Scalar types of the header.  Every pointer (handles, arrays, structs, out-parameters) is a c_void_p: the callers pass
+# array addresses, ctypes arrays, C.byref(...) and oracle Cells alike.
+_SCALARS = {"double": C.c_double, "int": C.c_int, "lcs_status": C.c_int, "uint8_t": C.c_uint8, "uint16_t": C.c_uint16,
+            "uint32_t": C.c_uint32, "uint64_t": C.c_uint64}
+
+
+def _ctype(fn, decl, ret=False):
+    words = re.sub(r"\bconst\b", " ", decl).replace("*", " * ").split()
+    if "*" in words:
+        return C.c_char_p if ret and words == ["char", "*"] else C.c_void_p
+    if ret and words == ["void"]:
+        return None
+    if not words or words[0] not in _SCALARS:
+        raise LcsError("%s: no ctypes type for %r in %s" % (fn, decl.strip(), HEADER))
+    return _SCALARS[words[0]]
+
+
+def prototypes():
+    """{name: (restype, argtypes)} for every function declared in include/lcs_b200.h."""
+    txt = re.sub(r"/\*.*?\*/", " ", open(HEADER).read(), flags=re.S)
+    txt = re.sub(r"^\s*#.*$", "", txt, flags=re.M)
+    table = {}
+    for decl in re.split(r"[;{}]", txt):
+        m = re.fullmatch(r"\s*(.+?)\b(lcs_\w+)\s*\((.*)\)\s*", decl, re.S)
+        if m:
+            ret, name, args = m.groups()
+            args = [] if args.strip() == "void" else args.split(",")
+            table[name] = (_ctype(name, ret, ret=True), [_ctype(name, a) for a in args])
+    return table
+
+
+def declared_symbols():
+    """Function names declared in include/lcs_b200.h."""
+    return sorted(prototypes())
 
 
 _lib = None
@@ -59,64 +95,25 @@ def lib():
         if not os.path.exists(LIB_PATH):
             raise LcsError("liblcs_b200.so is not built (run `make -C lte-cell-scanner_b200`); "
                            "there is no CPU fallback")
-        _lib = C.CDLL(LIB_PATH)
-        _lib.lcs_version.restype = C.c_char_p
-        _lib.lcs_last_error.restype = C.c_char_p
-        _lib.lcs_last_error.argtypes = [C.c_void_p]
-        _lib.lcs_launch_count.restype = C.c_uint64
-        _lib.lcs_launch_count.argtypes = [C.c_void_p]
-        _lib.lcs_xcorr_plan_n_comb_xc.restype = C.c_uint16
-        _lib.lcs_xcorr_plan_n_comb_sp.restype = C.c_uint16
-        _lib.lcs_xcorr_plan_n_comb_xc.argtypes = [C.c_void_p]
-        _lib.lcs_xcorr_plan_n_comb_sp.argtypes = [C.c_void_p]
-        _lib.lcs_xcorr_plan_kernel.argtypes = [C.c_void_p, C.c_int]
-        _lib.lcs_ctx_destroy.argtypes = [C.c_void_p]
-        _lib.lcs_xcorr_plan_destroy.argtypes = [C.c_void_p]
-        _lib.lcs_xcorr_plan_timing_enable.argtypes = [C.c_void_p, C.c_int]
-        _lib.lcs_xcorr_plan_timing_read.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
-        _lib.lcs_framer_destroy.argtypes = [C.c_void_p]
-        _lib.lcs_sweep_destroy.argtypes = [C.c_void_p]
-        _lib.lcs_sweep_destroy.restype = None
-        _lib.lcs_framer_destroy.restype = None
-        _lib.lcs_framer_request.argtypes = [C.c_void_p]
-        _lib.lcs_framer_request.restype = None
-        _lib.lcs_framer_sample_time.argtypes = [C.c_void_p]
-        _lib.lcs_framer_sample_time.restype = C.c_double
-        _lib.lcs_track_destroy.argtypes = [C.c_void_p]
-        _lib.lcs_track_destroy.restype = None
-        _lib.lcs_track_add_cell.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_double]
-        _lib.lcs_track_push_cu8.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
-        _lib.lcs_track_frequency_offset.argtypes = [C.c_void_p, C.c_void_p]
-        _lib.lcs_track_read.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p]
-        _lib.lcs_track_sample_time.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p]
-        _lib.lcs_track_timing_read.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
-        _lib.lcs_chan_design_taps.argtypes = [C.c_double, C.c_void_p, C.c_void_p]
-        _lib.lcs_chan_create.argtypes = [C.c_void_p, C.c_double, C.c_double, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]
-        _lib.lcs_chan_destroy.argtypes = [C.c_void_p]
-        _lib.lcs_chan_destroy.restype = None
-        _lib.lcs_chan_auto_gain_ci16.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
-        _lib.lcs_chan_gain.argtypes = [C.c_void_p, C.c_void_p]
-        _lib.lcs_chan_n_out.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p]
-        _lib.lcs_chan_push_ci16.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_int, C.c_void_p,
-                                            C.c_void_p]
-        _lib.lcs_chan_timing_read.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
-        _lib.lcs_chan_design_rational.argtypes = [C.c_double, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-        _lib.lcs_chan_create_rational.argtypes = [C.c_void_p, C.c_double, C.c_int, C.c_double, C.c_uint32, C.c_void_p,
-                                                  C.c_void_p, C.c_void_p]
-        _lib.lcs_chan_push.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_int, C.c_void_p,
-                                       C.c_void_p]
-        _lib.lcs_chan_auto_gain.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
+        l = C.CDLL(LIB_PATH)
+        table = prototypes()
+        missing = sorted(name for name in table if not hasattr(l, name))
+        if missing:
+            raise LcsError("%s lacks functions declared in include/lcs_b200.h: %s" % (LIB_PATH, ", ".join(missing)))
+        for name, (restype, argtypes) in table.items():
+            f = getattr(l, name)
+            f.restype, f.argtypes = restype, argtypes
+        _lib = l
     return _lib
 
 
 def _p(a):
-    return None if a is None else C.c_void_p(a.ctypes.data)
+    return None if a is None else a.ctypes.data
 
 
 def _chk(rc, ctx=None):
     if rc != 0:
-        msg = lib().lcs_last_error(ctx).decode() if ctx else lib().lcs_last_error(None).decode()
-        raise LcsError("lcs_b200 error %d: %s" % (rc, msg))
+        raise LcsError("lcs_b200 error %d: %s" % (rc, lib().lcs_last_error(ctx).decode()))
 
 
 def new_cell(**kw):
@@ -133,18 +130,50 @@ def _copy(c):
     return o
 
 
-def f_search_set(freq_start, ppm):
+def _cell_rows(cells, n, max_cells, values=None):
+    """Row b of the [len(n)][max_cells] array `cells` holds n[b] Cells, truncated at max_cells: one list of copies per
+    row, or of (Cell, values[i]) pairs when the parallel array `values` is given."""
+    rows = []
+    for b, nb in enumerate(n):
+        idx = range(b * max_cells, b * max_cells + min(nb, max_cells))
+        rows.append([_copy(cells[i]) if values is None else (_copy(cells[i]), values[i]) for i in idx])
+    return rows
+
+
+def _query_then_fill(fn, *args, dtype=np.float64):
+    """fn(*args, out, &n) sets n when out is NULL, then fills an n-element out: the filled array."""
     n = C.c_uint32(0)
-    _chk(lib().lcs_f_search_set(C.c_double(freq_start), C.c_double(ppm), None, C.byref(n)))
-    out = np.zeros(n.value)
-    _chk(lib().lcs_f_search_set(C.c_double(freq_start), C.c_double(ppm), _p(out), C.byref(n)))
+    _chk(fn(*args, None, C.byref(n)))
+    out = np.zeros(n.value, dtype)
+    _chk(fn(*args, _p(out), C.byref(n)))
     return out
+
+
+class _Handle:
+    """A library object: `_h` is its handle, freed by the function named `_destroy` on close() or garbage collection."""
+    _h = None
+    _destroy = None
+
+    def close(self):
+        if self._h:
+            getattr(lib(), self._destroy)(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def f_search_set(freq_start, ppm):
+    return _query_then_fill(lib().lcs_f_search_set, freq_start, ppm)
 
 
 def calc_z_th1(sp_incoherent, n_comb_xc, ds_comb_arm):
     s = np.ascontiguousarray(sp_incoherent, np.float64)
     z = np.zeros_like(s)
-    _chk(lib().lcs_calc_z_th1(_p(s), C.c_uint32(s.size), C.c_uint16(n_comb_xc), C.c_uint8(ds_comb_arm), _p(z)))
+    _chk(lib().lcs_calc_z_th1(_p(s), s.size, n_comb_xc, ds_comb_arm, _p(z)))
     return z
 
 
@@ -154,16 +183,15 @@ def peak_search(pw, frq, z_th1, f_set, fc_requested, fc_programmed, single_plana
     z = np.ascontiguousarray(z_th1, np.float64); f = np.ascontiguousarray(f_set, np.float64)
     sp = np.ascontiguousarray(single_planar, np.float32)
     cells = (Cell * max_cells)(); n = C.c_uint32(0)
-    _chk(lib().lcs_peak_search(_p(pw), _p(frq), _p(z), _p(f), C.c_uint32(f.size), C.c_double(fc_requested),
-                               C.c_double(fc_programmed), _p(sp), C.c_uint8(ds_comb_arm), cells,
-                               C.c_uint32(max_cells), C.byref(n)))
+    _chk(lib().lcs_peak_search(_p(pw), _p(frq), _p(z), _p(f), f.size, fc_requested, fc_programmed, _p(sp), ds_comb_arm,
+                               cells, max_cells, C.byref(n)))
     return [_copy(cells[i]) for i in range(min(n.value, max_cells))]
 
 
 def dedup(cells):
     n = len(cells)
     arr = (Cell * max(n, 1))(*cells); out = (Cell * max(n, 1))(); m = C.c_uint32(0)
-    _chk(lib().lcs_dedup(arr, C.c_uint32(n), out, C.byref(m)))
+    _chk(lib().lcs_dedup(arr, n, out, C.byref(m)))
     return [_copy(out[i]) for i in range(m.value)]
 
 
@@ -173,8 +201,7 @@ def tfoec(cell, tfg, ts, fc_requested, fc_programmed):
     g = np.asfortranarray(tfg, np.complex128)                        # column-major cmat for the ABI
     ts = np.ascontiguousarray(ts, np.float64)
     gc = np.zeros((n, 72), np.complex128, order="F"); tsc = np.zeros(n); out = Cell()
-    _chk(lib().lcs_tfoec(None, C.byref(cell), C.c_void_p(g.ctypes.data), _p(ts), C.c_uint32(n),
-                         C.c_double(fc_requested), C.c_double(fc_programmed), C.c_void_p(gc.ctypes.data), _p(tsc),
+    _chk(lib().lcs_tfoec(None, C.byref(cell), _p(g), _p(ts), n, fc_requested, fc_programmed, _p(gc), _p(tsc),
                          C.byref(out)))
     return out, np.ascontiguousarray(gc), tsc
 
@@ -183,27 +210,17 @@ def decode_mib(cell, tfg):
     """searcher.h:115-119 - host stage (no GPU needed)."""
     g = np.asfortranarray(tfg, np.complex128)
     out = Cell()
-    _chk(lib().lcs_decode_mib(None, C.byref(cell), C.c_void_p(g.ctypes.data), C.c_uint32(g.shape[0]), C.byref(out)))
+    _chk(lib().lcs_decode_mib(None, C.byref(cell), _p(g), g.shape[0], C.byref(out)))
     return out
 
 
-class Context:
+class Context(_Handle):
     """lcs_ctx: one per process per GPU."""
+    _destroy = "lcs_ctx_destroy"
 
     def __init__(self, device=0):
         self._h = C.c_void_p()
         _chk(lib().lcs_ctx_create(int(device), C.byref(self._h)))
-
-    def close(self):
-        if self._h:
-            lib().lcs_ctx_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
     @property
     def launches(self):
@@ -222,10 +239,9 @@ class Context:
         xc = np.zeros((3, n_cap - 136, n_f), np.complex64) if want_xc else None
         sp = np.zeros(((n_cap - 273) // 9600) * 9600) if want_sp else None
         ncx, ncs = C.c_uint16(0), C.c_uint16(0)
-        _chk(lib().lcs_xcorr_pss(self._h, _p(capbuf), C.c_uint32(n_cap), _p(f), C.c_uint32(n_f), C.c_uint8(ds_comb_arm),
-                                 C.c_double(fc_requested), C.c_double(fc_programmed), C.c_double(fs_programmed),
-                                 _p(pw), _p(frq), _p(single), _p(inc), _p(spi), _p(xc), _p(sp), C.byref(ncx), C.byref(ncs)),
-             self._h)
+        _chk(lib().lcs_xcorr_pss(self._h, _p(capbuf), n_cap, _p(f), n_f, ds_comb_arm, fc_requested, fc_programmed,
+                                 fs_programmed, _p(pw), _p(frq), _p(single), _p(inc), _p(spi), _p(xc), _p(sp),
+                                 C.byref(ncx), C.byref(ncs)), self._h)
         return dict(pow=pw.T.copy(), frq=frq.T.copy(), single=single, incoherent=inc, sp_incoherent=spi, xc=xc, sp=sp,
                     n_comb_xc=ncx.value, n_comb_sp=ncs.value)
 
@@ -235,10 +251,9 @@ class Context:
         h1_np = np.zeros(62); h2_np = np.zeros(62)
         arrs = [np.zeros(62, np.complex128) for _ in range(4)]
         lln = np.zeros((2, 168)); lle = np.zeros((2, 168))
-        _chk(lib().lcs_sss_detect(self._h, C.byref(cell), _p(capbuf), C.c_uint32(capbuf.size), C.c_double(thresh2_n_sigma),
-                                  C.c_double(fc_requested), C.c_double(fc_programmed), C.c_double(fs_programmed),
-                                  C.byref(out), _p(h1_np), _p(h2_np), _p(arrs[0]), _p(arrs[1]), _p(arrs[2]), _p(arrs[3]),
-                                  _p(lln), _p(lle)), self._h)
+        _chk(lib().lcs_sss_detect(self._h, C.byref(cell), _p(capbuf), capbuf.size, thresh2_n_sigma, fc_requested,
+                                  fc_programmed, fs_programmed, C.byref(out), _p(h1_np), _p(h2_np), _p(arrs[0]),
+                                  _p(arrs[1]), _p(arrs[2]), _p(arrs[3]), _p(lln), _p(lle)), self._h)
         d = dict(h1_np=h1_np, h2_np=h2_np, h1_nrm=arrs[0], h2_nrm=arrs[1], h1_ext=arrs[2], h2_ext=arrs[3],
                  log_lik_nrm=lln.T.copy(), log_lik_ext=lle.T.copy())
         return out, d
@@ -246,16 +261,15 @@ class Context:
     def pss_sss_foe(self, cell, capbuf, fc_requested, fc_programmed, fs_programmed):
         capbuf = np.ascontiguousarray(capbuf, np.complex128)
         out = Cell()
-        _chk(lib().lcs_pss_sss_foe(self._h, C.byref(cell), _p(capbuf), C.c_uint32(capbuf.size), C.c_double(fc_requested),
-                                   C.c_double(fc_programmed), C.c_double(fs_programmed), C.byref(out)), self._h)
+        _chk(lib().lcs_pss_sss_foe(self._h, C.byref(cell), _p(capbuf), capbuf.size, fc_requested, fc_programmed,
+                                   fs_programmed, C.byref(out)), self._h)
         return out
 
     def extract_tfg(self, cell, capbuf, fc_requested, fc_programmed, fs_programmed):
         capbuf = np.ascontiguousarray(capbuf, np.complex128)
         tfg = np.zeros(72 * 854, np.complex128); ts = np.zeros(854); n = C.c_uint32(0)
-        _chk(lib().lcs_extract_tfg(self._h, C.byref(cell), _p(capbuf), C.c_uint32(capbuf.size), C.c_double(fc_requested),
-                                   C.c_double(fc_programmed), C.c_double(fs_programmed), _p(tfg), _p(ts), C.byref(n)),
-             self._h)
+        _chk(lib().lcs_extract_tfg(self._h, C.byref(cell), _p(capbuf), capbuf.size, fc_requested, fc_programmed,
+                                   fs_programmed, _p(tfg), _p(ts), C.byref(n)), self._h)
         n = n.value
         return tfg[:72 * n].reshape(72, n).T.copy(), ts[:n].copy()      # cmat(n_ofdm,72) column-major
 
@@ -276,9 +290,8 @@ class Context:
         else:
             cb = np.ascontiguousarray(capbuf, np.complex128)
             fn, n_cap = lib().lcs_cell_search, cb.size
-        _chk(fn(self._h, _p(cb), C.c_uint32(n_cap), _p(f), C.c_uint32(f.size), C.c_double(fc_requested),
-                C.c_double(fc_programmed), C.c_double(fs_programmed), cells, C.c_uint32(max_cells), C.byref(n), peaks,
-                C.byref(npk)), self._h)
+        _chk(fn(self._h, _p(cb), n_cap, _p(f), f.size, fc_requested, fc_programmed, fs_programmed, cells, max_cells,
+                C.byref(n), peaks, C.byref(npk)), self._h)
         return ([_copy(cells[i]) for i in range(min(n.value, max_cells))],
                 [_copy(peaks[i]) for i in range(min(npk.value, max_cells))])
 
@@ -288,19 +301,17 @@ class Context:
         cb = np.ascontiguousarray(capbuf_cu8, np.uint8)
         tr = np.ascontiguousarray(list(tracked), np.int32)
         cells = (Cell * max_cells)(); ft = (C.c_double * max_cells)(); n = C.c_uint32(0)
-        _chk(lib().lcs_tracker_search_cu8(self._h, _p(cb), C.c_uint32(cb.size // 2), C.c_double(frequency_offset),
-                                          C.c_double(fc_requested), C.c_double(fc_programmed), C.c_double(fs_programmed),
-                                          C.c_double(late), _p(tr) if tr.size else None, C.c_uint32(tr.size), cells, ft,
-                                          C.c_uint32(max_cells), C.byref(n)), self._h)
+        _chk(lib().lcs_tracker_search_cu8(self._h, _p(cb), cb.size // 2, frequency_offset, fc_requested, fc_programmed,
+                                          fs_programmed, late, _p(tr) if tr.size else None, tr.size, cells, ft,
+                                          max_cells, C.byref(n)), self._h)
         return [(_copy(cells[i]), ft[i]) for i in range(min(n.value, max_cells))]
 
     def kalibrate_cu8(self, capbuf_cu8, fc_requested, fc_programmed, fs_programmed, ppm, correction=1.0):
         """LTE-Tracker.cpp:565-741.  Returns (best Cell or None, correction_residual, number of cells found)."""
         cb = np.ascontiguousarray(capbuf_cu8, np.uint8)
         best = Cell(); res = C.c_double(0); n = C.c_uint32(0)
-        _chk(lib().lcs_kalibrate_cu8(self._h, _p(cb), C.c_uint32(cb.size // 2), C.c_double(fc_requested), C.c_double(fc_programmed),
-                                     C.c_double(fs_programmed), C.c_double(ppm), C.c_double(correction), C.byref(best), C.byref(res),
-                                     C.byref(n)), self._h)
+        _chk(lib().lcs_kalibrate_cu8(self._h, _p(cb), cb.size // 2, fc_requested, fc_programmed, fs_programmed, ppm,
+                                     correction, C.byref(best), C.byref(res), C.byref(n)), self._h)
         return (best if n.value else None), res.value, n.value
 
     def plan(self, n_cap, f_set, ds_comb_arm, fc_requested, fc_programmed, fs_programmed, max_batch=1,
@@ -308,8 +319,9 @@ class Context:
         return XcorrPlan(self, n_cap, f_set, ds_comb_arm, fc_requested, fc_programmed, fs_programmed, max_batch, kernel)
 
 
-class XcorrPlan:
+class XcorrPlan(_Handle):
     """lcs_xcorr_plan: templates + fold offsets + scratch for a fixed search configuration."""
+    _destroy = "lcs_xcorr_plan_destroy"
 
     def __init__(self, ctx, n_cap, f_set, ds_comb_arm, fc_requested, fc_programmed, fs_programmed, max_batch, kernel):
         self.ctx = ctx
@@ -318,23 +330,10 @@ class XcorrPlan:
         self.n_f = self.f_set.size
         self.max_batch = int(max_batch)
         self._h = C.c_void_p()
-        _chk(lib().lcs_xcorr_plan_create(ctx._h, C.c_uint32(n_cap), _p(self.f_set), C.c_uint32(self.n_f),
-                                         C.c_uint8(ds_comb_arm), C.c_double(fc_requested), C.c_double(fc_programmed),
-                                         C.c_double(fs_programmed), C.c_uint32(max_batch), int(kernel), C.byref(self._h)),
-             ctx._h)
+        _chk(lib().lcs_xcorr_plan_create(ctx._h, n_cap, _p(self.f_set), self.n_f, ds_comb_arm, fc_requested,
+                                         fc_programmed, fs_programmed, max_batch, int(kernel), C.byref(self._h)), ctx._h)
         self.n_comb_xc = lib().lcs_xcorr_plan_n_comb_xc(self._h)
         self.n_comb_sp = lib().lcs_xcorr_plan_n_comb_sp(self._h)
-
-    def close(self):
-        if self._h:
-            lib().lcs_xcorr_plan_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
     def timing_enable(self, on=True):
         _chk(lib().lcs_xcorr_plan_timing_enable(self._h, int(bool(on))), self.ctx._h)
@@ -350,16 +349,13 @@ class XcorrPlan:
     def run_device(self, d_iq_ptr, iq_format, batch, d_single_ptr, d_pow_ptr, d_frq_ptr, d_spi_ptr,
                    d_inc_ptr=None, stream=None):
         """Raw device pointers (ints, e.g. torch.Tensor.data_ptr()); asynchronous on `stream`."""
-        _chk(lib().lcs_xcorr_pss_device(self._h, C.c_void_p(d_iq_ptr), int(iq_format), C.c_uint32(batch),
-                                        C.c_void_p(d_single_ptr), C.c_void_p(d_pow_ptr), C.c_void_p(d_frq_ptr),
-                                        C.c_void_p(d_spi_ptr), C.c_void_p(d_inc_ptr) if d_inc_ptr else None,
-                                        C.c_void_p(stream) if stream else None), self.ctx._h)
+        _chk(lib().lcs_xcorr_pss_device(self._h, d_iq_ptr, int(iq_format), batch, d_single_ptr, d_pow_ptr, d_frq_ptr,
+                                        d_spi_ptr, d_inc_ptr, stream), self.ctx._h)
 
     def run_host(self, h_iq_ptr, iq_format, batch, h_single_ptr, h_pow_ptr, h_frq_ptr, h_spi_ptr):
         """Host pointers (pinned for overlap): the e2e path."""
-        _chk(lib().lcs_xcorr_pss_batch_host(self._h, C.c_void_p(h_iq_ptr), int(iq_format), C.c_uint32(batch),
-                                            C.c_void_p(h_single_ptr) if h_single_ptr else None, C.c_void_p(h_pow_ptr),
-                                            C.c_void_p(h_frq_ptr), C.c_void_p(h_spi_ptr)), self.ctx._h)
+        _chk(lib().lcs_xcorr_pss_batch_host(self._h, h_iq_ptr, int(iq_format), batch, h_single_ptr, h_pow_ptr, h_frq_ptr,
+                                            h_spi_ptr), self.ctx._h)
 
     def run_host_np(self, iq, iq_format, want_single=True):
         """numpy convenience over run_host: iq [batch][n_cap] in the given format."""
@@ -367,8 +363,7 @@ class XcorrPlan:
         batch = iq.shape[0]
         single = np.zeros((batch, 3, self.n_f, N_FOLD), np.float32) if want_single else None
         pw = np.zeros((batch, 3, N_FOLD)); frq = np.zeros((batch, 3, N_FOLD), np.int32); spi = np.zeros((batch, N_FOLD))
-        self.run_host(iq.ctypes.data, iq_format, batch, single.ctypes.data if want_single else None, pw.ctypes.data,
-                      frq.ctypes.data, spi.ctypes.data)
+        self.run_host(_p(iq), iq_format, batch, _p(single), _p(pw), _p(frq), _p(spi))
         return dict(single=single, pow=pw, frq=frq, sp_incoherent=spi)
 
     def peaks_batch(self, iq, iq_format, max_peaks=32, host_ptr=None, batch=None):
@@ -379,9 +374,8 @@ class XcorrPlan:
             host_ptr, batch = iq.ctypes.data, iq.shape[0]
         peaks = (Cell * (batch * max_peaks))()
         n = (C.c_uint32 * batch)()
-        _chk(lib().lcs_xcorr_peaks_batch_host(self._h, C.c_void_p(host_ptr), int(iq_format), C.c_uint32(batch), peaks,
-                                              C.c_uint32(max_peaks), n), self.ctx._h)
-        return [[_copy(peaks[b * max_peaks + k]) for k in range(min(n[b], max_peaks))] for b in range(batch)]
+        _chk(lib().lcs_xcorr_peaks_batch_host(self._h, host_ptr, int(iq_format), batch, peaks, max_peaks, n), self.ctx._h)
+        return _cell_rows(peaks, n, max_peaks)
 
     def cell_search_batch_cu8(self, iq_cu8, max_cells=16, host_ptr=None, batch=None):
         """The whole CellSearch chain for every buffer of a batch of raw rtl-sdr byte buffers (uint8 [batch][n_cap][2])."""
@@ -390,30 +384,19 @@ class XcorrPlan:
             host_ptr, batch = iq_cu8.ctypes.data, iq_cu8.shape[0]
         cells = (Cell * (batch * max_cells))()
         n = (C.c_uint32 * batch)()
-        _chk(lib().lcs_cell_search_batch_cu8(self._h, C.c_void_p(host_ptr), C.c_uint32(batch), cells, C.c_uint32(max_cells), n),
-             self.ctx._h)
-        return [[_copy(cells[b * max_cells + k]) for k in range(min(n[b], max_cells))] for b in range(batch)]
+        _chk(lib().lcs_cell_search_batch_cu8(self._h, host_ptr, batch, cells, max_cells, n), self.ctx._h)
+        return _cell_rows(cells, n, max_cells)
 
 
-class Sweep:
+class Sweep(_Handle):
     """lcs_sweep: many channels (centre frequencies / tracked channels) through one correlator launch per chunk."""
+    _destroy = "lcs_sweep_destroy"
 
     def __init__(self, ctx, n_cap=153600):
         self.ctx = ctx
         self.n_cap = int(n_cap)
         self._h = C.c_void_p()
-        _chk(lib().lcs_sweep_create(ctx._h, C.c_uint32(n_cap), C.byref(self._h)), ctx._h)
-
-    def close(self):
-        if self._h:
-            lib().lcs_sweep_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+        _chk(lib().lcs_sweep_create(ctx._h, n_cap, C.byref(self._h)), ctx._h)
 
     def search_cu8(self, iq_cu8, fc_requested, f_set, fs_programmed=1.92e6, fc_programmed=None, max_cells=8, host_ptr=None):
         """CellSearch.cpp:465-558 for all channels.  iq_cu8: uint8 [n_ch][n_cap][2] (or host_ptr).  Returns a list
@@ -427,9 +410,9 @@ class Sweep:
             host_ptr = iq_cu8.ctypes.data
         cells = (Cell * (n_ch * max_cells))()
         n = (C.c_uint32 * n_ch)()
-        _chk(lib().lcs_sweep_search_cu8(self._h, C.c_void_p(host_ptr), C.c_uint32(n_ch), _p(fc), _p(fcp), C.c_double(fs_programmed),
-                                        _p(f), C.c_uint32(f.size), cells, C.c_uint32(max_cells), n), self.ctx._h)
-        return [[_copy(cells[b * max_cells + k]) for k in range(min(n[b], max_cells))] for b in range(n_ch)]
+        _chk(lib().lcs_sweep_search_cu8(self._h, host_ptr, n_ch, _p(fc), _p(fcp), fs_programmed, _p(f), f.size, cells,
+                                        max_cells, n), self.ctx._h)
+        return _cell_rows(cells, n, max_cells)
 
     def search_cu8_device(self, iq, fc_requested, f_set, fs_programmed=1.92e6, fc_programmed=None, max_cells=8, n_ch=None):
         """search_cu8 on capture buffers in device memory, read in place: iq is a uint8 CUDA tensor [n_ch][n_cap][2]
@@ -449,10 +432,9 @@ class Sweep:
             ptr = iq.data_ptr()
         cells = (Cell * (n_ch * max_cells))()
         n = (C.c_uint32 * n_ch)()
-        _chk(lib().lcs_sweep_search_cu8_device(self._h, C.c_void_p(ptr), C.c_uint32(n_ch), _p(fc), _p(fcp),
-                                               C.c_double(fs_programmed), _p(f), C.c_uint32(f.size), cells,
-                                               C.c_uint32(max_cells), n), self.ctx._h)
-        return [[_copy(cells[b * max_cells + k]) for k in range(min(n[b], max_cells))] for b in range(n_ch)]
+        _chk(lib().lcs_sweep_search_cu8_device(self._h, ptr, n_ch, _p(fc), _p(fcp), fs_programmed, _p(f), f.size, cells,
+                                               max_cells, n), self.ctx._h)
+        return _cell_rows(cells, n, max_cells)
 
     def track_cu8(self, iq_cu8, frequency_offset, fc_requested, fs_programmed=1.92e6, fc_programmed=None, late=None, tracked=None,
                   max_cells=8, host_ptr=None):
@@ -478,19 +460,19 @@ class Sweep:
         cells = (Cell * (n_ch * max_cells))()
         ft = (C.c_double * (n_ch * max_cells))()
         n = (C.c_uint32 * n_ch)()
-        _chk(lib().lcs_sweep_track_cu8(self._h, C.c_void_p(host_ptr), C.c_uint32(n_ch), _p(fo), _p(fc), _p(fcp), C.c_double(fs_programmed),
-                                       _p(lt), _p(tr), _p(nt), C.c_uint32(stride), cells, ft, C.c_uint32(max_cells), n), self.ctx._h)
-        return [[(_copy(cells[b * max_cells + k]), ft[b * max_cells + k]) for k in range(min(n[b], max_cells))] for b in range(n_ch)]
+        _chk(lib().lcs_sweep_track_cu8(self._h, host_ptr, n_ch, _p(fo), _p(fc), _p(fcp), fs_programmed, _p(lt), _p(tr),
+                                       _p(nt), stride, cells, ft, max_cells, n), self.ctx._h)
+        return _cell_rows(cells, n, max_cells, ft)
 
 
-class Framer:
+class Framer(_Handle):
     """lcs_framer: producer-side framing of a raw IQ byte stream into searcher capture buffers (host only)."""
+    _destroy = "lcs_framer_destroy"
 
     def __init__(self, fc_requested, fc_programmed, fs_programmed, n_cap=153600):
         self._h = C.c_void_p()
         self.n_cap = n_cap
-        _chk(lib().lcs_framer_create(C.c_double(fc_requested), C.c_double(fc_programmed), C.c_double(fs_programmed),
-                                     C.c_uint32(n_cap), C.byref(self._h)))
+        _chk(lib().lcs_framer_create(fc_requested, fc_programmed, fs_programmed, n_cap, C.byref(self._h)))
 
     def request(self):
         lib().lcs_framer_request(self._h)
@@ -502,19 +484,11 @@ class Framer:
         """iq_u8: uint8 [n][2].  Returns None, or (capbuf uint8 [n_cap][2] copy, late) once a requested buffer is full."""
         iq = np.ascontiguousarray(iq_u8, np.uint8)
         ready = C.c_int(0); cap = C.POINTER(C.c_uint8)(); late = C.c_double(0)
-        _chk(lib().lcs_framer_push(self._h, _p(iq), C.c_uint32(iq.size // 2), C.c_double(frequency_offset), C.byref(ready),
-                                   C.byref(cap), C.byref(late)))
+        _chk(lib().lcs_framer_push(self._h, _p(iq), iq.size // 2, frequency_offset, C.byref(ready), C.byref(cap),
+                                   C.byref(late)))
         if not ready.value:
             return None
         return np.ctypeslib.as_array(cap, shape=(self.n_cap, 2)).copy(), late.value
-
-    def close(self):
-        if self._h:
-            lib().lcs_framer_destroy(self._h)
-            self._h = None
-
-    def __del__(self):
-        self.close()
 
 
 class TrackCell(C.Structure):
@@ -551,8 +525,9 @@ class TrackCell(C.Structure):
 TRACK_BLOCK = 10000
 
 
-class Tracker:
+class Tracker(_Handle):
     """lcs_track: the per-cell tracker loop of LTE-Tracker for every cell of n_ch channels, one launch per push."""
+    _destroy = "lcs_track_destroy"
 
     def __init__(self, ctx, fc_requested, frequency_offset, fs_programmed=1.92e6, fc_programmed=None, max_cells=8):
         self.ctx = ctx
@@ -562,11 +537,11 @@ class Tracker:
         fo = np.ascontiguousarray(np.broadcast_to(np.asarray(frequency_offset, np.float64), (self.n_ch,)))
         self.max_cells = int(max_cells)
         self._h = C.c_void_p()
-        _chk(lib().lcs_track_create(ctx._h, C.c_uint32(self.n_ch), _p(fc), _p(fcp), C.c_double(fs_programmed), _p(fo),
-                                    C.c_uint32(self.max_cells), C.byref(self._h)), ctx._h)
+        _chk(lib().lcs_track_create(ctx._h, self.n_ch, _p(fc), _p(fcp), fs_programmed, _p(fo), self.max_cells,
+                                    C.byref(self._h)), ctx._h)
 
     def add_cell(self, ch, cell, frame_timing):
-        _chk(lib().lcs_track_add_cell(self._h, C.c_uint32(ch), C.byref(cell), C.c_double(frame_timing)), self.ctx._h)
+        _chk(lib().lcs_track_add_cell(self._h, ch, C.byref(cell), frame_timing), self.ctx._h)
 
     def push_cu8(self, iq_cu8):
         """iq_cu8: uint8 [n_ch][n][2] (or [n][2] for one channel)."""
@@ -574,7 +549,7 @@ class Tracker:
         n = iq.shape[-2]
         if iq.size != self.n_ch * n * 2:
             raise ValueError("push_cu8: expected [n_ch][n][2] samples")
-        _chk(lib().lcs_track_push_cu8(self._h, _p(iq), C.c_uint32(n)), self.ctx._h)
+        _chk(lib().lcs_track_push_cu8(self._h, _p(iq), n), self.ctx._h)
 
     def frequency_offset(self):
         fo = np.zeros(self.n_ch)
@@ -583,7 +558,7 @@ class Tracker:
 
     def sample_time(self, ch=0):
         v = C.c_double(0)
-        _chk(lib().lcs_track_sample_time(self._h, C.c_uint32(ch), C.byref(v)), self.ctx._h)
+        _chk(lib().lcs_track_sample_time(self._h, ch, C.byref(v)), self.ctx._h)
         return v.value
 
     def timing_read(self):
@@ -596,37 +571,20 @@ class Tracker:
         """The channel's cells in the order added, as dicts; a dropped cell is reported once."""
         out = (TrackCell * self.max_cells)()
         n = C.c_uint32(0)
-        _chk(lib().lcs_track_read(self._h, C.c_uint32(ch), out, C.c_uint32(self.max_cells), C.byref(n)), self.ctx._h)
+        _chk(lib().lcs_track_read(self._h, ch, out, self.max_cells, C.byref(n)), self.ctx._h)
         return [out[i].as_dict() for i in range(n.value)]
-
-    def close(self):
-        if self._h:
-            lib().lcs_track_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
 
 def chan_design_taps(fs_in):
     """The channelizer's prototype low-pass for input rate fs_in (host only, no device needed): float32 [L]."""
-    n = C.c_uint32(0)
-    _chk(lib().lcs_chan_design_taps(C.c_double(fs_in), None, C.byref(n)))
-    h = np.zeros(n.value, np.float32)
-    _chk(lib().lcs_chan_design_taps(C.c_double(fs_in), _p(h), C.byref(n)))
-    return h
+    return _query_then_fill(lib().lcs_chan_design_taps, fs_in, dtype=np.float32)
 
 
 def chan_design_rational(fs_in):
     """fs_in / 1.92 MHz = down / up in lowest terms and the prototype low-pass at up * fs_in, DC gain up (host only):
     (up, down, float32 [L])."""
-    up, down, n = C.c_uint32(0), C.c_uint32(0), C.c_uint32(0)
-    _chk(lib().lcs_chan_design_rational(C.c_double(fs_in), C.byref(up), C.byref(down), None, C.byref(n)))
-    h = np.zeros(n.value, np.float32)
-    _chk(lib().lcs_chan_design_rational(C.c_double(fs_in), C.byref(up), C.byref(down), _p(h), C.byref(n)))
+    up, down = C.c_uint32(0), C.c_uint32(0)
+    h = _query_then_fill(lib().lcs_chan_design_rational, fs_in, C.byref(up), C.byref(down), dtype=np.float32)
     return up.value, down.value, h
 
 
@@ -635,9 +593,10 @@ CHAN_FORMATS = {"ci16": (IQ_CI16, np.int16), "cs8": (IQ_CS8, np.int8), "cu8": (I
                 "cf32": (IQ_CF32, np.float32)}
 
 
-class RationalChannelizer:
+class RationalChannelizer(_Handle):
     """lcs_chan at any allowed SDR rate: a wideband ci16 / cs8 / cu8 / cf32 recording -> one 1.92 Msps cu8 stream per LTE
     raster channel, resampled by up / down (DESIGN.md sections 4.6 and 4.7)."""
+    _destroy = "lcs_chan_destroy"
 
     def __init__(self, ctx, fs_in, fc_in, fc_ch, fmt="ci16", gain=None):
         if fmt not in CHAN_FORMATS:
@@ -655,8 +614,8 @@ class RationalChannelizer:
         self.M = (self.taps.size - 1) // 2
 
     def _create(self, fs_in, fc_in, fc, g):
-        return lib().lcs_chan_create_rational(self.ctx._h, C.c_double(fs_in), self._iq_format, C.c_double(fc_in),
-                                              C.c_uint32(self.n_ch), _p(fc), _p(g), C.byref(self._h))
+        return lib().lcs_chan_create_rational(self.ctx._h, fs_in, self._iq_format, fc_in, self.n_ch, _p(fc), _p(g),
+                                              C.byref(self._h))
 
     def _samples(self, iq):
         """iq as a contiguous [n][2] array of the format's dtype (complex64 [n] is accepted for cf32)."""
@@ -670,7 +629,7 @@ class RationalChannelizer:
     def auto_gain(self, iq):
         """Set every channel's gain to 0.25 / RMS of its output over these samples (the stream is not touched)."""
         iq = self._samples(iq)
-        _chk(lib().lcs_chan_auto_gain(self._h, _p(iq), C.c_uint32(iq.shape[0])), self.ctx._h)
+        _chk(lib().lcs_chan_auto_gain(self._h, _p(iq), iq.shape[0]), self.ctx._h)
         return self.gain
 
     @property
@@ -681,7 +640,7 @@ class RationalChannelizer:
 
     def n_out(self, n_in):
         k = C.c_uint32(0)
-        _chk(lib().lcs_chan_n_out(self._h, C.c_uint64(n_in), C.byref(k)), self.ctx._h)
+        _chk(lib().lcs_chan_n_out(self._h, n_in, C.byref(k)), self.ctx._h)
         return k.value
 
     def push(self, iq):
@@ -691,8 +650,7 @@ class RationalChannelizer:
         out = np.zeros((self.n_ch, k, 2), np.uint8)
         clip = np.zeros(self.n_ch, np.uint64)
         got = C.c_uint32(0)
-        _chk(lib().lcs_chan_push(self._h, _p(iq), C.c_uint32(iq.shape[0]), _p(out), C.c_uint32(k), 0, C.byref(got),
-                                 _p(clip)), self.ctx._h)
+        _chk(lib().lcs_chan_push(self._h, _p(iq), iq.shape[0], _p(out), k, 0, C.byref(got), _p(clip)), self.ctx._h)
         return out, clip
 
     def push_device(self, iq, out):
@@ -704,8 +662,8 @@ class RationalChannelizer:
             raise ValueError("push_device: expected a contiguous uint8 CUDA tensor [n_ch][capacity][2]")
         clip = np.zeros(self.n_ch, np.uint64)
         got = C.c_uint32(0)
-        _chk(lib().lcs_chan_push(self._h, _p(iq), C.c_uint32(iq.shape[0]), C.c_void_p(out.data_ptr()),
-                                 C.c_uint32(out.shape[1]), 1, C.byref(got), _p(clip)), self.ctx._h)
+        _chk(lib().lcs_chan_push(self._h, _p(iq), iq.shape[0], out.data_ptr(), out.shape[1], 1, C.byref(got), _p(clip)),
+             self.ctx._h)
         return got.value, clip
 
     def timing_read(self):
@@ -713,17 +671,6 @@ class RationalChannelizer:
         ms = C.c_double(0); n = C.c_uint64(0)
         _chk(lib().lcs_chan_timing_read(self._h, C.byref(ms), C.byref(n)), self.ctx._h)
         return ms.value, n.value
-
-    def close(self):
-        if self._h:
-            lib().lcs_chan_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
 
 class Channelizer(RationalChannelizer):
@@ -734,8 +681,7 @@ class Channelizer(RationalChannelizer):
         self.D = self.down
 
     def _create(self, fs_in, fc_in, fc, g):
-        return lib().lcs_chan_create(self.ctx._h, C.c_double(fs_in), C.c_double(fc_in), C.c_uint32(self.n_ch), _p(fc),
-                                     _p(g), C.byref(self._h))
+        return lib().lcs_chan_create(self.ctx._h, fs_in, fc_in, self.n_ch, _p(fc), _p(g), C.byref(self._h))
 
     def _samples(self, iq):
         """iq as contiguous int16 [n][2], cast from other integer types."""
@@ -746,10 +692,3 @@ class Channelizer(RationalChannelizer):
 
     push_ci16 = RationalChannelizer.push
     push_ci16_device = RationalChannelizer.push_device
-
-
-def declared_symbols():
-    """Function names declared in include/lcs_b200.h (for the export test)."""
-    import re
-    txt = open(HEADER).read()
-    return sorted(set(re.findall(r"\b(lcs_[a-z0-9_]+)\s*\(", txt)))

@@ -24,8 +24,7 @@ def build():
 def lib():
     global _lib
     if _lib is None:
-        if not os.path.exists(LIB_PATH):
-            build()
+        build()                                   # make is incremental: an edited track_oracle.cpp is rebuilt
         _lib = C.CDLL(LIB_PATH)
         _lib.to_create.restype = C.c_void_p
         _lib.to_create.argtypes = [C.c_uint32, C.c_void_p, C.c_void_p, C.c_double, C.c_void_p, C.c_uint32]
