@@ -47,6 +47,12 @@ static void print_usage() {
   cout << "                                 up <= 128, down <= 640 (e.g. 2.048, 2.4, 2.5, 6, 10, 20, 25, 56, 100 Msps)" << endl;
   cout << "     --format F                  with --resample: the recording's sample format, ci16 (default), cs8 (HackRF)," << endl;
   cout << "                                 cu8 (rtl_sdr) or cf32 (GNU Radio, SigMF cf32_le)" << endl;
+  cout << "     --spectrum OUT.csv          with --wideband: Welch power spectrum of the WHOLE recording (periodic Hann," << endl;
+  cout << "                                 50 % overlap) written as freq_hz,psd_dbfs_per_hz lines; with a search the cell" << endl;
+  cout << "                                 table gains each cell's carrier power in dBFS over n_rb_dl * 180 kHz.  -s may" << endl;
+  cout << "                                 then be omitted (no search), and --fs-in may be any integer number of Hz up to" << endl;
+  cout << "                                 250 MHz and --format any of the four without --resample" << endl;
+  cout << "     --nfft N                    with --spectrum: FFT length, a power of two in [64, 65536] (default 4096)" << endl;
   cout << "  -r --record / -i --device-index need a live rtl-sdr dongle: not supported by this build" << endl;
 }
 
@@ -61,12 +67,72 @@ static string freq_formatter(const double& freq) {   // CellSearch.cpp:322-341
   return temp.str();
 }
 
+// ---- --spectrum ----------------------------------------------------------------------------------------------------------
+// The checks of --spectrum that need no device: sample format, rate, --fc-in and a readable recording.
+static bool spectrum_args(const string& wideband, const string& format, double fs_in, double fc_in, int* fmt) {
+  if (format == "ci16") *fmt = LCS_IQ_CI16;
+  else if (format == "cs8") *fmt = LCS_IQ_CS8;
+  else if (format == "cu8") *fmt = LCS_IQ_CU8;
+  else if (format == "cf32") *fmt = LCS_IQ_CF32;
+  else { cerr << "Error: --format must be ci16, cs8, cu8 or cf32" << endl; return false; }
+  if (!(fs_in > 0 && fs_in <= 250e6) || std::fabs(fs_in - std::round(fs_in)) > 1e-6) {
+    cerr << "Error: --spectrum needs --fs-in, an integer number of Hz in (0, 250] MHz" << endl;
+    return false;
+  }
+  if (fc_in <= 0) { cerr << "Error: --wideband needs --fc-in" << endl; return false; }
+  FILE* f = std::fopen(wideband.c_str(), "rb");
+  if (!f) { cerr << "Error: cannot read " << wideband << endl; return false; }
+  std::fclose(f);
+  return true;
+}
+
+static FILE* open_output(const string& path) {
+  FILE* f = std::fopen(path.c_str(), "w");
+  if (!f) cerr << "Error: cannot write " << path << endl;
+  return f;
+}
+
+// Welch PSD of the whole recording (wideband_psd), written to `out` as freq_hz,psd_dbfs_per_hz lines; psd is kept for the
+// carrier-power column.
+static void write_spectrum(const string& wideband, int fmt, double fs_in, double fc_in, uint32_t nfft, const string& path,
+                           FILE* out, vector<double>& psd) {
+  uint64_t n_seg = 0;
+  try {
+    wideband_psd(wideband, fmt, fs_in, nfft, psd, n_seg);
+  } catch (const char*) {
+    std::fclose(out);
+    throw;
+  }
+  std::fprintf(out, "freq_hz,psd_dbfs_per_hz\n");
+  for (uint32_t i = 0; i < nfft; i++)
+    std::fprintf(out, "%.17g,%.17g\n", fc_in + ((double)i - nfft / 2) * (fs_in / nfft), 10 * std::log10(psd[i]));
+  const bool ok = std::fclose(out) == 0;
+  if (!ok) throw("cannot write the spectrum file");
+  if (verbosity >= 1)
+    cout << "Power spectrum of " << wideband << " (" << n_seg << " segments of " << nfft << " samples) written to " << path << endl;
+}
+
+// 10 log10 of the power in the bins whose centre lies within n_rb_dl * 90 kHz of the cell's carrier fc_requested +
+// freq_superfine, in full-scale^2 (dBFS).
+static double carrier_power_dbfs(const vector<double>& psd, double fs_in, double fc_in, const Cell& c) {
+  const size_t N = psd.size();
+  const double fc = c.fc_requested + c.freq_superfine, half = 90e3 * (int)c.n_rb_dl, df = fs_in / N;
+  double p = 0;
+  for (size_t i = 0; i < N; i++) {
+    const double f = fc_in + ((double)i - (double)(N / 2)) * df;
+    if (f >= fc - half && f <= fc + half) p += psd[i] * df;
+  }
+  return 10 * std::log10(p);
+}
+
 int main(int argc, char* const argv[]) {
   double freq_start = -1, freq_end = -1, ppm = 120, correction = 1;
   bool save_cap = false, use_recorded_data = false, raw = false, batched = false;
   string data_dir = ".", wideband, format = "ci16";
   double fs_in = -1, fc_in = -1;
   bool resample = false;
+  string spectrum;
+  long nfft = 4096;
   static struct option long_options[] = {
       {"help", no_argument, 0, 'h'},          {"verbose", no_argument, 0, 'v'},       {"brief", no_argument, 0, 'b'},
       {"freq-start", required_argument, 0, 's'}, {"freq-end", required_argument, 0, 'e'}, {"ppm", required_argument, 0, 'p'},
@@ -74,6 +140,7 @@ int main(int argc, char* const argv[]) {
       {"data-dir", required_argument, 0, 'd'},   {"device-index", required_argument, 0, 'i'}, {"raw", no_argument, 0, 'R'}, {"sweep", no_argument, 0, 'W'},
       {"wideband", required_argument, 0, 'B'},   {"fs-in", required_argument, 0, 'F'},   {"fc-in", required_argument, 0, 'C'},
       {"resample", no_argument, 0, 'S'},         {"format", required_argument, 0, 'T'},
+      {"spectrum", required_argument, 0, 'P'},   {"nfft", required_argument, 0, 'N'},
       {0, 0, 0, 0}};
   for (;;) {
     int idx = 0;
@@ -98,11 +165,30 @@ int main(int argc, char* const argv[]) {
       case 'C': fc_in = strtod(optarg, &endp); if (optarg == endp || *endp) { cerr << "Error: could not parse --fc-in" << endl; return -1; } break;
       case 'S': resample = true; break;
       case 'T': format = optarg; break;
+      case 'P': spectrum = optarg; break;
+      case 'N': nfft = strtol(optarg, &endp, 10); if (optarg == endp || *endp) { cerr << "Error: could not parse --nfft" << endl; return -1; } break;
       case 'i': break;
       default: return -1;
     }
   }
   if (optind < argc) { cerr << "Error: unknown/extra arguments specified on command line" << endl; return -1; }
+  const bool spec = !spectrum.empty(), search = !spec || freq_start != -1;   // --spectrum alone: no search
+  if (spec && wideband.empty()) { cerr << "Error: --spectrum needs --wideband" << endl; return -1; }
+  if (nfft < 64 || nfft > 65536 || (nfft & (nfft - 1))) { cerr << "Error: --nfft must be a power of two in [64, 65536]" << endl; return -1; }
+  int spec_format = LCS_IQ_CI16;
+  FILE* spec_file = nullptr;
+  vector<double> psd;
+  if (spec && !spectrum_args(wideband, format, fs_in, fc_in, &spec_format)) return -1;
+  if (!search) {
+    if (!(spec_file = open_output(spectrum))) return -1;
+    try {
+      write_spectrum(wideband, spec_format, fs_in, fc_in, (uint32_t)nfft, spectrum, spec_file, psd);
+    } catch (const char* msg) {
+      cerr << "Error: " << msg << endl;
+      return -1;
+    }
+    return 0;
+  }
   if (freq_start == -1) { cerr << "Error: must specify a start frequency. (Try --help)" << endl; return -1; }
   if (freq_start < 1e6) { cerr << "Error: start frequency must be greater than 1MHz" << endl; return -1; }
   if (freq_start / 100e3 != std::round(freq_start / 100e3)) {
@@ -172,6 +258,7 @@ int main(int argc, char* const argv[]) {
       return -1;
     }
   }
+  if (spec && !(spec_file = open_output(spectrum))) return -1;
   if (verbosity >= 1) {
     cout << "LTE CellSearch (GPU drop-in, " << lcs_version() << ") beginning" << endl;
     if (freq_start == freq_end) cout << "  Search frequency: " << freq_start / 1e6 << " MHz" << endl;
@@ -195,6 +282,7 @@ int main(int argc, char* const argv[]) {
     const int n_fc = (int)floor((freq_end - freq_start) / 100e3) + 1;                   // :465
     vector<list<Cell> > detected_cells(n_fc);
     xcorr_pss_skip_debug_outputs(true);
+    if (spec) write_spectrum(wideband, spec_format, fs_in, fc_in, (uint32_t)nfft, spectrum, spec_file, psd);
     if (wide) {
       // every raster point channelized out of the one recording on the device, then the batched search in place
       vector<double> fcs;
@@ -297,7 +385,7 @@ int main(int argc, char* const argv[]) {
     } else {   // CellSearch.cpp:579-613
       cout << "Detected the following cells:" << endl;
       cout << "A: #antenna ports C: CP type ; P: PHICH duration ; PR: PHICH resource type" << endl;
-      cout << "CID A      fc   foff RXPWR C nRB P  PR CrystalCorrectionFactor" << endl;
+      cout << "CID A      fc   foff RXPWR C nRB P  PR CrystalCorrectionFactor" << (spec ? " CarrierPower[dBFS]" : "") << endl;
       for (list<Cell>::iterator it = cells_final.begin(); it != cells_final.end(); ++it) {
         stringstream ss;
         ss << setw(3) << (*it).n_id_cell();
@@ -318,6 +406,7 @@ int main(int argc, char* const argv[]) {
         const double crystal_freq_actual = (*it).fc_requested - (*it).freq_superfine;
         const double correction_new = correction * ((*it).fc_requested / crystal_freq_actual);
         ss << " " << setprecision(20) << correction_new;
+        if (spec) ss << " " << fixed << setprecision(2) << carrier_power_dbfs(psd, fs_in, fc_in, *it);
         cout << ss.str() << endl;
       }
     }

@@ -2,6 +2,7 @@
 // (include/searcher.h:22-124), bodies marshal the IT++ containers to the C ABI of
 // include/lcs_b200.h and back.  No numerical work happens here.
 #include "searcher_dropin.hpp"
+#include "../../include/lcs_psd.h"
 
 #include <cmath>
 #include <cstdlib>
@@ -135,6 +136,29 @@ void wideband_search_rational(const void* iq, int iq_format, uint32_t n, double 
                               const std::vector<double>& fc_requested, const vec& f_search_set,
                               const double& fs_programmed, std::vector<std::list<Cell> >& detected_cells) {
   wideband_search(iq, iq_format, n, fs_in, fc_in, fc_requested, f_search_set, fs_programmed, detected_cells);
+}
+
+void wideband_psd(const std::string& path, int iq_format, double fs_in, uint32_t nfft, std::vector<double>& psd,
+                  uint64_t& n_segments) {
+  const size_t es = iq_format == LCS_IQ_CI16 ? 4 : iq_format == LCS_IQ_CF32 ? 8 : 2;
+  const size_t block = (size_t)1 << 22;                              // samples per push
+  FILE* f = std::fopen(path.c_str(), "rb");
+  if (!f) throw("wideband_psd: cannot read the recording");
+  lcs_psd* p = nullptr;
+  lcs_status rc = lcs_psd_create(lcs_dropin_ctx(), fs_in, iq_format, nfft, &p);
+  const char* where = "lcs_psd_create";
+  std::vector<unsigned char> buf(block * es);
+  while (rc == LCS_OK) {
+    const size_t got = std::fread(buf.data(), es, block, f);
+    if (!got) break;
+    rc = lcs_psd_push(p, buf.data(), (uint32_t)got);
+    where = "lcs_psd_push";
+  }
+  std::fclose(f);
+  psd.assign(nfft, 0.0);
+  if (rc == LCS_OK) { rc = lcs_psd_read(p, psd.data(), &n_segments); where = "lcs_psd_read"; }
+  if (p) lcs_psd_destroy(p);
+  check(rc, where);
 }
 
 // ---- searcher.h:22-41 ----

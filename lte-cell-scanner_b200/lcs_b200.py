@@ -1,4 +1,5 @@
-"""ctypes binding of liblcs_b200.so - the C ABI declared in include/lcs_b200.h.
+"""ctypes binding of liblcs_b200.so - the C ABI declared in include/lcs_b200.h - and of liblcs_psd.so, the Welch
+spectrum of include/lcs_psd.h built on top of it.
 
 This module is plumbing for tests/, bench.py and __graft_entry__.py: every call goes through the
 same `extern "C"` entry points a C++/IT++ host would bind (INTEGRATION.md).  lib() gives every
@@ -16,6 +17,8 @@ import numpy as np
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("LCS_B200_LIB") or os.path.join(HERE, "liblcs_b200.so")
 HEADER = os.path.join(HERE, "..", "include", "lcs_b200.h")
+PSD_LIB_PATH = os.environ.get("LCS_PSD_LIB") or os.path.join(HERE, "liblcs_psd.so")
+PSD_HEADER = os.path.join(HERE, "..", "include", "lcs_psd.h")
 
 IQ_CF32, IQ_CU8, IQ_C128, IQ_CI16, IQ_CS8 = 0, 1, 2, 3, 4
 KERNEL_AUTO, KERNEL_FP32, KERNEL_TC = 0, 1, 2
@@ -67,9 +70,10 @@ def _ctype(fn, decl, ret=False):
     return _SCALARS[words[0]]
 
 
-def prototypes():
-    """{name: (restype, argtypes)} for every function declared in include/lcs_b200.h."""
-    txt = re.sub(r"/\*.*?\*/", " ", open(HEADER).read(), flags=re.S)
+def prototypes(header=HEADER):
+    """{name: (restype, argtypes)} for every function declared in `header` (default include/lcs_b200.h; included
+    headers are not followed)."""
+    txt = re.sub(r"/\*.*?\*/", " ", open(header).read(), flags=re.S)
     txt = re.sub(r"^\s*#.*$", "", txt, flags=re.M)
     table = {}
     for decl in re.split(r"[;{}]", txt):
@@ -86,25 +90,35 @@ def declared_symbols():
     return sorted(prototypes())
 
 
-_lib = None
+_libs = {}
 
 
-def lib():
-    global _lib
-    if _lib is None:
-        if not os.path.exists(LIB_PATH):
-            raise LcsError("liblcs_b200.so is not built (run `make -C lte-cell-scanner_b200`); "
-                           "there is no CPU fallback")
-        l = C.CDLL(LIB_PATH)
-        table = prototypes()
+def _bind(path, header):
+    """The library at `path` with every function of `header` given its prototype; raises naming any it lacks."""
+    if path not in _libs:
+        if not os.path.exists(path):
+            raise LcsError("%s is not built (run `make -C lte-cell-scanner_b200`); there is no CPU fallback"
+                           % os.path.basename(path))
+        l = C.CDLL(path)
+        table = prototypes(header)
         missing = sorted(name for name in table if not hasattr(l, name))
         if missing:
-            raise LcsError("%s lacks functions declared in include/lcs_b200.h: %s" % (LIB_PATH, ", ".join(missing)))
+            raise LcsError("%s lacks functions declared in %s: %s" % (path, os.path.basename(header), ", ".join(missing)))
         for name, (restype, argtypes) in table.items():
             f = getattr(l, name)
             f.restype, f.argtypes = restype, argtypes
-        _lib = l
-    return _lib
+        _libs[path] = l
+    return _libs[path]
+
+
+def lib():
+    return _bind(LIB_PATH, HEADER)
+
+
+def psd_lib():
+    """liblcs_psd.so (include/lcs_psd.h); it takes the contexts of lib()."""
+    lib()
+    return _bind(PSD_LIB_PATH, PSD_HEADER)
 
 
 def _p(a):
@@ -154,9 +168,11 @@ class _Handle:
     _h = None
     _destroy = None
 
+    _lib = staticmethod(lib)          # the library that owns `_destroy`
+
     def close(self):
         if self._h:
-            getattr(lib(), self._destroy)(self._h)
+            getattr(self._lib(), self._destroy)(self._h)
             self._h = C.c_void_p()
 
     def __del__(self):
@@ -692,3 +708,48 @@ class Channelizer(RationalChannelizer):
 
     push_ci16 = RationalChannelizer.push
     push_ci16_device = RationalChannelizer.push_device
+
+
+class Spectrum(_Handle):
+    """lcs_psd: Welch's power spectral density of a wideband ci16 / cs8 / cu8 / cf32 recording pushed in pieces of any
+    size, periodic Hann window of nfft points, hop nfft/2 (DESIGN.md section 4.8)."""
+    _destroy = "lcs_psd_destroy"
+    _lib = staticmethod(psd_lib)
+
+    def __init__(self, ctx, fs_in, fmt="ci16", nfft=4096, fc_in=0.0):
+        if fmt not in CHAN_FORMATS:
+            raise ValueError("fmt must be one of %s" % ", ".join(CHAN_FORMATS))
+        self.ctx = ctx
+        self.fmt = fmt
+        self.fs_in = float(fs_in)
+        self.fc_in = float(fc_in)
+        self.nfft = int(nfft)
+        self._iq_format, self._dtype = CHAN_FORMATS[fmt]
+        self._h = C.c_void_p()
+        _chk(psd_lib().lcs_psd_create(ctx._h, fs_in, self._iq_format, nfft, C.byref(self._h)), ctx._h)
+
+    _samples = RationalChannelizer._samples
+
+    def push(self, iq):
+        """Push [n][2] samples in the handle's format (complex64 [n] is accepted for cf32)."""
+        iq = self._samples(iq)
+        _chk(psd_lib().lcs_psd_push(self._h, _p(iq), iq.shape[0]), self.ctx._h)
+
+    @property
+    def freqs(self):
+        """Centre frequency of every output bin, fc_in + (i - nfft/2) * fs_in / nfft."""
+        return self.fc_in + (np.arange(self.nfft) - self.nfft // 2) * (self.fs_in / self.nfft)
+
+    def read(self):
+        """(freqs, psd, n_segments): the PSD in full-scale^2 per Hz, fftshift order, over the segments completed since the
+        last read; the accumulator then restarts."""
+        psd = np.zeros(self.nfft)
+        n = C.c_uint64(0)
+        _chk(psd_lib().lcs_psd_read(self._h, _p(psd), C.byref(n)), self.ctx._h)
+        return self.freqs, psd, n.value
+
+    def timing_read(self):
+        """(kernel ms, kernel launches) since the last read, from CUDA events around the kernels of each launch chunk."""
+        ms = C.c_double(0); n = C.c_uint64(0)
+        _chk(psd_lib().lcs_psd_timing_read(self._h, C.byref(ms), C.byref(n)), self.ctx._h)
+        return ms.value, n.value
