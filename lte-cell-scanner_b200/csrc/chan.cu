@@ -516,9 +516,9 @@ using namespace lcs::chn;
 
 struct lcs_chan {
   lcs_ctx* ctx = nullptr;
-  // fs / 1.92 MHz = down / up in lowest terms (decimation by D: up = 1, down = D); samples of esz bytes in format fmt;
+  // fs / 1.92 MHz = down / up in lowest terms (decimation by D: up = 1, down = D); samples in format fmt;
   // L = 2M + 1 prototype taps, J = 2M / up + 1 of them per output; a tile is 32 * RM * up outputs
-  int fmt = LCS_IQ_CI16, esz = 4, up = 1, down = 0, L = 0, M = 0, J = 0, RM = 1;
+  int fmt = LCS_IQ_CI16, up = 1, down = 0, L = 0, M = 0, J = 0, RM = 1;
   long long fs = 0;
   uint32_t n_ch = 0;
   std::vector<float> h;
@@ -533,15 +533,9 @@ struct lcs_chan {
   DevBuf<unsigned long long> d_clip;
   DevBuf<double> d_pw;
   uint32_t chunk = TILE;                 // outputs per launch (bounds the device scratch)
-  std::vector<unsigned char> carry;      // stream samples [i_hi(n_out) - (J-1), n_in) (zeros before the stream starts)
+  SampleCarry carry;                     // stream samples [i_hi(n_out) - (J-1), n_in) (zeros before the stream starts)
   uint64_t n_in = 0, n_out = 0;
-  cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-  double kernel_ms = 0;
-  uint64_t kernel_launches = 0;
-  ~lcs_chan() {
-    if (ev0) cudaEventDestroy(ev0);
-    if (ev1) cudaEventDestroy(ev1);
-  }
+  KernelClock clock;                     // one kernel per launch chunk
 };
 
 namespace {
@@ -559,14 +553,12 @@ uint64_t outputs_after(const lcs_chan* c, uint64_t n) {
   const uint64_t q = n * c->up;
   return q >= (uint64_t)c->M + 1 ? (q - 1 - c->M) / c->down + 1 : 0;
 }
-// n samples of value 0 in the channelizer's format (cu8 127)
-std::vector<unsigned char> zero_samples(const lcs_chan* c, size_t n) {
-  return std::vector<unsigned char>(n * c->esz, c->fmt == LCS_IQ_CU8 ? 127 : 0);
+// the carry of a fresh stream: the inputs of output 0 before sample 0, of value 0 in the channelizer's format (cu8 127)
+SampleCarry fresh_carry(const lcs_chan* c) {
+  const size_t esz = stream_sample_bytes(c->fmt);
+  return SampleCarry{esz, std::vector<unsigned char>((size_t)-first_input(c, 0) * esz, c->fmt == LCS_IQ_CU8 ? 127 : 0)};
 }
 int outputs_per_tile(const lcs_chan* c) { return 32 * c->RM * c->up; }
-size_t sample_bytes(int fmt) {
-  return fmt == LCS_IQ_CI16 ? 4 : fmt == LCS_IQ_CS8 || fmt == LCS_IQ_CU8 ? 2 : fmt == LCS_IQ_CF32 ? 8 : 0;
-}
 
 template <int FMT>
 void launch_rchan(bool power, dim3 grid, size_t smem, cudaStream_t st, const RParams& P) {
@@ -648,17 +640,16 @@ void build_taps(lcs_chan* c, std::vector<float2>& taps, std::vector<double2>& ta
   }
 }
 
-// Outputs [0, n_out) of the virtual input a (na samples) ++ b (nb samples) in the channelizer's format, whose sample 0 is
-// the first input of output 0 (stream output n_abs0).  power: per-channel sums of |y|^2 are added to pw_sum; otherwise
-// bytes go to out (row stride out_stride, on the device or the host) and clip counts to d_clip.
-lcs_status run(lcs_chan* c, const unsigned char* a, size_t na, const unsigned char* b, size_t nb, uint64_t n_abs0,
-               uint64_t n_out, bool power, unsigned char* out, size_t out_stride, bool out_dev, std::vector<double>* pw_sum) {
+// Outputs [0, n_out) of the virtual input a ++ b (nb samples) in the channelizer's format, whose sample 0 is the first input
+// of output 0 (stream output n_abs0).  power: per-channel sums of |y|^2 are added to pw_sum; otherwise bytes go to out
+// (row stride out_stride, on the device or the host) and clip counts to d_clip.
+lcs_status run(lcs_chan* c, const SampleCarry& a, const unsigned char* b, size_t nb, uint64_t n_abs0, uint64_t n_out,
+               bool power, unsigned char* out, size_t out_stride, bool out_dev, std::vector<double>* pw_sum) {
   lcs_ctx* ctx = c->ctx;
   cudaStream_t st = ctx->streams[0];
   const int T = outputs_per_tile(c);
-  const size_t es = c->esz;
   const size_t span_max = (size_t)c->chunk * c->down / c->up + c->J + 2;
-  LCS_CUDA(ctx, c->d_in.ensure(span_max * es));
+  LCS_CUDA(ctx, c->d_in.ensure(span_max * a.esz));
   if (!power && !out_dev) LCS_CUDA(ctx, c->d_out.ensure((size_t)c->n_ch * c->chunk * 2));
   if (power) LCS_CUDA(ctx, c->d_pw.ensure((size_t)c->n_ch * ((c->chunk + T - 1) / T)));
   const size_t smem = tile_smem(c->down, c->J, c->RM);
@@ -669,12 +660,8 @@ lcs_status run(lcs_chan* c, const unsigned char* a, size_t na, const unsigned ch
     const uint64_t n0 = n_abs0 + e0;
     // samples [lo, hi) of a ++ b
     const size_t lo = (size_t)(first_input(c, n0) - base);
-    const size_t hi = std::min((size_t)(newest_input(c, n0 + ne - 1) + 1 - base), na + nb);
-    if (lo < na) LCS_CUDA(ctx, cudaMemcpyAsync(c->d_in.p, a + lo * es, (std::min(hi, na) - lo) * es, cudaMemcpyHostToDevice, st));
-    if (hi > na) {
-      const size_t s = std::max(lo, na);
-      LCS_CUDA(ctx, cudaMemcpyAsync(c->d_in.p + (s - lo) * es, b + (s - na) * es, (hi - s) * es, cudaMemcpyHostToDevice, st));
-    }
+    const size_t hi = std::min((size_t)(newest_input(c, n0 + ne - 1) + 1 - base), a.size() + nb);
+    LCS_CUDA(ctx, a.upload(b, lo, hi, c->d_in.p, st));
     auto shared = [&](auto& P) {
       P.in = c->d_in.p;
       P.n_in = (long long)(hi - lo);
@@ -694,11 +681,11 @@ lcs_status run(lcs_chan* c, const unsigned char* a, size_t na, const unsigned ch
       P.pw = c->d_pw.p;
     };
     const dim3 grid((ne + T - 1) / T, (c->n_ch + CH_CTA - 1) / CH_CTA);
-    LCS_CUDA(ctx, cudaEventRecord(c->ev0, st));
+    LCS_CUDA(ctx, c->clock.begin(st));
     launch(c, power, grid, smem, st, shared);
     ctx->launches++;
     LCS_CUDA(ctx, cudaGetLastError());
-    LCS_CUDA(ctx, cudaEventRecord(c->ev1, st));
+    LCS_CUDA(ctx, c->clock.end(st, 1));
     if (power) {
       pw.resize((size_t)c->n_ch * grid.x);
       LCS_CUDA(ctx, cudaMemcpyAsync(pw.data(), c->d_pw.p, pw.size() * 8, cudaMemcpyDeviceToHost, st));
@@ -707,10 +694,6 @@ lcs_status run(lcs_chan* c, const unsigned char* a, size_t na, const unsigned ch
                                       cudaMemcpyDeviceToHost, st));
     }
     LCS_CUDA(ctx, cudaStreamSynchronize(st));
-    float ms = 0;
-    LCS_CUDA(ctx, cudaEventElapsedTime(&ms, c->ev0, c->ev1));
-    c->kernel_ms += ms;
-    c->kernel_launches++;
     if (power)   // fixed order: tiles of a chunk, chunks in stream order
       for (uint32_t ch = 0; ch < c->n_ch; ch++)
         for (uint32_t t = 0; t < grid.x; t++) (*pw_sum)[ch] += pw[(size_t)ch * grid.x + t];
@@ -738,7 +721,6 @@ lcs_status create(lcs_ctx* ctx, const std::string& who, long long fs, int up, in
   if (!c) return fail(ctx, LCS_ERR_STATE, who + ": out of memory");
   c->ctx = ctx;
   c->fmt = fmt;
-  c->esz = (int)sample_bytes(fmt);
   c->up = up;
   c->down = down;
   c->fs = fs;
@@ -754,14 +736,14 @@ lcs_status create(lcs_ctx* ctx, const std::string& who, long long fs, int up, in
   c->delta = delta;
   c->gain.assign(n_ch, 1.0f);
   if (gain) c->gain.assign(gain, gain + n_ch);
-  c->carry = zero_samples(c, (size_t)-first_input(c, 0));
+  c->carry = fresh_carry(c);
   if (tile_smem(down, c->J, c->RM) > (size_t)RSMEM_CAP) {
     delete c;
     return fail(ctx, LCS_ERR_RANGE, who + ": the input tile exceeds shared memory");
   }
   // outputs per launch, whole tiles: device output scratch <= 32 MB, input <= 64 MB
   const uint64_t T = (uint64_t)outputs_per_tile(c);
-  const uint64_t by_out = (32ull << 20) / (2ull * n_ch), by_in = (64ull << 20) / c->esz * up / down;
+  const uint64_t by_out = (32ull << 20) / (2ull * n_ch), by_in = (64ull << 20) / c->carry.esz * up / down;
   c->chunk = (uint32_t)std::max<uint64_t>(T, std::min(by_out, by_in) / T * T);
   std::vector<float2> taps;
   std::vector<double2> taps64;
@@ -776,8 +758,6 @@ lcs_status create(lcs_ctx* ctx, const std::string& who, long long fs, int up, in
   if (e == cudaSuccess) e = cudaMemcpy(c->d_taps64.p, taps64.data(), taps64.size() * sizeof(double2), cudaMemcpyHostToDevice);
   if (e == cudaSuccess) e = cudaMemcpy(c->d_step.p, c->step.data(), n_ch * 8, cudaMemcpyHostToDevice);
   if (e == cudaSuccess) e = cudaMemcpy(c->d_gain.p, c->gain.data(), n_ch * 4, cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) e = cudaEventCreate(&c->ev0);
-  if (e == cudaSuccess) e = cudaEventCreate(&c->ev1);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(chan_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_CAP);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(chan_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_CAP);
   if (e == cudaSuccess) e = set_rchan_smem<LCS_IQ_CI16>();
@@ -845,7 +825,7 @@ lcs_status lcs_chan_create_rational(lcs_ctx* ctx, double fs_in, int iq_format, d
   if (!rational_rate(fs_in, &fs, &up, &down))
     return fail(ctx, LCS_ERR_ARG, "lcs_chan_create_rational: fs_in must be an integer number of Hz in (1.92, 122.88] MHz "
                                   "with fs_in / 1.92 MHz = down / up, up <= 128, down <= 640");
-  if (!sample_bytes(iq_format))
+  if (!stream_sample_bytes(iq_format))
     return fail(ctx, LCS_ERR_ARG, "lcs_chan_create_rational: iq_format must be LCS_IQ_CI16, CS8, CU8 or CF32");
   return create(ctx, "lcs_chan_create_rational", fs, up, down, iq_format, fc_in, n_ch, fc_ch, gain, out);
 }
@@ -862,10 +842,8 @@ lcs_status lcs_chan_auto_gain(lcs_chan* c, const void* iq_host, uint32_t n) {
   const uint64_t n_out = outputs_after(c, n);             // what a fresh channelizer would produce
   if (n_out == 0) return cfail(c, "lcs_chan_auto_gain: fewer samples than one output needs");
   LCS_CUDA(c->ctx, cudaSetDevice(c->ctx->device));
-  const std::vector<unsigned char> zeros = zero_samples(c, (size_t)-first_input(c, 0));
   std::vector<double> sum(c->n_ch, 0.0);
-  lcs_status rc = run(c, zeros.data(), zeros.size() / c->esz, static_cast<const unsigned char*>(iq_host), n, 0, n_out,
-                      true, nullptr, 0, false, &sum);
+  lcs_status rc = run(c, fresh_carry(c), static_cast<const unsigned char*>(iq_host), n, 0, n_out, true, nullptr, 0, false, &sum);
   if (rc != LCS_OK) return rc;
   for (uint32_t ch = 0; ch < c->n_ch; ch++) {
     const double ms = sum[ch] / (double)n_out;
@@ -907,19 +885,12 @@ lcs_status lcs_chan_push(lcs_chan* c, const void* iq_host, uint32_t n_in, uint8_
   LCS_CUDA(c->ctx, cudaSetDevice(c->ctx->device));
   LCS_CUDA(c->ctx, cudaMemsetAsync(c->d_clip.p, 0, c->n_ch * 8, c->ctx->streams[0]));
   const unsigned char* b = static_cast<const unsigned char*>(iq_host);
-  const size_t es = c->esz, na = c->carry.size() / es;
   if (k) {
-    lcs_status rc = run(c, c->carry.data(), na, b, n_in, c->n_out, k, false, out, (size_t)out_capacity * 2,
-                        out_on_device != 0, nullptr);
+    lcs_status rc = run(c, c->carry, b, n_in, c->n_out, k, false, out, (size_t)out_capacity * 2, out_on_device != 0, nullptr);
     if (rc != LCS_OK) return rc;
   }
   // keep the samples from the first input of the next output on
-  const size_t drop = (size_t)(first_input(c, c->n_out + k) - first_input(c, c->n_out));
-  std::vector<unsigned char> nc;
-  nc.reserve((na + n_in - drop) * es);
-  if (drop < na) nc.insert(nc.end(), c->carry.begin() + drop * es, c->carry.end());
-  nc.insert(nc.end(), b + (drop > na ? drop - na : 0) * es, b + (size_t)n_in * es);
-  c->carry.swap(nc);
+  c->carry.advance(b, n_in, (size_t)(first_input(c, c->n_out + k) - first_input(c, c->n_out)));
   c->n_in += n_in;
   c->n_out += k;
   *n_out = (uint32_t)k;
@@ -942,10 +913,7 @@ lcs_status lcs_chan_push_ci16(lcs_chan* c, const int16_t* iq_host, uint32_t n_in
 lcs_status lcs_chan_timing_read(lcs_chan* c, double* kernel_ms, uint64_t* launches) {
   if (!c) return LCS_ERR_ARG;
   if (!kernel_ms || !launches) return cfail(c, "lcs_chan_timing_read: null pointer");
-  *kernel_ms = c->kernel_ms;
-  *launches = c->kernel_launches;
-  c->kernel_ms = 0;
-  c->kernel_launches = 0;
+  LCS_CUDA(c->ctx, c->clock.read(kernel_ms, launches));
   return LCS_OK;
 }
 

@@ -55,28 +55,11 @@ static lcs_status run_device(lcs_xcorr_plan* p, const void* d_iq, int iq_format,
   if (batch == 0 || batch > p->max_batch) return fail(ctx, LCS_ERR_ARG, "xcorr_pss_device: batch exceeds plan max_batch");
   if (!p->timing)
     return planset_run(p->ps, p->kernel, d_iq, iq_format, batch, nullptr, d_single, d_pow, d_frq, d_spi, d_inc, st);
-  std::pair<cudaEvent_t, cudaEvent_t> ev{nullptr, nullptr};
-  if (p->ev_pool.empty()) {
-    LCS_CUDA(ctx, cudaEventCreate(&ev.first));
-    LCS_CUDA(ctx, cudaEventCreate(&ev.second));
-  } else {
-    ev = p->ev_pool.back();
-    p->ev_pool.pop_back();
-  }
-  lcs_status rc = planset_run(p->ps, p->kernel, d_iq, iq_format, batch, nullptr, d_single, d_pow, d_frq, d_spi, d_inc, st, &ev);
-  if (rc != LCS_OK) { p->ev_pool.push_back(ev); return rc; }     // nothing usable was recorded
-  p->ev_used.push_back(ev);
-  if (p->ev_used.size() >= 1024) {                                // bound the list: fold the oldest half into the running sum
-    for (size_t i = 0; i < 512; i++) {
-      float ms = 0;
-      LCS_CUDA(ctx, cudaEventSynchronize(p->ev_used[i].second));
-      LCS_CUDA(ctx, cudaEventElapsedTime(&ms, p->ev_used[i].first, p->ev_used[i].second));
-      p->ev_acc_ms += ms;
-      p->ev_acc_n++;
-      p->ev_pool.push_back(p->ev_used[i]);
-    }
-    p->ev_used.erase(p->ev_used.begin(), p->ev_used.begin() + 512);
-  }
+  const KernelClock::Pair* ev = nullptr;
+  LCS_CUDA(ctx, p->clock.open(&ev));
+  lcs_status rc = planset_run(p->ps, p->kernel, d_iq, iq_format, batch, nullptr, d_single, d_pow, d_frq, d_spi, d_inc, st, ev);
+  if (rc != LCS_OK) return rc;
+  LCS_CUDA(ctx, p->clock.commit(1));
   return LCS_OK;
 }
 
@@ -200,8 +183,6 @@ void lcs_xcorr_plan_destroy(lcs_xcorr_plan* plan) {
   if (!plan) return;
   cudaSetDevice(plan->ctx->device);
   cudaDeviceSynchronize();
-  for (auto& ev : plan->ev_pool) { cudaEventDestroy(ev.first); cudaEventDestroy(ev.second); }
-  for (auto& ev : plan->ev_used) { cudaEventDestroy(ev.first); cudaEventDestroy(ev.second); }
   delete plan;
 }
 
@@ -212,20 +193,7 @@ lcs_status lcs_xcorr_plan_timing_enable(lcs_xcorr_plan* p, int enable) {
 }
 lcs_status lcs_xcorr_plan_timing_read(lcs_xcorr_plan* p, double* kernel_ms, uint64_t* launches) {
   if (!p || !kernel_ms || !launches) return fail(nullptr, LCS_ERR_ARG, "timing_read: null argument");
-  double tot = p->ev_acc_ms;
-  const uint64_t n_acc = p->ev_acc_n;
-  p->ev_acc_ms = 0;
-  p->ev_acc_n = 0;
-  for (auto& ev : p->ev_used) {
-    LCS_CUDA(p->ctx, cudaEventSynchronize(ev.second));
-    float ms = 0;
-    LCS_CUDA(p->ctx, cudaEventElapsedTime(&ms, ev.first, ev.second));
-    tot += ms;
-    p->ev_pool.push_back(ev);
-  }
-  *kernel_ms = tot;
-  *launches = p->ev_used.size() + n_acc;
-  p->ev_used.clear();
+  LCS_CUDA(p->ctx, p->clock.read(kernel_ms, launches));
   return LCS_OK;
 }
 

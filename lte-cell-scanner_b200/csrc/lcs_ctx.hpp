@@ -42,6 +42,116 @@ struct PinBuf {   // owning page-locked host allocation (asynchronous copies nee
   }
 };
 
+// Kernel time of a handle: CUDA event pairs recorded around groups of launches, each committed with the number of kernels
+// it covers.  Nothing waits for a pair before read(), so launches that are not synchronised can be timed as well.
+class KernelClock {
+ public:
+  typedef std::pair<cudaEvent_t, cudaEvent_t> Pair;
+  KernelClock() = default;
+  KernelClock(const KernelClock&) = delete;
+  KernelClock& operator=(const KernelClock&) = delete;
+  ~KernelClock() {
+    for (const Pair& ev : pool_) destroy(ev);
+    for (const Used& u : used_) destroy(u.ev);
+    destroy(open_);
+  }
+  // The pair of the next group, for a caller that records it; a group that fails before its commit leaves it open.
+  cudaError_t open(const Pair** ev) {
+    if (!open_.first && !pool_.empty()) {
+      open_ = pool_.back();
+      pool_.pop_back();
+    }
+    cudaError_t e = open_.first ? cudaSuccess : cudaEventCreate(&open_.first);
+    if (e == cudaSuccess && !open_.second) e = cudaEventCreate(&open_.second);
+    *ev = &open_;
+    return e;
+  }
+  // The open pair has been recorded around `kernels` kernels.
+  cudaError_t commit(uint64_t kernels) {
+    used_.push_back(Used{open_, kernels});
+    open_ = Pair(nullptr, nullptr);
+    return used_.size() >= 1024 ? fold(512) : cudaSuccess;   // bound the list: the oldest half into the running sum
+  }
+  // open and commit for a group whose launches are enqueued between begin and end on one stream.
+  cudaError_t begin(cudaStream_t st) {
+    const Pair* ev = nullptr;
+    cudaError_t e = open(&ev);
+    return e == cudaSuccess ? cudaEventRecord(ev->first, st) : e;
+  }
+  cudaError_t end(cudaStream_t st, uint64_t kernels) {
+    cudaError_t e = cudaEventRecord(open_.second, st);
+    return e == cudaSuccess ? commit(kernels) : e;
+  }
+  // Kernel time and kernel count of the groups committed since the last read, summed in record order.
+  cudaError_t read(double* ms, uint64_t* kernels) {
+    cudaError_t e = fold(used_.size());
+    if (e != cudaSuccess) return e;
+    *ms = acc_ms_;
+    *kernels = acc_n_;
+    acc_ms_ = 0;
+    acc_n_ = 0;
+    return cudaSuccess;
+  }
+
+ private:
+  struct Used {
+    Pair ev;
+    uint64_t kernels;
+  };
+  std::vector<Pair> pool_;
+  std::vector<Used> used_;
+  Pair open_{nullptr, nullptr};
+  double acc_ms_ = 0;        // the pairs already folded out of used_
+  uint64_t acc_n_ = 0;
+  static void destroy(const Pair& ev) {
+    if (ev.first) cudaEventDestroy(ev.first);
+    if (ev.second) cudaEventDestroy(ev.second);
+  }
+  // Wait for the oldest n pairs, add them to the running sums and return them to the pool.
+  cudaError_t fold(size_t n) {
+    cudaError_t e = cudaSuccess;
+    size_t i = 0;
+    for (; i < n; i++) {
+      float ms = 0;
+      e = cudaEventSynchronize(used_[i].ev.second);
+      if (e == cudaSuccess) e = cudaEventElapsedTime(&ms, used_[i].ev.first, used_[i].ev.second);
+      if (e != cudaSuccess) break;
+      acc_ms_ += ms;
+      acc_n_ += used_[i].kernels;
+      pool_.push_back(used_[i].ev);
+    }
+    used_.erase(used_.begin(), used_.begin() + i);
+    return e;
+  }
+};
+
+// The raw samples a streaming handle keeps from one push to the next: a push reads carry ++ pushed samples as one input.
+struct SampleCarry {
+  size_t esz = 0;                    // bytes per sample
+  std::vector<unsigned char> bytes;
+  size_t size() const { return bytes.size() / esz; }
+  // Copy samples [lo, hi) of carry ++ push to dst, asynchronously on st.
+  cudaError_t upload(const unsigned char* push, size_t lo, size_t hi, unsigned char* dst, cudaStream_t st) const {
+    const size_t na = size();
+    cudaError_t e = cudaSuccess;
+    if (lo < na) e = cudaMemcpyAsync(dst, bytes.data() + lo * esz, (std::min(hi, na) - lo) * esz, cudaMemcpyHostToDevice, st);
+    if (e == cudaSuccess && hi > na) {
+      const size_t s = std::max(lo, na);
+      e = cudaMemcpyAsync(dst + (s - lo) * esz, push + (s - na) * esz, (hi - s) * esz, cudaMemcpyHostToDevice, st);
+    }
+    return e;
+  }
+  // Consume the first `drop` samples of carry ++ push (n_push samples) and carry the rest.
+  void advance(const unsigned char* push, size_t n_push, size_t drop) {
+    const size_t na = size();
+    std::vector<unsigned char> nc;
+    nc.reserve((na + n_push - drop) * esz);
+    if (drop < na) nc.insert(nc.end(), bytes.begin() + drop * esz, bytes.end());
+    if (n_push) nc.insert(nc.end(), push + (drop > na ? drop - na : 0) * esz, push + n_push * esz);
+    bytes.swap(nc);
+  }
+};
+
 // One search configuration: what xcorr_pss is called with besides the capture buffer (searcher.h:22-31).
 struct PlanCfg {
   double fc_req = 0, fc_prog = 0, fs_prog = 0;
@@ -112,11 +222,8 @@ struct lcs_xcorr_plan {
   lcs::PlanSet ps;
   uint32_t max_batch = 1;
   int kernel = LCS_KERNEL_AUTO;
-  // kernel timing hook
-  bool timing = false;
-  std::vector<std::pair<cudaEvent_t, cudaEvent_t>> ev_pool, ev_used;
-  double ev_acc_ms = 0;                        // time of event pairs already harvested from ev_used
-  uint64_t ev_acc_n = 0;
+  bool timing = false;                         // time the correlator kernel of every launch on `clock`
+  lcs::KernelClock clock;
   // per-stream device buffers of the host-input entry points (lcs_xcorr_pss uses stream 0's)
   struct HostBatchBufs {
     lcs::DevBuf<unsigned char> iq;

@@ -17,6 +17,10 @@ typedef std::complex<double> cd;
 inline size_t iq_sample_bytes(int iq_format) {
   return iq_format == LCS_IQ_CU8 ? 2 : iq_format == LCS_IQ_CF32 ? 8 : iq_format == LCS_IQ_C128 ? 16 : 0;
 }
+// Bytes per complex sample of a format the channelizer and the spectrum take (ci16, cs8, cu8, cf32); 0 for anything else.
+inline size_t stream_sample_bytes(int fmt) {
+  return fmt == LCS_IQ_CI16 ? 4 : fmt == LCS_IQ_CS8 || fmt == LCS_IQ_CU8 ? 2 : fmt == LCS_IQ_CF32 ? 8 : 0;
+}
 
 // ---- geometry of the fused FP32 correlator (xcorr_fp32.cu) ----
 constexpr int XC_R = 7;                 // lags per lane (7*8 B stride is LDS.64 bank-conflict free)

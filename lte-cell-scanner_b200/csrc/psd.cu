@@ -182,10 +182,6 @@ __global__ void __launch_bounds__(ACC_THREADS) psd_accum_kernel(const float* __r
   acc[k] = s;
 }
 
-size_t sample_bytes(int fmt) {
-  return fmt == LCS_IQ_CI16 ? 4 : fmt == LCS_IQ_CS8 || fmt == LCS_IQ_CU8 ? 2 : fmt == LCS_IQ_CF32 ? 8 : 0;
-}
-
 }  // namespace psd
 }  // namespace lcs
 
@@ -194,7 +190,7 @@ using namespace lcs::psd;
 
 struct lcs_psd {
   lcs_ctx* ctx = nullptr;
-  int fmt = LCS_IQ_CI16, esz = 4;
+  int fmt = LCS_IQ_CI16;
   long long fs = 0;
   int lg = 0, lg1 = 0, lg2 = 0;          // lg1 = 0: one pass (N <= TILE)
   uint32_t N = 0;
@@ -206,15 +202,9 @@ struct lcs_psd {
   DevBuf<float> d_pw;
   DevBuf<double> d_acc;
   uint32_t chunk = 1;                    // segments per launch (bounds the device scratch)
-  std::vector<unsigned char> carry;      // stream samples from the first sample of the next segment on (< N of them)
+  SampleCarry carry;                     // stream samples from the first sample of the next segment on (< N of them)
   uint64_t n_seg = 0;                    // segments accumulated since the last read
-  cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-  double kernel_ms = 0;
-  uint64_t kernel_launches = 0;
-  ~lcs_psd() {
-    if (ev0) cudaEventDestroy(ev0);
-    if (ev1) cudaEventDestroy(ev1);
-  }
+  KernelClock clock;                     // the kernels of each launch chunk
 };
 
 namespace {
@@ -231,19 +221,14 @@ void launch_fft(const lcs_psd* p, const Params& P, cudaStream_t st) {
   }
 }
 
-// Segments [0, n) of the virtual input a (na samples) ++ b, whose sample 0 is the first sample of segment 0.
-lcs_status run(lcs_psd* p, const unsigned char* a, size_t na, const unsigned char* b, uint64_t n) {
+// Segments [0, n) of the virtual input carry ++ b, whose sample 0 is the first sample of segment 0.
+lcs_status run(lcs_psd* p, const unsigned char* b, uint64_t n) {
   lcs_ctx* ctx = p->ctx;
   cudaStream_t st = ctx->streams[0];
-  const size_t es = p->esz, N = p->N, hop = N / 2;
+  const size_t N = p->N, hop = N / 2;
   for (uint64_t c0 = 0; c0 < n; c0 += p->chunk) {
     const uint32_t ns = (uint32_t)std::min<uint64_t>(p->chunk, n - c0);
-    const size_t lo = c0 * hop, hi = (c0 + ns - 1) * hop + N;   // samples [lo, hi) of a ++ b
-    if (lo < na) LCS_CUDA(ctx, cudaMemcpyAsync(p->d_in.p, a + lo * es, (std::min(hi, na) - lo) * es, cudaMemcpyHostToDevice, st));
-    if (hi > na) {
-      const size_t s = std::max(lo, na);
-      LCS_CUDA(ctx, cudaMemcpyAsync(p->d_in.p + (s - lo) * es, b + (s - na) * es, (hi - s) * es, cudaMemcpyHostToDevice, st));
-    }
+    LCS_CUDA(ctx, p->carry.upload(b, c0 * hop, (c0 + ns - 1) * hop + N, p->d_in.p, st));
     Params P;
     P.in = p->d_in.p;
     P.n_seg = (int)ns;
@@ -254,7 +239,7 @@ lcs_status run(lcs_psd* p, const unsigned char* a, size_t na, const unsigned cha
     P.tw = p->d_tw.p;
     P.y = p->d_y.p;
     P.pw = p->d_pw.p;
-    LCS_CUDA(ctx, cudaEventRecord(p->ev0, st));
+    LCS_CUDA(ctx, p->clock.begin(st));
     switch (p->fmt) {
       case LCS_IQ_CI16: launch_fft<LCS_IQ_CI16>(p, P, st); break;
       case LCS_IQ_CS8: launch_fft<LCS_IQ_CS8>(p, P, st); break;
@@ -265,12 +250,8 @@ lcs_status run(lcs_psd* p, const unsigned char* a, size_t na, const unsigned cha
     const int launches = p->lg1 ? 3 : 2;
     ctx->launches += launches;
     LCS_CUDA(ctx, cudaGetLastError());
-    LCS_CUDA(ctx, cudaEventRecord(p->ev1, st));
+    LCS_CUDA(ctx, p->clock.end(st, launches));
     LCS_CUDA(ctx, cudaStreamSynchronize(st));
-    float ms = 0;
-    LCS_CUDA(ctx, cudaEventElapsedTime(&ms, p->ev0, p->ev1));
-    p->kernel_ms += ms;
-    p->kernel_launches += launches;
     p->n_seg += ns;
   }
   return LCS_OK;
@@ -285,7 +266,7 @@ lcs_status lcs_psd_create(lcs_ctx* ctx, double fs_in, int iq_format, uint32_t nf
   const double r = std::round(fs_in);
   if (!std::isfinite(fs_in) || std::fabs(fs_in - r) > 1e-6 || !(r > 0) || r > 250e6)
     return fail(ctx, LCS_ERR_ARG, "lcs_psd_create: fs_in must be an integer number of Hz in (0, 250] MHz");
-  if (!sample_bytes(iq_format))
+  if (!stream_sample_bytes(iq_format))
     return fail(ctx, LCS_ERR_ARG, "lcs_psd_create: iq_format must be LCS_IQ_CI16, CS8, CU8 or CF32");
   int lg = 0;
   while (lg <= LG_MAX && (1u << lg) < nfft) lg++;
@@ -295,7 +276,7 @@ lcs_status lcs_psd_create(lcs_ctx* ctx, double fs_in, int iq_format, uint32_t nf
   if (!p) return fail(ctx, LCS_ERR_STATE, "lcs_psd_create: out of memory");
   p->ctx = ctx;
   p->fmt = iq_format;
-  p->esz = (int)sample_bytes(iq_format);
+  p->carry.esz = stream_sample_bytes(iq_format);
   p->fs = (long long)r;
   p->N = nfft;
   p->lg = lg;
@@ -315,7 +296,7 @@ lcs_status lcs_psd_create(lcs_ctx* ctx, double fs_in, int iq_format, uint32_t nf
   // segments per launch: |X|^2 rows (and the four-step rows) within 64 MB
   const size_t per_seg = (size_t)nfft * (sizeof(float) + (p->lg1 ? sizeof(float2) : 0));
   p->chunk = (uint32_t)std::max<size_t>(1, (64ull << 20) / per_seg);
-  const size_t in_max = ((size_t)(p->chunk - 1) * (nfft / 2) + nfft) * p->esz;
+  const size_t in_max = ((size_t)(p->chunk - 1) * (nfft / 2) + nfft) * p->carry.esz;
   cudaError_t e = cudaSetDevice(ctx->device);
   if (e == cudaSuccess) e = p->d_win.alloc(nfft);
   if (e == cudaSuccess) e = p->d_tw.alloc(nfft);
@@ -326,8 +307,6 @@ lcs_status lcs_psd_create(lcs_ctx* ctx, double fs_in, int iq_format, uint32_t nf
   if (e == cudaSuccess) e = cudaMemcpy(p->d_win.p, win.data(), nfft * sizeof(float), cudaMemcpyHostToDevice);
   if (e == cudaSuccess) e = cudaMemcpy(p->d_tw.p, tw.data(), nfft * sizeof(float2), cudaMemcpyHostToDevice);
   if (e == cudaSuccess) e = cudaMemset(p->d_acc.p, 0, nfft * sizeof(double));
-  if (e == cudaSuccess) e = cudaEventCreate(&p->ev0);
-  if (e == cudaSuccess) e = cudaEventCreate(&p->ev1);
   if (e != cudaSuccess) {
     delete p;
     return fail(ctx, LCS_ERR_CUDA, std::string("lcs_psd_create: ") + cudaGetErrorString(e));
@@ -346,20 +325,15 @@ lcs_status lcs_psd_push(lcs_psd* p, const void* iq_host, uint32_t n_in) {
   if (!p) return LCS_ERR_ARG;
   if (!iq_host && n_in) return pfail(p, "lcs_psd_push: null samples");
   const unsigned char* b = static_cast<const unsigned char*>(iq_host);
-  const size_t es = p->esz, na = p->carry.size() / es, total = na + n_in, hop = p->N / 2;
+  const size_t total = p->carry.size() + n_in, hop = p->N / 2;
   const uint64_t k = total >= p->N ? (total - p->N) / hop + 1 : 0;   // segments this push completes
   if (k) {
     LCS_CUDA(p->ctx, cudaSetDevice(p->ctx->device));
-    lcs_status rc = run(p, p->carry.data(), na, b, k);
+    lcs_status rc = run(p, b, k);
     if (rc != LCS_OK) return rc;
   }
   // keep the samples from the first sample of the next segment on
-  const size_t drop = (size_t)k * hop;
-  std::vector<unsigned char> nc;
-  nc.reserve((total - drop) * es);
-  if (drop < na) nc.insert(nc.end(), p->carry.begin() + drop * es, p->carry.end());
-  if (n_in) nc.insert(nc.end(), b + (drop > na ? drop - na : 0) * es, b + (size_t)n_in * es);
-  p->carry.swap(nc);
+  p->carry.advance(b, n_in, (size_t)k * hop);
   return LCS_OK;
 }
 
@@ -383,10 +357,7 @@ lcs_status lcs_psd_read(lcs_psd* p, double* out, uint64_t* n_segments) {
 lcs_status lcs_psd_timing_read(lcs_psd* p, double* kernel_ms, uint64_t* launches) {
   if (!p) return LCS_ERR_ARG;
   if (!kernel_ms || !launches) return pfail(p, "lcs_psd_timing_read: null pointer");
-  *kernel_ms = p->kernel_ms;
-  *launches = p->kernel_launches;
-  p->kernel_ms = 0;
-  p->kernel_launches = 0;
+  LCS_CUDA(p->ctx, p->clock.read(kernel_ms, launches));
   return LCS_OK;
 }
 

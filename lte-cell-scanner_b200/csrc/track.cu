@@ -757,13 +757,7 @@ struct lcs_track {
   DevBuf<Scratch> d_scr;
   DevBuf<unsigned char> d_iq;
   PinBuf<unsigned char> h_iq;
-  cudaEvent_t ev0 = nullptr, ev1 = nullptr;    // around each launch
-  double kernel_ms = 0;                        // accumulated since the last lcs_track_timing_read
-  uint64_t kernel_launches = 0;
-  ~lcs_track() {
-    if (ev0) cudaEventDestroy(ev0);
-    if (ev1) cudaEventDestroy(ev1);
-  }
+  KernelClock clock;                           // one kernel per push that completes a block
 };
 
 static lcs_status tfail(lcs_track* t, lcs_status st, const char* msg) {
@@ -800,8 +794,6 @@ lcs_status lcs_track_create(lcs_ctx* ctx, uint32_t n_ch, const double* fc_reques
   if (e == cudaSuccess) e = t->d_scr.alloc(nc);
   if (e == cudaSuccess) e = cudaMemcpy(t->d_ch.p, h.data(), n_ch * sizeof(ChanState), cudaMemcpyHostToDevice);
   if (e == cudaSuccess) e = cudaMemset(t->d_cells.p, 0, nc * sizeof(CellState));
-  if (e == cudaSuccess) e = cudaEventCreate(&t->ev0);
-  if (e == cudaSuccess) e = cudaEventCreate(&t->ev1);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(track_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, BLOCK * (int)sizeof(double));
   if (e != cudaSuccess) {
     delete t;
@@ -918,16 +910,12 @@ lcs_status lcs_track_push_cu8(lcs_track* t, const uint8_t* iq_host, uint32_t n) 
     P.cells = t->d_cells.p;
     P.tab = t->d_tab.p;
     P.scr = t->d_scr.p;
-    LCS_CUDA(t->ctx, cudaEventRecord(t->ev0, st));
+    LCS_CUDA(t->ctx, t->clock.begin(st));
     track_kernel<<<t->n_ch, THREADS, BLOCK * sizeof(double), st>>>(P);
     t->ctx->launches++;
     LCS_CUDA(t->ctx, cudaGetLastError());
-    LCS_CUDA(t->ctx, cudaEventRecord(t->ev1, st));
+    LCS_CUDA(t->ctx, t->clock.end(st, 1));
     LCS_CUDA(t->ctx, cudaStreamSynchronize(st));
-    float ms = 0;
-    LCS_CUDA(t->ctx, cudaEventElapsedTime(&ms, t->ev0, t->ev1));
-    t->kernel_ms += ms;
-    t->kernel_launches++;
   }
   t->carry.swap(carry);
   t->carry_n = (uint32_t)rest;
@@ -937,10 +925,7 @@ lcs_status lcs_track_push_cu8(lcs_track* t, const uint8_t* iq_host, uint32_t n) 
 lcs_status lcs_track_timing_read(lcs_track* t, double* kernel_ms, uint64_t* launches) {
   if (!t) return LCS_ERR_ARG;
   if (!kernel_ms || !launches) return tfail(t, LCS_ERR_ARG, "lcs_track_timing_read: null pointer");
-  *kernel_ms = t->kernel_ms;
-  *launches = t->kernel_launches;
-  t->kernel_ms = 0;
-  t->kernel_launches = 0;
+  LCS_CUDA(t->ctx, t->clock.read(kernel_ms, launches));
   return LCS_OK;
 }
 

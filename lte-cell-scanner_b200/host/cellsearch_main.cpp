@@ -68,13 +68,8 @@ static string freq_formatter(const double& freq) {   // CellSearch.cpp:322-341
 }
 
 // ---- --spectrum ----------------------------------------------------------------------------------------------------------
-// The checks of --spectrum that need no device: sample format, rate, --fc-in and a readable recording.
-static bool spectrum_args(const string& wideband, const string& format, double fs_in, double fc_in, int* fmt) {
-  if (format == "ci16") *fmt = LCS_IQ_CI16;
-  else if (format == "cs8") *fmt = LCS_IQ_CS8;
-  else if (format == "cu8") *fmt = LCS_IQ_CU8;
-  else if (format == "cf32") *fmt = LCS_IQ_CF32;
-  else { cerr << "Error: --format must be ci16, cs8, cu8 or cf32" << endl; return false; }
+// The checks of --spectrum that need no device: rate, --fc-in and a readable recording.
+static bool spectrum_args(const string& wideband, double fs_in, double fc_in) {
   if (!(fs_in > 0 && fs_in <= 250e6) || std::fabs(fs_in - std::round(fs_in)) > 1e-6) {
     cerr << "Error: --spectrum needs --fs-in, an integer number of Hz in (0, 250] MHz" << endl;
     return false;
@@ -94,11 +89,11 @@ static FILE* open_output(const string& path) {
 
 // Welch PSD of the whole recording (wideband_psd), written to `out` as freq_hz,psd_dbfs_per_hz lines; psd is kept for the
 // carrier-power column.
-static void write_spectrum(const string& wideband, int fmt, double fs_in, double fc_in, uint32_t nfft, const string& path,
-                           FILE* out, vector<double>& psd) {
+static void write_spectrum(const string& wideband, int fmt, size_t bytes, double fs_in, double fc_in, uint32_t nfft,
+                           const string& path, FILE* out, vector<double>& psd) {
   uint64_t n_seg = 0;
   try {
-    wideband_psd(wideband, fmt, fs_in, nfft, psd, n_seg);
+    wideband_psd(wideband, fmt, bytes, fs_in, nfft, psd, n_seg);
   } catch (const char*) {
     std::fclose(out);
     throw;
@@ -175,14 +170,22 @@ int main(int argc, char* const argv[]) {
   const bool spec = !spectrum.empty(), search = !spec || freq_start != -1;   // --spectrum alone: no search
   if (spec && wideband.empty()) { cerr << "Error: --spectrum needs --wideband" << endl; return -1; }
   if (nfft < 64 || nfft > 65536 || (nfft & (nfft - 1))) { cerr << "Error: --nfft must be a power of two in [64, 65536]" << endl; return -1; }
-  int spec_format = LCS_IQ_CI16;
+  const bool wide = !wideband.empty();
+  int wide_format = LCS_IQ_CI16;   // --format, for the spectrum and the search
+  size_t wide_bytes = 4;           // per sample
+  if (wide) {
+    if (format == "cs8") { wide_format = LCS_IQ_CS8; wide_bytes = 2; }
+    else if (format == "cu8") { wide_format = LCS_IQ_CU8; wide_bytes = 2; }
+    else if (format == "cf32") { wide_format = LCS_IQ_CF32; wide_bytes = 8; }
+    else if (format != "ci16") { cerr << "Error: --format must be ci16, cs8, cu8 or cf32" << endl; return -1; }
+  }
   FILE* spec_file = nullptr;
   vector<double> psd;
-  if (spec && !spectrum_args(wideband, format, fs_in, fc_in, &spec_format)) return -1;
+  if (spec && !spectrum_args(wideband, fs_in, fc_in)) return -1;
   if (!search) {
     if (!(spec_file = open_output(spectrum))) return -1;
     try {
-      write_spectrum(wideband, spec_format, fs_in, fc_in, (uint32_t)nfft, spectrum, spec_file, psd);
+      write_spectrum(wideband, wide_format, wide_bytes, fs_in, fc_in, (uint32_t)nfft, spectrum, spec_file, psd);
     } catch (const char* msg) {
       cerr << "Error: " << msg << endl;
       return -1;
@@ -204,7 +207,6 @@ int main(int argc, char* const argv[]) {
   if (ppm < 0) { cerr << "Error: ppm value must be positive" << endl; return -1; }
   if (ppm > 200) cout << "Warning: ppm value appears to be set unreasonably high" << endl;
   if (abs(correction - 1) > 1000e-6) cout << "Warning: crystal correction factor appears to be unreasonable" << endl;
-  const bool wide = !wideband.empty();
   if (save_cap || (!use_recorded_data && !wide)) {
     cerr << "Error: live capture / recording needs an rtl-sdr dongle, which this build does not support; use -l or --wideband" << endl;
     return -1;
@@ -212,16 +214,10 @@ int main(int argc, char* const argv[]) {
   // wideband recording: every argument and the file length are checked before any device work
   vector<unsigned char> wide_iq;
   uint32_t wide_n = 0;
-  int wide_format = LCS_IQ_CI16;
-  size_t wide_bytes = 4;   // per sample
   if (wide) {
     if (use_recorded_data || batched) { cerr << "Error: --wideband cannot be combined with -l or --sweep" << endl; return -1; }
     if (fc_in <= 0) { cerr << "Error: --wideband needs --fc-in" << endl; return -1; }
-    if (format == "cs8") { wide_format = LCS_IQ_CS8; wide_bytes = 2; }
-    else if (format == "cu8") { wide_format = LCS_IQ_CU8; wide_bytes = 2; }
-    else if (format == "cf32") { wide_format = LCS_IQ_CF32; wide_bytes = 8; }
-    else if (format != "ci16") { cerr << "Error: --format must be ci16, cs8, cu8 or cf32" << endl; return -1; }
-    if (!resample && format != "ci16") { cerr << "Error: --format needs --resample" << endl; return -1; }
+    if (!resample && wide_format != LCS_IQ_CI16) { cerr << "Error: --format needs --resample" << endl; return -1; }
     uint32_t n_taps = 0, up = 1, down = 1;
     if (resample) {
       if (lcs_chan_design_rational(fs_in, &up, &down, nullptr, &n_taps) != LCS_OK) {
@@ -282,7 +278,7 @@ int main(int argc, char* const argv[]) {
     const int n_fc = (int)floor((freq_end - freq_start) / 100e3) + 1;                   // :465
     vector<list<Cell> > detected_cells(n_fc);
     xcorr_pss_skip_debug_outputs(true);
-    if (spec) write_spectrum(wideband, spec_format, fs_in, fc_in, (uint32_t)nfft, spectrum, spec_file, psd);
+    if (spec) write_spectrum(wideband, wide_format, wide_bytes, fs_in, fc_in, (uint32_t)nfft, spectrum, spec_file, psd);
     if (wide) {
       // every raster point channelized out of the one recording on the device, then the batched search in place
       vector<double> fcs;

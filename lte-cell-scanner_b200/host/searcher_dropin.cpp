@@ -138,9 +138,8 @@ void wideband_search_rational(const void* iq, int iq_format, uint32_t n, double 
   wideband_search(iq, iq_format, n, fs_in, fc_in, fc_requested, f_search_set, fs_programmed, detected_cells);
 }
 
-void wideband_psd(const std::string& path, int iq_format, double fs_in, uint32_t nfft, std::vector<double>& psd,
+void wideband_psd(const std::string& path, int iq_format, size_t es, double fs_in, uint32_t nfft, std::vector<double>& psd,
                   uint64_t& n_segments) {
-  const size_t es = iq_format == LCS_IQ_CI16 ? 4 : iq_format == LCS_IQ_CF32 ? 8 : 2;
   const size_t block = (size_t)1 << 22;                              // samples per push
   FILE* f = std::fopen(path.c_str(), "rb");
   if (!f) throw("wideband_psd: cannot read the recording");

@@ -105,7 +105,7 @@ void wideband_search_rational(const void* iq, int iq_format, uint32_t n, double 
                               const std::vector<double>& fc_requested, const itpp::vec& f_search_set,
                               const double& fs_programmed, std::vector<std::list<Cell> >& detected_cells);
    // skip the 136 MB `xc`/`sp`/`xc_incoherent` debug outputs (CLI does)
-// Welch power spectral density (lcs_psd of liblcs_psd.so, DESIGN.md section 4.8) of the whole recording in `path` ([n][2] in iq_format at
-// fs_in, read in blocks): psd [nfft] in fftshift order, full-scale^2 per Hz, over n_segments segments.
-void wideband_psd(const std::string& path, int iq_format, double fs_in, uint32_t nfft, std::vector<double>& psd,
-                  uint64_t& n_segments);
+// Welch power spectral density (lcs_psd of liblcs_psd.so, DESIGN.md section 4.8) of the whole recording in `path` ([n][2] in iq_format,
+// sample_bytes per sample, at fs_in, read in blocks): psd [nfft] in fftshift order, full-scale^2 per Hz, over n_segments segments.
+void wideband_psd(const std::string& path, int iq_format, size_t sample_bytes, double fs_in, uint32_t nfft,
+                  std::vector<double>& psd, uint64_t& n_segments);

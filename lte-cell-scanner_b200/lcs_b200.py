@@ -167,13 +167,20 @@ class _Handle:
     """A library object: `_h` is its handle, freed by the function named `_destroy` on close() or garbage collection."""
     _h = None
     _destroy = None
+    _timing_read = None               # the handle's lcs_*_timing_read, if it times its kernels
 
-    _lib = staticmethod(lib)          # the library that owns `_destroy`
+    _lib = staticmethod(lib)          # the library that owns `_destroy` and `_timing_read`
 
     def close(self):
         if self._h:
             getattr(self._lib(), self._destroy)(self._h)
             self._h = C.c_void_p()
+
+    def timing_read(self):
+        """(kernel ms, kernel launches) since the last read, from CUDA events around the launches."""
+        ms = C.c_double(0); n = C.c_uint64(0)
+        _chk(getattr(self._lib(), self._timing_read)(self._h, C.byref(ms), C.byref(n)), self.ctx._h)
+        return ms.value, n.value
 
     def __del__(self):
         try:
@@ -338,6 +345,7 @@ class Context(_Handle):
 class XcorrPlan(_Handle):
     """lcs_xcorr_plan: templates + fold offsets + scratch for a fixed search configuration."""
     _destroy = "lcs_xcorr_plan_destroy"
+    _timing_read = "lcs_xcorr_plan_timing_read"
 
     def __init__(self, ctx, n_cap, f_set, ds_comb_arm, fc_requested, fc_programmed, fs_programmed, max_batch, kernel):
         self.ctx = ctx
@@ -353,11 +361,6 @@ class XcorrPlan(_Handle):
 
     def timing_enable(self, on=True):
         _chk(lib().lcs_xcorr_plan_timing_enable(self._h, int(bool(on))), self.ctx._h)
-
-    def timing_read(self):
-        ms = C.c_double(0); n = C.c_uint64(0)
-        _chk(lib().lcs_xcorr_plan_timing_read(self._h, C.byref(ms), C.byref(n)), self.ctx._h)
-        return ms.value, n.value
 
     def kernel_for(self, iq_format):
         return lib().lcs_xcorr_plan_kernel(self._h, int(iq_format))
@@ -544,6 +547,7 @@ TRACK_BLOCK = 10000
 class Tracker(_Handle):
     """lcs_track: the per-cell tracker loop of LTE-Tracker for every cell of n_ch channels, one launch per push."""
     _destroy = "lcs_track_destroy"
+    _timing_read = "lcs_track_timing_read"
 
     def __init__(self, ctx, fc_requested, frequency_offset, fs_programmed=1.92e6, fc_programmed=None, max_cells=8):
         self.ctx = ctx
@@ -577,12 +581,6 @@ class Tracker(_Handle):
         _chk(lib().lcs_track_sample_time(self._h, ch, C.byref(v)), self.ctx._h)
         return v.value
 
-    def timing_read(self):
-        """(kernel ms, launches) since the last read, from CUDA events around each launch."""
-        ms = C.c_double(0); n = C.c_uint64(0)
-        _chk(lib().lcs_track_timing_read(self._h, C.byref(ms), C.byref(n)), self.ctx._h)
-        return ms.value, n.value
-
     def read(self, ch=0):
         """The channel's cells in the order added, as dicts; a dropped cell is reported once."""
         out = (TrackCell * self.max_cells)()
@@ -609,17 +607,34 @@ CHAN_FORMATS = {"ci16": (IQ_CI16, np.int16), "cs8": (IQ_CS8, np.int8), "cu8": (I
                 "cf32": (IQ_CF32, np.float32)}
 
 
+def _iq_format(fmt):
+    """The lcs format of a sample format name of CHAN_FORMATS."""
+    if fmt not in CHAN_FORMATS:
+        raise ValueError("fmt must be one of %s" % ", ".join(CHAN_FORMATS))
+    return CHAN_FORMATS[fmt][0]
+
+
+def _samples(iq, fmt):
+    """iq as a contiguous [n][2] array of fmt's dtype (complex64 [n] is accepted for cf32)."""
+    dtype = CHAN_FORMATS[fmt][1]
+    iq = np.asarray(iq)
+    if fmt == "cf32" and iq.dtype == np.complex64 and iq.ndim == 1:
+        iq = iq.view(np.float32).reshape(-1, 2)
+    if iq.dtype != dtype or iq.ndim != 2 or iq.shape[1] != 2:
+        raise ValueError("expected %s samples: %s [n][2]" % (fmt, np.dtype(dtype).name))
+    return np.ascontiguousarray(iq)
+
+
 class RationalChannelizer(_Handle):
     """lcs_chan at any allowed SDR rate: a wideband ci16 / cs8 / cu8 / cf32 recording -> one 1.92 Msps cu8 stream per LTE
     raster channel, resampled by up / down (DESIGN.md sections 4.6 and 4.7)."""
     _destroy = "lcs_chan_destroy"
+    _timing_read = "lcs_chan_timing_read"
 
     def __init__(self, ctx, fs_in, fc_in, fc_ch, fmt="ci16", gain=None):
-        if fmt not in CHAN_FORMATS:
-            raise ValueError("fmt must be one of %s" % ", ".join(CHAN_FORMATS))
+        self._iq_format = _iq_format(fmt)
         self.ctx = ctx
         self.fmt = fmt
-        self._iq_format, self._dtype = CHAN_FORMATS[fmt]
         fc = np.ascontiguousarray(np.atleast_1d(fc_ch), np.float64)
         self.n_ch = fc.size
         self.fc_ch = fc
@@ -634,13 +649,7 @@ class RationalChannelizer(_Handle):
                                               C.byref(self._h))
 
     def _samples(self, iq):
-        """iq as a contiguous [n][2] array of the format's dtype (complex64 [n] is accepted for cf32)."""
-        iq = np.asarray(iq)
-        if self.fmt == "cf32" and iq.dtype == np.complex64 and iq.ndim == 1:
-            iq = iq.view(np.float32).reshape(-1, 2)
-        if iq.dtype != self._dtype or iq.ndim != 2 or iq.shape[1] != 2:
-            raise ValueError("expected %s samples: %s [n][2]" % (self.fmt, np.dtype(self._dtype).name))
-        return np.ascontiguousarray(iq)
+        return _samples(iq, self.fmt)
 
     def auto_gain(self, iq):
         """Set every channel's gain to 0.25 / RMS of its output over these samples (the stream is not touched)."""
@@ -682,12 +691,6 @@ class RationalChannelizer(_Handle):
              self.ctx._h)
         return got.value, clip
 
-    def timing_read(self):
-        """(kernel ms, launches) since the last read, from CUDA events around each launch."""
-        ms = C.c_double(0); n = C.c_uint64(0)
-        _chk(lib().lcs_chan_timing_read(self._h, C.byref(ms), C.byref(n)), self.ctx._h)
-        return ms.value, n.value
-
 
 class Channelizer(RationalChannelizer):
     """The ci16 channelizer of DESIGN.md section 4.6, made by lcs_chan_create: fs_in must be D * 1.92 MHz."""
@@ -714,25 +717,22 @@ class Spectrum(_Handle):
     """lcs_psd: Welch's power spectral density of a wideband ci16 / cs8 / cu8 / cf32 recording pushed in pieces of any
     size, periodic Hann window of nfft points, hop nfft/2 (DESIGN.md section 4.8)."""
     _destroy = "lcs_psd_destroy"
+    _timing_read = "lcs_psd_timing_read"
     _lib = staticmethod(psd_lib)
 
     def __init__(self, ctx, fs_in, fmt="ci16", nfft=4096, fc_in=0.0):
-        if fmt not in CHAN_FORMATS:
-            raise ValueError("fmt must be one of %s" % ", ".join(CHAN_FORMATS))
+        iq_format = _iq_format(fmt)
         self.ctx = ctx
         self.fmt = fmt
         self.fs_in = float(fs_in)
         self.fc_in = float(fc_in)
         self.nfft = int(nfft)
-        self._iq_format, self._dtype = CHAN_FORMATS[fmt]
         self._h = C.c_void_p()
-        _chk(psd_lib().lcs_psd_create(ctx._h, fs_in, self._iq_format, nfft, C.byref(self._h)), ctx._h)
-
-    _samples = RationalChannelizer._samples
+        _chk(psd_lib().lcs_psd_create(ctx._h, fs_in, iq_format, nfft, C.byref(self._h)), ctx._h)
 
     def push(self, iq):
         """Push [n][2] samples in the handle's format (complex64 [n] is accepted for cf32)."""
-        iq = self._samples(iq)
+        iq = _samples(iq, self.fmt)
         _chk(psd_lib().lcs_psd_push(self._h, _p(iq), iq.shape[0]), self.ctx._h)
 
     @property
@@ -747,9 +747,3 @@ class Spectrum(_Handle):
         n = C.c_uint64(0)
         _chk(psd_lib().lcs_psd_read(self._h, _p(psd), C.byref(n)), self.ctx._h)
         return self.freqs, psd, n.value
-
-    def timing_read(self):
-        """(kernel ms, kernel launches) since the last read, from CUDA events around the kernels of each launch chunk."""
-        ms = C.c_double(0); n = C.c_uint64(0)
-        _chk(psd_lib().lcs_psd_timing_read(self._h, C.byref(ms), C.byref(n)), self.ctx._h)
-        return ms.value, n.value

@@ -314,7 +314,8 @@ def test_tracker_push_size_and_time_stamps(lcs, ctx):
                     r["crs_np_av"].tobytes(), r["mib_attempts"]))
         g.close()
     assert res[0] == res[1] == res[2]
-    # a framer fed block by block with the tracker's offsets keeps the same time stamps
+    # a framer fed block by block with the tracker's offsets keeps the same time stamps; every push completes a block,
+    # so it is one kernel launch, which a timing read reports once
     g = lcs.Tracker(ctx, FC, 1900.0)
     g.add_cell(0, lcs_cell(d), d["t0"] - 2 + 0.3)
     fr = lcs.Framer(FC, FC, 1.92e6)
@@ -323,6 +324,10 @@ def test_tracker_push_size_and_time_stamps(lcs, ctx):
         g.push_cu8(cu8[i:i + 10000])
         fr.push(cu8[i:i + 10000], fo)
         assert g.sample_time() == fr.sample_time()
+        ms, launches = g.timing_read()
+        assert launches == 1 and ms > 0
+    g.push_cu8(cu8[:9999])                          # completes no block: no launch
+    assert g.timing_read() == (0.0, 0)
 
 
 @pytest.mark.gpu
