@@ -53,6 +53,9 @@ static void print_usage() {
   cout << "                                 then be omitted (no search), and --fs-in may be any integer number of Hz up to" << endl;
   cout << "                                 250 MHz and --format any of the four without --resample" << endl;
   cout << "     --nfft N                    with --spectrum: FFT length, a power of two in [64, 65536] (default 4096)" << endl;
+  cout << "     --measure                   add RSRP[dBFS] RSRQ[dB] SINR[dB] columns (antenna port 0) to the cell table," << endl;
+  cout << "                                 measured on the GPU from the CRS of each cell's central 6 RBs over 60 ms of the" << endl;
+  cout << "                                 capture (with --wideband, RSRP in the recording's full scale)" << endl;
   cout << "  -r --record / -i --device-index need a live rtl-sdr dongle: not supported by this build" << endl;
 }
 
@@ -107,6 +110,20 @@ static void write_spectrum(const string& wideband, int fmt, size_t bytes, double
     cout << "Power spectrum of " << wideband << " (" << n_seg << " segments of " << nfft << " samples) written to " << path << endl;
 }
 
+// The measurement of a final (deduplicated) cell: that of the detected cell it was copied from, in the list of its
+// centre frequency.
+static const lcs_cell_meas* measurement_of(const Cell& c, double freq_start, const vector<list<Cell> >& detected,
+                                           const vector<vector<lcs_cell_meas> >& meas) {
+  const long fci = std::lround((c.fc_requested - freq_start) / 100e3);
+  if (fci < 0 || fci >= (long)detected.size() || fci >= (long)meas.size()) return nullptr;
+  size_t k = 0;
+  for (list<Cell>::const_iterator it = detected[fci].begin(); it != detected[fci].end(); ++it, ++k)
+    if (it->n_id_cell() == c.n_id_cell() && it->frame_start == c.frame_start && it->freq_superfine == c.freq_superfine &&
+        k < meas[fci].size())
+      return &meas[fci][k];
+  return nullptr;
+}
+
 // 10 log10 of the power in the bins whose centre lies within n_rb_dl * 90 kHz of the cell's carrier fc_requested +
 // freq_superfine, in full-scale^2 (dBFS).
 static double carrier_power_dbfs(const vector<double>& psd, double fs_in, double fc_in, const Cell& c) {
@@ -125,7 +142,7 @@ int main(int argc, char* const argv[]) {
   bool save_cap = false, use_recorded_data = false, raw = false, batched = false;
   string data_dir = ".", wideband, format = "ci16";
   double fs_in = -1, fc_in = -1;
-  bool resample = false;
+  bool resample = false, measure = false;
   string spectrum;
   long nfft = 4096;
   static struct option long_options[] = {
@@ -135,7 +152,7 @@ int main(int argc, char* const argv[]) {
       {"data-dir", required_argument, 0, 'd'},   {"device-index", required_argument, 0, 'i'}, {"raw", no_argument, 0, 'R'}, {"sweep", no_argument, 0, 'W'},
       {"wideband", required_argument, 0, 'B'},   {"fs-in", required_argument, 0, 'F'},   {"fc-in", required_argument, 0, 'C'},
       {"resample", no_argument, 0, 'S'},         {"format", required_argument, 0, 'T'},
-      {"spectrum", required_argument, 0, 'P'},   {"nfft", required_argument, 0, 'N'},
+      {"spectrum", required_argument, 0, 'P'},   {"nfft", required_argument, 0, 'N'},   {"measure", no_argument, 0, 'M'},
       {0, 0, 0, 0}};
   for (;;) {
     int idx = 0;
@@ -162,6 +179,7 @@ int main(int argc, char* const argv[]) {
       case 'T': format = optarg; break;
       case 'P': spectrum = optarg; break;
       case 'N': nfft = strtol(optarg, &endp, 10); if (optarg == endp || *endp) { cerr << "Error: could not parse --nfft" << endl; return -1; } break;
+      case 'M': measure = true; break;
       case 'i': break;
       default: return -1;
     }
@@ -169,6 +187,7 @@ int main(int argc, char* const argv[]) {
   if (optind < argc) { cerr << "Error: unknown/extra arguments specified on command line" << endl; return -1; }
   const bool spec = !spectrum.empty(), search = !spec || freq_start != -1;   // --spectrum alone: no search
   if (spec && wideband.empty()) { cerr << "Error: --spectrum needs --wideband" << endl; return -1; }
+  if (measure && !search) { cerr << "Error: --measure needs a search (-s)" << endl; return -1; }
   if (nfft < 64 || nfft > 65536 || (nfft & (nfft - 1))) { cerr << "Error: --nfft must be a power of two in [64, 65536]" << endl; return -1; }
   const bool wide = !wideband.empty();
   int wide_format = LCS_IQ_CI16;   // --format, for the spectrum and the search
@@ -277,6 +296,7 @@ int main(int argc, char* const argv[]) {
     for (int i = 0; i < 2 * n_extra + 1; i++) f_search_set(i) = (i - (int)n_extra) * 5000.0;
     const int n_fc = (int)floor((freq_end - freq_start) / 100e3) + 1;                   // :465
     vector<list<Cell> > detected_cells(n_fc);
+    vector<vector<lcs_cell_meas> > meas;   // --measure: meas[fci][k] of detected_cells[fci]'s k-th cell
     xcorr_pss_skip_debug_outputs(true);
     if (spec) write_spectrum(wideband, wide_format, wide_bytes, fs_in, fc_in, (uint32_t)nfft, spectrum, spec_file, psd);
     if (wide) {
@@ -286,10 +306,10 @@ int main(int argc, char* const argv[]) {
       if (verbosity >= 1) cout << "Channelizing and examining " << n_fc << " center frequencies of one wideband recording ..." << endl;
       if (resample)
         wideband_search_rational(wide_iq.data(), wide_format, wide_n, fs_in, fc_in, fcs, f_search_set, fs_programmed,
-                                 detected_cells);
+                                 detected_cells, measure ? &meas : nullptr);
       else
         wideband_search_ci16(reinterpret_cast<const int16_t*>(wide_iq.data()), wide_n, fs_in, fc_in, fcs, f_search_set,
-                             fs_programmed, detected_cells);
+                             fs_programmed, detected_cells, measure ? &meas : nullptr);
     }
     if (batched) {
       // every centre frequency of the sweep in one call: the raw byte dumps are concatenated and handed to the batched
@@ -310,6 +330,7 @@ int main(int argc, char* const argv[]) {
       }
       if (verbosity >= 1) cout << "Examining " << n_fc << " center frequencies in one batched sweep ..." << endl;
       sweep_search_cu8(all, n_cap, fcs, f_search_set, fs_programmed, detected_cells);
+      if (measure) measure_cells(all.data(), LCS_IQ_CU8, n_cap, detected_cells, fs_programmed, meas);
     }
     if (batched || wide) {
       if (verbosity >= 1)
@@ -373,6 +394,13 @@ int main(int argc, char* const argv[]) {
         }
         ++it;
       }
+      if (measure) {   // this centre frequency's cells on its own capture buffer
+        vector<vector<lcs_cell_meas> > m;
+        measure_cells(capbuf._data(), LCS_IQ_C128, (uint32_t)capbuf.length(), vector<list<Cell> >(1, detected_cells[fci]),
+                      fs_programmed, m);
+        meas.resize(n_fc);
+        meas[fci] = m[0];
+      }
     }
     list<Cell> cells_final;
     dedup(detected_cells, cells_final);
@@ -381,7 +409,8 @@ int main(int argc, char* const argv[]) {
     } else {   // CellSearch.cpp:579-613
       cout << "Detected the following cells:" << endl;
       cout << "A: #antenna ports C: CP type ; P: PHICH duration ; PR: PHICH resource type" << endl;
-      cout << "CID A      fc   foff RXPWR C nRB P  PR CrystalCorrectionFactor" << (spec ? " CarrierPower[dBFS]" : "") << endl;
+      cout << "CID A      fc   foff RXPWR C nRB P  PR CrystalCorrectionFactor" << (spec ? " CarrierPower[dBFS]" : "")
+           << (measure ? " RSRP[dBFS] RSRQ[dB] SINR[dB]" : "") << endl;
       for (list<Cell>::iterator it = cells_final.begin(); it != cells_final.end(); ++it) {
         stringstream ss;
         ss << setw(3) << (*it).n_id_cell();
@@ -403,6 +432,12 @@ int main(int argc, char* const argv[]) {
         const double correction_new = correction * ((*it).fc_requested / crystal_freq_actual);
         ss << " " << setprecision(20) << correction_new;
         if (spec) ss << " " << fixed << setprecision(2) << carrier_power_dbfs(psd, fs_in, fc_in, *it);
+        if (measure) {
+          const lcs_cell_meas* m = measurement_of(*it, freq_start, detected_cells, meas);
+          if (!m) throw("--measure: a listed cell has no measurement");
+          ss << " " << fixed << setprecision(2) << 10 * log10(m->rsrp[0]) << " " << 10 * log10(m->rsrq) << " "
+             << 10 * log10(m->sinr[0]);
+        }
         cout << ss.str() << endl;
       }
     }

@@ -2,6 +2,7 @@
 // (include/searcher.h:22-124), bodies marshal the IT++ containers to the C ABI of
 // include/lcs_b200.h and back.  No numerical work happens here.
 #include "searcher_dropin.hpp"
+#include "../../include/lcs_meas.h"
 #include "../../include/lcs_psd.h"
 
 #include <cmath>
@@ -66,6 +67,39 @@ static Cell from_pod(const lcs_cell& p) {
   return c;
 }
 
+// lcs_meas_cells on every cell of cells[c], found in channel c of iq ([cells.size()][n_cap][2]); meas[c][k] is the k-th
+// cell's.  Returns the status and sets *where for check().
+static lcs_status measure_lists(const void* iq, int iq_format, int on_device, uint32_t n_cap,
+                                const std::vector<std::list<Cell> >& cells, double fs_programmed,
+                                std::vector<std::vector<lcs_cell_meas> >& meas, const char** where) {
+  std::vector<lcs_cell> flat;
+  std::vector<uint32_t> ch;
+  for (size_t c = 0; c < cells.size(); c++)
+    for (const Cell& cell : cells[c]) {
+      flat.push_back(to_pod(cell));
+      ch.push_back((uint32_t)c);
+    }
+  std::vector<lcs_cell_meas> out(flat.size());
+  lcs_meas* m = nullptr;
+  *where = "lcs_meas_create";
+  lcs_status rc = lcs_meas_create(lcs_dropin_ctx(), &m);
+  if (rc == LCS_OK) {
+    rc = lcs_meas_cells(m, iq, iq_format, on_device, (uint32_t)cells.size(), n_cap, flat.data(), ch.data(),
+                        (uint32_t)flat.size(), fs_programmed, out.data());
+    *where = "lcs_meas_cells";
+  }
+  if (m) lcs_meas_destroy(m);
+  meas.assign(cells.size(), std::vector<lcs_cell_meas>());
+  for (size_t i = 0; i < flat.size(); i++) meas[ch[i]].push_back(out[i]);
+  return rc;
+}
+
+void measure_cells(const void* iq, int iq_format, uint32_t n_cap, const std::vector<std::list<Cell> >& detected_cells,
+                   const double& fs_programmed, std::vector<std::vector<lcs_cell_meas> >& meas) {
+  const char* where = "";
+  check(measure_lists(iq, iq_format, 0, n_cap, detected_cells, fs_programmed, meas, &where), where);
+}
+
 void sweep_search_cu8(const std::vector<unsigned char>& iq, uint32_t n_cap, const std::vector<double>& fc_requested,
                       const vec& f_search_set, const double& fs_programmed, std::vector<std::list<Cell> >& detected_cells) {
   const uint32_t n_ch = (uint32_t)fc_requested.size(), max_cells = 16;
@@ -86,7 +120,7 @@ void sweep_search_cu8(const std::vector<unsigned char>& iq, uint32_t n_cap, cons
 // iq_format < 0: lcs_chan_create (ci16 at D * 1.92 MHz); otherwise lcs_chan_create_rational with that format
 static void wideband_search(const void* iq, int iq_format, uint32_t n, double fs_in, double fc_in,
                             const std::vector<double>& fc_requested, const vec& f_search_set, const double& fs_programmed,
-                            std::vector<std::list<Cell> >& detected_cells) {
+                            std::vector<std::list<Cell> >& detected_cells, std::vector<std::vector<lcs_cell_meas> >* meas) {
   const uint32_t n_ch = (uint32_t)fc_requested.size(), max_cells = 16, n_cap = 153600;
   lcs_ctx* ctx = lcs_dropin_ctx();
   lcs_chan* ch = nullptr;
@@ -118,24 +152,40 @@ static void wideband_search(const void* iq, int iq_format, uint32_t n, double fs
                                      (uint32_t)f_search_set.length(), cells.data(), max_cells, found.data());
     where = "lcs_sweep_search_cu8_device";
   }
+  if (rc == LCS_OK) {
+    detected_cells.assign(n_ch, std::list<Cell>());
+    for (uint32_t c = 0; c < n_ch; c++)
+      for (uint32_t k = 0; k < found[c] && k < max_cells; k++) detected_cells[c].push_back(from_pod(cells[(size_t)c * max_cells + k]));
+  }
+  // measured on the channelized buffers in place, then brought back to the recording's full scale: channel c's bytes
+  // carry gain[c] times the recording
+  std::vector<float> gain(n_ch);
+  if (rc == LCS_OK && meas) rc = measure_lists(d_iq, LCS_IQ_CU8, 1, n_cap, detected_cells, fs_programmed, *meas, &where);
+  if (rc == LCS_OK && meas) { rc = lcs_chan_gain(ch, gain.data()); where = "lcs_chan_gain"; }
+  if (rc == LCS_OK && meas)
+    for (uint32_t c = 0; c < n_ch; c++)
+      for (lcs_cell_meas& m : (*meas)[c]) {
+        const double g2 = (double)gain[c] * gain[c];
+        for (int p = 0; p < 4; p++) { m.rsrp[p] /= g2; m.noise[p] /= g2; }
+        m.rssi /= g2;
+      }
   if (sw) lcs_sweep_destroy(sw);
   if (d_iq) cudaFree(d_iq);
   if (ch) lcs_chan_destroy(ch);
   check(rc, where);
-  detected_cells.assign(n_ch, std::list<Cell>());
-  for (uint32_t c = 0; c < n_ch; c++)
-    for (uint32_t k = 0; k < found[c] && k < max_cells; k++) detected_cells[c].push_back(from_pod(cells[(size_t)c * max_cells + k]));
 }
 
 void wideband_search_ci16(const int16_t* iq, uint32_t n, double fs_in, double fc_in, const std::vector<double>& fc_requested,
-                          const vec& f_search_set, const double& fs_programmed, std::vector<std::list<Cell> >& detected_cells) {
-  wideband_search(iq, -1, n, fs_in, fc_in, fc_requested, f_search_set, fs_programmed, detected_cells);
+                          const vec& f_search_set, const double& fs_programmed, std::vector<std::list<Cell> >& detected_cells,
+                          std::vector<std::vector<lcs_cell_meas> >* meas) {
+  wideband_search(iq, -1, n, fs_in, fc_in, fc_requested, f_search_set, fs_programmed, detected_cells, meas);
 }
 
 void wideband_search_rational(const void* iq, int iq_format, uint32_t n, double fs_in, double fc_in,
                               const std::vector<double>& fc_requested, const vec& f_search_set,
-                              const double& fs_programmed, std::vector<std::list<Cell> >& detected_cells) {
-  wideband_search(iq, iq_format, n, fs_in, fc_in, fc_requested, f_search_set, fs_programmed, detected_cells);
+                              const double& fs_programmed, std::vector<std::list<Cell> >& detected_cells,
+                              std::vector<std::vector<lcs_cell_meas> >* meas) {
+  wideband_search(iq, iq_format, n, fs_in, fc_in, fc_requested, f_search_set, fs_programmed, detected_cells, meas);
 }
 
 void wideband_psd(const std::string& path, int iq_format, size_t es, double fs_in, uint32_t nfft, std::vector<double>& psd,

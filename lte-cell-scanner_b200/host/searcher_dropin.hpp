@@ -20,6 +20,7 @@
 #include "itpp_min.hpp"
 #endif
 #include "../../include/lcs_b200.h"
+#include "../../include/lcs_meas.h"
 
 // --- include/common.h.in ---
 typedef char int8;
@@ -97,13 +98,22 @@ void xcorr_pss_skip_debug_outputs(bool skip);
 void sweep_search_cu8(const std::vector<unsigned char>& iq, uint32_t n_cap, const std::vector<double>& fc_requested,
                       const itpp::vec& f_search_set, const double& fs_programmed, std::vector<std::list<Cell> >& detected_cells);
 // The same sweep fed from one wideband ci16 recording (iq [n][2] at fs_in, centred on fc_in): lcs_chan auto gain, every
-// channel channelized into device memory (153 600 samples each), then lcs_sweep_search_cu8_device.
+// channel channelized into device memory (153 600 samples each), then lcs_sweep_search_cu8_device.  With meas, every
+// found cell is also measured (lcs_meas_cells) on the channelized buffer in place, with rsrp, noise and rssi divided by
+// the channel's gain^2 so that they are in the recording's full scale: meas[c][k] is that of detected_cells[c]'s k-th.
 void wideband_search_ci16(const int16_t* iq, uint32_t n, double fs_in, double fc_in, const std::vector<double>& fc_requested,
-                          const itpp::vec& f_search_set, const double& fs_programmed, std::vector<std::list<Cell> >& detected_cells);
+                          const itpp::vec& f_search_set, const double& fs_programmed, std::vector<std::list<Cell> >& detected_cells,
+                          std::vector<std::vector<lcs_cell_meas> >* meas = nullptr);
 // The same at any rate lcs_chan_create_rational allows, iq [n][2] in iq_format (LCS_IQ_CI16, CS8, CU8 or CF32).
 void wideband_search_rational(const void* iq, int iq_format, uint32_t n, double fs_in, double fc_in,
                               const std::vector<double>& fc_requested, const itpp::vec& f_search_set,
-                              const double& fs_programmed, std::vector<std::list<Cell> >& detected_cells);
+                              const double& fs_programmed, std::vector<std::list<Cell> >& detected_cells,
+                              std::vector<std::vector<lcs_cell_meas> >* meas = nullptr);
+// RSRP / RSRQ / SINR (lcs_meas of liblcs_meas.so, DESIGN.md section 4.9) of every cell of detected_cells[c], found in
+// capture buffer c of iq ([detected_cells.size()][n_cap][2] in iq_format LCS_IQ_CU8, CF32 or C128, host memory), in one
+// call: meas[c][k] is that of detected_cells[c]'s k-th cell.
+void measure_cells(const void* iq, int iq_format, uint32_t n_cap, const std::vector<std::list<Cell> >& detected_cells,
+                   const double& fs_programmed, std::vector<std::vector<lcs_cell_meas> >& meas);
    // skip the 136 MB `xc`/`sp`/`xc_incoherent` debug outputs (CLI does)
 // Welch power spectral density (lcs_psd of liblcs_psd.so, DESIGN.md section 4.8) of the whole recording in `path` ([n][2] in iq_format,
 // sample_bytes per sample, at fs_in, read in blocks): psd [nfft] in fftshift order, full-scale^2 per Hz, over n_segments segments.

@@ -1,5 +1,6 @@
-"""ctypes binding of liblcs_b200.so - the C ABI declared in include/lcs_b200.h - and of liblcs_psd.so, the Welch
-spectrum of include/lcs_psd.h built on top of it.
+"""ctypes binding of liblcs_b200.so - the C ABI declared in include/lcs_b200.h - and of the two modules built on top of
+it: liblcs_psd.so, the Welch spectrum of include/lcs_psd.h, and liblcs_meas.so, the per-cell RSRP / RSRQ / SINR of
+include/lcs_meas.h.
 
 This module is plumbing for tests/, bench.py and __graft_entry__.py: every call goes through the
 same `extern "C"` entry points a C++/IT++ host would bind (INTEGRATION.md).  lib() gives every
@@ -19,6 +20,8 @@ LIB_PATH = os.environ.get("LCS_B200_LIB") or os.path.join(HERE, "liblcs_b200.so"
 HEADER = os.path.join(HERE, "..", "include", "lcs_b200.h")
 PSD_LIB_PATH = os.environ.get("LCS_PSD_LIB") or os.path.join(HERE, "liblcs_psd.so")
 PSD_HEADER = os.path.join(HERE, "..", "include", "lcs_psd.h")
+MEAS_LIB_PATH = os.environ.get("LCS_MEAS_LIB") or os.path.join(HERE, "liblcs_meas.so")
+MEAS_HEADER = os.path.join(HERE, "..", "include", "lcs_meas.h")
 
 IQ_CF32, IQ_CU8, IQ_C128, IQ_CI16, IQ_CS8 = 0, 1, 2, 3, 4
 KERNEL_AUTO, KERNEL_FP32, KERNEL_TC = 0, 1, 2
@@ -119,6 +122,12 @@ def psd_lib():
     """liblcs_psd.so (include/lcs_psd.h); it takes the contexts of lib()."""
     lib()
     return _bind(PSD_LIB_PATH, PSD_HEADER)
+
+
+def meas_lib():
+    """liblcs_meas.so (include/lcs_meas.h); it takes the contexts of lib()."""
+    lib()
+    return _bind(MEAS_LIB_PATH, MEAS_HEADER)
 
 
 def _p(a):
@@ -747,3 +756,64 @@ class Spectrum(_Handle):
         n = C.c_uint64(0)
         _chk(psd_lib().lcs_psd_read(self._h, _p(psd), C.byref(n)), self.ctx._h)
         return self.freqs, psd, n.value
+
+
+# lcs_cell_meas as a numpy record
+CELL_MEAS = np.dtype([("rsrp", np.float64, 4), ("noise", np.float64, 4), ("sinr", np.float64, 4), ("rssi", np.float64),
+                      ("rsrq", np.float64), ("n_pairs", np.uint32, 4)], align=True)
+MEAS_FORMATS = {"cu8": (IQ_CU8, np.uint8), "cf32": (IQ_CF32, np.float32), "c128": (IQ_C128, np.float64)}
+
+
+class CellMeasure(_Handle):
+    """lcs_meas: RSRP, RSRQ and SINR of found cells from the CRS of their central six resource blocks (DESIGN.md section
+    4.9), every cell of a call in one grid launch and one measurement launch."""
+    _destroy = "lcs_meas_destroy"
+    _timing_read = "lcs_meas_timing_read"
+    _lib = staticmethod(meas_lib)
+
+    def __init__(self, ctx):
+        self.ctx = ctx
+        self._h = C.c_void_p()
+        _chk(meas_lib().lcs_meas_create(ctx._h, C.byref(self._h)), ctx._h)
+
+    def measure(self, iq, cells, ch=None, fs_programmed=1.92e6, fmt="cu8"):
+        """Measure `cells` (Cells, or lists of them) found in the capture buffers iq [n_ch][n_cap][2] (or [n_cap][2] for
+        one channel) of format fmt: cu8 (uint8), cf32 (float32) or c128 (float64); complex64 / complex128 [n_ch][n_cap]
+        are accepted for cf32 / c128.  iq may be a contiguous CUDA tensor (read in place; its stream is synchronised
+        first).  ch[i] is the channel of cell i (default 0).  Returns a CELL_MEAS record array, one row per cell."""
+        iq_format, dtype = MEAS_FORMATS[fmt]
+        cells = list(cells)
+        n = len(cells)
+        arr = (Cell * max(n, 1))()
+        for i, c in enumerate(cells):                   # any struct of lcs_cell's layout (the oracle's Cell too)
+            C.memmove(C.addressof(arr) + i * C.sizeof(Cell), C.byref(c), C.sizeof(Cell))
+        chv = np.ascontiguousarray(np.zeros(n) if ch is None else ch, np.uint32)
+        if chv.shape != (n,):
+            raise ValueError("ch must hold one channel per cell")
+        if hasattr(iq, "is_cuda"):
+            if not (iq.is_cuda and iq.is_contiguous()):
+                raise ValueError("measure: expected a contiguous CUDA tensor")
+            shape = tuple(iq.shape)
+            if iq.is_complex():
+                shape = shape + (2,)
+            import torch
+            torch.cuda.current_stream(iq.device).synchronize()
+            ptr, on_device = iq.data_ptr(), 1
+        else:
+            iq = np.asarray(iq)
+            if iq.dtype in (np.complex64, np.complex128):
+                iq = iq.view(iq.real.dtype).reshape(iq.shape + (2,))
+            if iq.dtype != dtype:
+                raise ValueError("expected %s samples: %s [n_ch][n_cap][2]" % (fmt, np.dtype(dtype).name))
+            iq = np.ascontiguousarray(iq)
+            shape, ptr, on_device = iq.shape, iq.ctypes.data, 0
+        if len(shape) == 2:
+            shape = (1,) + shape
+        if len(shape) != 3 or shape[2] != 2:
+            raise ValueError("expected capture buffers [n_ch][n_cap][2]")
+        out = np.zeros(n, CELL_MEAS)
+        self._iq = iq                                   # kept alive until the call has returned
+        _chk(meas_lib().lcs_meas_cells(self._h, ptr, iq_format, on_device, shape[0], shape[1], arr, _p(chv), n,
+                                       fs_programmed, _p(out)), self.ctx._h)
+        self._iq = None
+        return out

@@ -1,0 +1,99 @@
+"""Cost of the per-cell RSRP / RSRQ / SINR measurement (lcs_meas_cells, DESIGN.md section 4.9), next to the search's.
+
+A few synthetic 80 ms cu8 capture buffers (each with one or two cells) are tiled to --channels channels in device memory.
+The batched search (lcs_sweep_search_cu8_device) finds the cells of every channel; then all of them are measured, read in
+place, in one call, --reps times after a warm-up call.  One JSON line reports:
+  - the measurement's device time per cell (CUDA events around its two launches, lcs_meas_timing_read) and its host clock
+    per call, beside the search's host clock per found cell (the search's call ends in a synchronise);
+  - the bytes the two kernels need per cell (capture samples read, the 854 x 72 grid written, and the grid's CRS and
+    RSSI resource elements read back), the achieved byte rate and the lower bound at 3.35 TB/s (H100 SXM data sheet);
+  - the card name, power limit and SM clocks, read in the same run.
+
+Usage: python tools/meas_bench.py [--channels 64] [--reps 20]
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+
+import numpy as np
+
+ROOT = os.path.abspath(os.path.join(os.path.dirname(__file__), ".."))
+sys.path.insert(0, os.path.join(ROOT, "lte-cell-scanner_b200"))
+sys.path.insert(0, os.path.join(ROOT, "track_oracle"))
+
+import lcs_b200 as L  # noqa: E402
+import lte_dl_synth as S  # noqa: E402
+
+HBM_BPS = 3.35e12
+FC = 739e6
+
+
+def cell(nid, ports, cp, t0, scale=1.0):
+    g = [1.0, 0.8 * np.exp(0.7j), 0.9 * np.exp(-1.1j), 0.7 * np.exp(2.2j)]
+    return dict(n_id_cell=nid, n_ports=ports, cp_type=cp, n_rb_dl=50, phich_duration=1, phich_resource=2, t0=t0, sfn0=7,
+                gains=[scale * v for v in g])
+
+
+BUFFERS = [[cell(137, 2, 1, 1234.0)], [cell(52, 4, 2, 7000.0)], [cell(277, 2, 1, 3000.0), cell(271, 1, 1, 15000.0, 0.6)],
+           [cell(100, 1, 1, 500.0)]]
+
+
+def cell_bytes(c):
+    """Bytes the two kernels move for one cell: the samples of its 122-slot grid (cu8), the grid written and read back
+    at its CRS pairs and RSSI symbols (complex double)."""
+    n_symb = 7 if c.cp_type == 1 else 6
+    n_ofdm = 122 * n_symb
+    pairs = sum([2880, 2880, 1440, 1440][:c.n_ports])
+    return n_ofdm * 128 * 2 + n_ofdm * 72 * 16 + 2 * pairs * 16 + 244 * 72 * 16
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--channels", type=int, default=64)
+    ap.add_argument("--reps", type=int, default=20)
+    a = ap.parse_args()
+    import torch
+    bufs = [S.synth_cu8(153600, cs, fc=FC, snr_db=12.0, seed=i) for i, cs in enumerate(BUFFERS)]
+    iq = np.stack([bufs[c % len(bufs)] for c in range(a.channels)])
+    ctx = L.Context(0)
+    d_iq = torch.from_numpy(iq).cuda()
+    fcs = np.full(a.channels, FC)
+    f_set = L.f_search_set(FC, 20.0)
+    sw = L.Sweep(ctx)
+    sw.search_cu8_device(d_iq, fcs, f_set)                       # warm-up
+    t = time.perf_counter()
+    found = sw.search_cu8_device(d_iq, fcs, f_set)
+    search_s = time.perf_counter() - t
+    sw.close()
+    cells = [c for row in found for c in row]
+    ch = [i for i, row in enumerate(found) for _ in row]
+    m = L.CellMeasure(ctx)
+    m.measure(d_iq, cells, ch)                                    # warm-up
+    m.timing_read()
+    wall = []
+    for _ in range(a.reps):
+        t = time.perf_counter()
+        m.measure(d_iq, cells, ch)
+        wall.append(time.perf_counter() - t)
+    ms, launches = m.timing_read()
+    m.close()
+    n = len(cells)
+    dev_s = ms / 1e3 / a.reps
+    bytes_ = sum(cell_bytes(c) for c in cells)
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"],
+                       capture_output=True, text=True).stdout.strip().splitlines()
+    print(json.dumps({
+        "channels": a.channels, "cells": n, "reps": a.reps, "launches": launches,
+        "meas_device_us_per_cell": 1e6 * dev_s / n, "meas_host_us_per_cell": 1e6 * float(np.median(wall)) / n,
+        "search_host_us_per_cell": 1e6 * search_s / n, "search_host_ms": 1e3 * search_s,
+        "meas_bytes_per_cell": bytes_ / n, "meas_gbytes_per_s": bytes_ / dev_s / 1e9,
+        "bound_hbm_us_per_cell": 1e6 * bytes_ / HBM_BPS / n, "gpu": q[0] if q else "unknown",
+    }), flush=True)
+    ctx.close()
+
+
+if __name__ == "__main__":
+    main()
