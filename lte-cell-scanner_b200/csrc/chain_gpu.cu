@@ -7,6 +7,7 @@
 
 #include "chain_gpu.hpp"
 #include "fft128.cuh"
+#include "iq_format.cuh"
 
 namespace lcs {
 
@@ -216,13 +217,6 @@ __global__ void __launch_bounds__(64) tfg_kernel(const void* __restrict__ cap, c
   }
 }
 
-#define DISPATCH(fmt, CALL)                               \
-  do {                                                    \
-    if ((fmt) == LCS_IQ_CU8) { CALL(LCS_IQ_CU8); }        \
-    else if ((fmt) == LCS_IQ_CF32) { CALL(LCS_IQ_CF32); } \
-    else { CALL(LCS_IQ_C128); }                           \
-  } while (0)
-
 // =============================================================================================
 // Host drivers (device-resident capture buffer)
 // =============================================================================================
@@ -294,9 +288,10 @@ static lcs_status run_psss(lcs_ctx* ctx, ChainScratch& cs, const void* d_cap, in
   std::memcpy(hk, kseg.data(), n * 8);
   LCS_CUDA(ctx, cudaMemcpyAsync(cs.d_starts.p, hs, n * 4, cudaMemcpyHostToDevice, st));
   LCS_CUDA(ctx, cudaMemcpyAsync(cs.d_kseg.p, hk, n * 8, cudaMemcpyHostToDevice, st));
-#define CALL(F) psss_kernel<F><<<(unsigned)n, 64, 0, st>>>(d_cap, cs.d_starts.p, cs.d_kseg.p, cs.d_psss.p)
-  DISPATCH(fmt, CALL);
-#undef CALL
+  if (SearchFormats::dispatch(fmt, [&](auto FMT) {
+        psss_kernel<FMT><<<(unsigned)n, 64, 0, st>>>(d_cap, cs.d_starts.p, cs.d_kseg.p, cs.d_psss.p);
+      }) != LCS_OK)
+    return fail(ctx, LCS_ERR_ARG, "psss: bad iq_format");
   ctx->launches++;
   LCS_CUDA(ctx, cudaGetLastError());
   return LCS_OK;
@@ -537,11 +532,11 @@ lcs_status tfg_geometry(const lcs_cell& cell, double fc_req, double fc_prog, dou
   return LCS_OK;
 }
 
-void launch_tfg(const void* d_cap, int fmt, const uint64_t* d_base, const int* d_pos, const double* d_late,
-                const double* d_k, const int* d_nofdm, uint32_t n_cells, double2* d_tfg, cudaStream_t st) {
-#define CALL(F) tfg_kernel<F><<<dim3(TFG_MAX, n_cells), 64, 0, st>>>(d_cap, d_base, d_pos, d_late, d_k, d_nofdm, d_tfg)
-  DISPATCH(fmt, CALL);
-#undef CALL
+lcs_status launch_tfg(const void* d_cap, int fmt, const uint64_t* d_base, const int* d_pos, const double* d_late,
+                      const double* d_k, const int* d_nofdm, uint32_t n_cells, double2* d_tfg, cudaStream_t st) {
+  return SearchFormats::dispatch(fmt, [&](auto FMT) {
+    tfg_kernel<FMT><<<dim3(TFG_MAX, n_cells), 64, 0, st>>>(d_cap, d_base, d_pos, d_late, d_k, d_nofdm, d_tfg);
+  });
 }
 
 // extract_tfg (searcher.cpp:857-935) for several cells: one launch of (854 symbols x cells) FFT blocks, one copy back.
@@ -586,7 +581,8 @@ lcs_status dev_extract_tfg_batch(lcs_ctx* ctx, ChainScratch& cs, const void* d_c
   LCS_CUDA(ctx, cudaMemcpyAsync(cs.d_late.p, h_late, L * TFG_MAX * 8, cudaMemcpyHostToDevice, st));
   LCS_CUDA(ctx, cudaMemcpyAsync(cs.d_kseg.p, h_k, L * 8, cudaMemcpyHostToDevice, st));
   LCS_CUDA(ctx, cudaMemcpyAsync(cs.d_nofdm.p, h_n, L * 4, cudaMemcpyHostToDevice, st));
-  launch_tfg(d_cap, fmt, nullptr, cs.d_starts.p, cs.d_late.p, cs.d_kseg.p, cs.d_nofdm.p, (uint32_t)L, cs.d_tfg.p, st);
+  if (launch_tfg(d_cap, fmt, nullptr, cs.d_starts.p, cs.d_late.p, cs.d_kseg.p, cs.d_nofdm.p, (uint32_t)L, cs.d_tfg.p, st) != LCS_OK)
+    return fail(ctx, LCS_ERR_ARG, "extract_tfg: bad iq_format");
   ctx->launches++;
   LCS_CUDA(ctx, cudaGetLastError());
   LCS_CUDA(ctx, cudaMemcpyAsync(cs.h_down.p, cs.d_tfg.p, L * TFG_MAX * 72 * 16, cudaMemcpyDeviceToHost, st));

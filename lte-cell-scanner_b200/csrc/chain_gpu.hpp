@@ -51,9 +51,10 @@ lcs_status tfg_geometry(const lcs_cell& cell, double fc_req, double fc_prog, dou
                         double* late, double* ts, double* kcell, int* n_ofdm, const char** why);
 // One tfg_kernel launch over n_cells cells (asynchronous on st): d_pos / d_late [cell][TFG_MAX] from tfg_geometry, d_k and
 // d_nofdm [cell]; the grids land in d_tfg [cell][TFG_MAX][72] (1/sqrt(128) DFT scaling).  d_base [cell] (NULL: all 0) is
-// the sample index in d_cap at which the cell's capture buffer starts.
-void launch_tfg(const void* d_cap, int fmt, const uint64_t* d_base, const int* d_pos, const double* d_late,
-                const double* d_k, const int* d_nofdm, uint32_t n_cells, double2* d_tfg, cudaStream_t st);
+// the sample index in d_cap at which the cell's capture buffer starts.  A format other than cu8, cf32 or c128 launches
+// nothing and returns LCS_ERR_ARG.
+lcs_status launch_tfg(const void* d_cap, int fmt, const uint64_t* d_base, const int* d_pos, const double* d_late,
+                      const double* d_k, const int* d_nofdm, uint32_t n_cells, double2* d_tfg, cudaStream_t st);
 lcs_status dev_extract_tfg_batch(lcs_ctx* ctx, ChainScratch& cs, const void* d_cap, int fmt, uint32_t n_cap,
                                  const std::vector<lcs_cell>& cells, double fc_req, double fc_prog, double fs_prog,
                                  std::vector<std::vector<cd>>& tfg_rowmajor, std::vector<std::vector<double>>& ts,

@@ -22,7 +22,7 @@
 #include <type_traits>
 #include <vector>
 
-#include "iq_load.cuh"
+#include "iq_format.cuh"
 #include "lcs_ctx.hpp"
 
 namespace lcs {
@@ -555,22 +555,15 @@ uint64_t outputs_after(const lcs_chan* c, uint64_t n) {
 }
 // the carry of a fresh stream: the inputs of output 0 before sample 0, of value 0 in the channelizer's format (cu8 127)
 SampleCarry fresh_carry(const lcs_chan* c) {
-  const size_t esz = stream_sample_bytes(c->fmt);
-  return SampleCarry{esz, std::vector<unsigned char>((size_t)-first_input(c, 0) * esz, c->fmt == LCS_IQ_CU8 ? 127 : 0)};
+  const size_t esz = sample_bytes(c->fmt);
+  return SampleCarry{esz, std::vector<unsigned char>((size_t)-first_input(c, 0) * esz, zero_sample_byte(c->fmt))};
 }
 int outputs_per_tile(const lcs_chan* c) { return 32 * c->RM * c->up; }
 
-template <int FMT>
-void launch_rchan(bool power, dim3 grid, size_t smem, cudaStream_t st, const RParams& P) {
-  if (power)
-    rchan_kernel<FMT, true><<<grid, THREADS, smem, st>>>(P);
-  else
-    rchan_kernel<FMT, false><<<grid, THREADS, smem, st>>>(P);
-}
-
 // One launch of the channelizer's kernel: `shared` assigns the fields both kernels read, the rest is the kernel's own.
+// LCS_ERR_ARG, and no launch, for a format the channelizer does not take.
 template <class F>
-void launch(const lcs_chan* c, bool power, dim3 grid, size_t smem, cudaStream_t st, F shared) {
+lcs_status launch(const lcs_chan* c, bool power, dim3 grid, size_t smem, cudaStream_t st, F shared) {
   if (decimating_kernel(c)) {
     Params P;
     shared(P);
@@ -580,7 +573,7 @@ void launch(const lcs_chan* c, bool power, dim3 grid, size_t smem, cudaStream_t 
       chan_kernel<true><<<grid, THREADS, smem, st>>>(P);
     else
       chan_kernel<false><<<grid, THREADS, smem, st>>>(P);
-    return;
+    return LCS_OK;
   }
   RParams P;
   shared(P);
@@ -588,19 +581,12 @@ void launch(const lcs_chan* c, bool power, dim3 grid, size_t smem, cudaStream_t 
   P.J = c->J;
   P.RM = c->RM;
   P.q0 = P.n0 * c->down + c->M;
-  switch (c->fmt) {
-    case LCS_IQ_CI16: launch_rchan<LCS_IQ_CI16>(power, grid, smem, st, P); break;
-    case LCS_IQ_CS8: launch_rchan<LCS_IQ_CS8>(power, grid, smem, st, P); break;
-    case LCS_IQ_CU8: launch_rchan<LCS_IQ_CU8>(power, grid, smem, st, P); break;
-    default: launch_rchan<LCS_IQ_CF32>(power, grid, smem, st, P); break;
-  }
-}
-
-template <int FMT>
-cudaError_t set_rchan_smem() {
-  cudaError_t e = cudaFuncSetAttribute(rchan_kernel<FMT, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, RSMEM_CAP);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(rchan_kernel<FMT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, RSMEM_CAP);
-  return e;
+  return StreamFormats::dispatch(c->fmt, [&](auto FMT) {
+    if (power)
+      rchan_kernel<FMT, true><<<grid, THREADS, smem, st>>>(P);
+    else
+      rchan_kernel<FMT, false><<<grid, THREADS, smem, st>>>(P);
+  });
 }
 
 // The per-channel complex taps (float and double) and epilogue phase step in the format of the channelizer's kernel.
@@ -682,7 +668,7 @@ lcs_status run(lcs_chan* c, const SampleCarry& a, const unsigned char* b, size_t
     };
     const dim3 grid((ne + T - 1) / T, (c->n_ch + CH_CTA - 1) / CH_CTA);
     LCS_CUDA(ctx, c->clock.begin(st));
-    launch(c, power, grid, smem, st, shared);
+    if (launch(c, power, grid, smem, st, shared) != LCS_OK) return fail(ctx, LCS_ERR_ARG, "lcs_chan: bad iq_format");
     ctx->launches++;
     LCS_CUDA(ctx, cudaGetLastError());
     LCS_CUDA(ctx, c->clock.end(st, 1));
@@ -760,10 +746,11 @@ lcs_status create(lcs_ctx* ctx, const std::string& who, long long fs, int up, in
   if (e == cudaSuccess) e = cudaMemcpy(c->d_gain.p, c->gain.data(), n_ch * 4, cudaMemcpyHostToDevice);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(chan_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_CAP);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(chan_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_CAP);
-  if (e == cudaSuccess) e = set_rchan_smem<LCS_IQ_CI16>();
-  if (e == cudaSuccess) e = set_rchan_smem<LCS_IQ_CS8>();
-  if (e == cudaSuccess) e = set_rchan_smem<LCS_IQ_CU8>();
-  if (e == cudaSuccess) e = set_rchan_smem<LCS_IQ_CF32>();
+  if (e == cudaSuccess)
+    StreamFormats::dispatch(fmt, [&](auto FMT) {
+      e = cudaFuncSetAttribute(rchan_kernel<FMT, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, RSMEM_CAP);
+      if (e == cudaSuccess) e = cudaFuncSetAttribute(rchan_kernel<FMT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, RSMEM_CAP);
+    });
   if (e != cudaSuccess) {
     delete c;
     return fail(ctx, LCS_ERR_CUDA, who + ": " + cudaGetErrorString(e));
@@ -825,7 +812,7 @@ lcs_status lcs_chan_create_rational(lcs_ctx* ctx, double fs_in, int iq_format, d
   if (!rational_rate(fs_in, &fs, &up, &down))
     return fail(ctx, LCS_ERR_ARG, "lcs_chan_create_rational: fs_in must be an integer number of Hz in (1.92, 122.88] MHz "
                                   "with fs_in / 1.92 MHz = down / up, up <= 128, down <= 640");
-  if (!stream_sample_bytes(iq_format))
+  if (!StreamFormats::has(iq_format))
     return fail(ctx, LCS_ERR_ARG, "lcs_chan_create_rational: iq_format must be LCS_IQ_CI16, CS8, CU8 or CF32");
   return create(ctx, "lcs_chan_create_rational", fs, up, down, iq_format, fc_in, n_ch, fc_ch, gain, out);
 }

@@ -1,29 +1,9 @@
-// fft128.cuh - FP64 device helpers shared by the companion kernels (chain_gpu.cu, track.cu): sample loads as
-// complex<double>, complex multiply, and the shared-memory 128-point FFT.
+// fft128.cuh - FP64 device helpers shared by the companion kernels (chain_gpu.cu, track.cu): complex multiply and the
+// shared-memory 128-point FFT.
 #pragma once
 #include <cuda_runtime.h>
 
-#include "../../include/lcs_b200.h"
-
 namespace lcs {
-
-// ---- sample loads as complex<double> ----
-template <int FMT>
-__device__ __forceinline__ double2 load_c(const void* __restrict__ base, size_t i);
-template <>
-__device__ __forceinline__ double2 load_c<LCS_IQ_C128>(const void* __restrict__ base, size_t i) {
-  return __ldg(reinterpret_cast<const double2*>(base) + i);
-}
-template <>
-__device__ __forceinline__ double2 load_c<LCS_IQ_CF32>(const void* __restrict__ base, size_t i) {
-  float2 v = __ldg(reinterpret_cast<const float2*>(base) + i);
-  return make_double2((double)v.x, (double)v.y);
-}
-template <>
-__device__ __forceinline__ double2 load_c<LCS_IQ_CU8>(const void* __restrict__ base, size_t i) {
-  uchar2 v = __ldg(reinterpret_cast<const uchar2*>(base) + i);
-  return make_double2(((int)v.x - 127) / 128.0, ((int)v.y - 127) / 128.0);
-}
 
 __device__ __forceinline__ double2 cmul(double2 a, double2 b) { return make_double2(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x); }
 

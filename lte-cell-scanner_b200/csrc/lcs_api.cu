@@ -7,6 +7,7 @@
 #include <cstring>
 #include <mutex>
 
+#include "iq_format.cuh"
 #include "lcs_ctx.hpp"
 
 namespace lcs {
@@ -219,8 +220,8 @@ lcs_status lcs_xcorr_pss_batch_host(lcs_xcorr_plan* p, const void* h_iq, int iq_
   if (!h_iq || !h_pow || !h_frq || !h_spi) return fail(ctx, LCS_ERR_ARG, "xcorr_pss_batch_host: null pointer");
   if (batch == 0) return LCS_OK;
   const XcorrGeom& g = p->ps.geom;
-  const size_t samp_bytes = iq_sample_bytes(iq_format);
-  if (!samp_bytes) return fail(ctx, LCS_ERR_ARG, "xcorr_pss_batch_host: bad iq_format");
+  if (!SearchFormats::has(iq_format)) return fail(ctx, LCS_ERR_ARG, "xcorr_pss_batch_host: bad iq_format");
+  const size_t samp_bytes = sample_bytes(iq_format);
   LCS_CUDA(ctx, cudaSetDevice(ctx->device));
   // chunk: large enough that the persistent correlator CTAs get many tiles each (64 buffers x 38 tiles = 16.4 tiles per
   // CTA, 3 % rounding loss), small enough that the copies of neighbouring chunks overlap the kernels

@@ -13,15 +13,6 @@ namespace lcs {
 
 typedef std::complex<double> cd;
 
-// Bytes per complex sample of an LCS_IQ_* format; 0 for anything else.
-inline size_t iq_sample_bytes(int iq_format) {
-  return iq_format == LCS_IQ_CU8 ? 2 : iq_format == LCS_IQ_CF32 ? 8 : iq_format == LCS_IQ_C128 ? 16 : 0;
-}
-// Bytes per complex sample of a format the channelizer and the spectrum take (ci16, cs8, cu8, cf32); 0 for anything else.
-inline size_t stream_sample_bytes(int fmt) {
-  return fmt == LCS_IQ_CI16 ? 4 : fmt == LCS_IQ_CS8 || fmt == LCS_IQ_CU8 ? 2 : fmt == LCS_IQ_CF32 ? 8 : 0;
-}
-
 // ---- geometry of the fused FP32 correlator (xcorr_fp32.cu) ----
 constexpr int XC_R = 7;                 // lags per lane (7*8 B stride is LDS.64 bank-conflict free)
 constexpr int XC_TI = 32 * XC_R;        // 224 fold positions per block
@@ -47,7 +38,8 @@ struct PlanView {
   const uint32_t* d_buf_plan; // [batch] plan of each capture buffer (NULL: every buffer uses plan 0)
 };
 
-// Launchers (all asynchronous on `st`); return the number of kernel launches they issued.
+// Launchers (all asynchronous on `st`); return the number of kernel launches they issued.  The caller checks iq_format
+// first (SearchFormats::has): for any other format they launch nothing and return 0.
 int launch_xcorr_fold_fp32(const XcorrGeom& g, const PlanView& pv, const void* d_iq, int iq_format, uint32_t batch,
                            const float4* d_w01, const float2* d_w2, const int* d_soff, const int* d_smin,
                            float* d_single_planar, cudaStream_t st);

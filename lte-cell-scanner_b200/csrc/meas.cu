@@ -16,6 +16,7 @@
 
 #include "../../include/lcs_meas.h"
 #include "chain_gpu.hpp"
+#include "iq_format.cuh"
 
 namespace lcs {
 namespace meas {
@@ -146,8 +147,8 @@ lcs_status lcs_meas_cells(lcs_meas* m, const void* iq, int iq_format, int on_dev
                           lcs_cell_meas* out) {
   if (!m) return LCS_ERR_ARG;
   if (!iq || (n_cells && (!cells || !ch || !out))) return mfail(m, "null pointer");
-  const size_t esz = iq_sample_bytes(iq_format);
-  if (!esz) return mfail(m, "iq_format must be LCS_IQ_CU8, CF32 or C128");
+  if (!SearchFormats::has(iq_format)) return mfail(m, "iq_format must be LCS_IQ_CU8, CF32 or C128");
+  const size_t esz = sample_bytes(iq_format);
   if (on_device && ((uintptr_t)iq & 15)) return mfail(m, "device iq must be 16-byte aligned");
   if (!n_ch || !n_cap || n_cap > 0x7fffffffu) return mfail(m, "n_ch and n_cap must be positive, n_cap < 2^31");
   if (!(std::isfinite(fs_programmed) && fs_programmed > 0)) return mfail(m, "fs_programmed must be finite and positive");
@@ -217,7 +218,8 @@ lcs_status lcs_meas_cells(lcs_meas* m, const void* iq, int iq_format, int on_dev
   LCS_CUDA(ctx, cudaMemcpyAsync(m->d_shift.p, shift_tab.data(), shift_tab.size(), cudaMemcpyHostToDevice, st));
   LCS_CUDA(ctx, cudaMemcpyAsync(m->d_par.p, par.data(), L * sizeof(int4), cudaMemcpyHostToDevice, st));
   LCS_CUDA(ctx, m->clock.begin(st));
-  launch_tfg(d_iq, iq_format, m->d_base.p, m->d_pos.p, m->d_late.p, m->d_k.p, m->d_nofdm.p, n_cells, m->d_tfg.p, st);
+  if (launch_tfg(d_iq, iq_format, m->d_base.p, m->d_pos.p, m->d_late.p, m->d_k.p, m->d_nofdm.p, n_cells, m->d_tfg.p, st) != LCS_OK)
+    return mfail(m, "no grid kernel for this iq_format");
   meas::meas_kernel<<<n_cells, meas::THREADS, 0, st>>>(m->d_tfg.p, m->d_rs.p, m->d_shift.p, m->d_par.p, m->d_out.p);
   ctx->launches += 2;
   LCS_CUDA(ctx, cudaGetLastError());

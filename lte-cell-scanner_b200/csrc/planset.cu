@@ -10,6 +10,7 @@
 #include <cmath>
 #include <cstring>
 
+#include "iq_format.cuh"
 #include "lcs_ctx.hpp"
 
 namespace lcs {
@@ -297,11 +298,10 @@ lcs_status planset_run(PlanSet& ps, int kernel, const void* d_iq, int iq_format,
   lcs_ctx* ctx = ps.ctx;
   if (!d_iq || !d_single || !d_pow || !d_frq || !d_spi) return fail(ctx, LCS_ERR_ARG, "xcorr_pss_device: null pointer");
   if (batch == 0) return fail(ctx, LCS_ERR_ARG, "xcorr_pss_device: empty batch");
-  if (iq_format != LCS_IQ_CF32 && iq_format != LCS_IQ_CU8 && iq_format != LCS_IQ_C128)
-    return fail(ctx, LCS_ERR_ARG, "xcorr_pss_device: bad iq_format");
+  if (!SearchFormats::has(iq_format)) return fail(ctx, LCS_ERR_ARG, "xcorr_pss_device: bad iq_format");
   // every kernel loads a whole sample at a time (uchar2 / float2 / double2); the epilogue reads `single` as float4 and
   // writes incoherent / pow / frq as float4 / double2 / int4; sp_fold_kernel stores single doubles
-  if ((uintptr_t)d_iq % iq_sample_bytes(iq_format) != 0)
+  if ((uintptr_t)d_iq % sample_bytes(iq_format) != 0)
     return fail(ctx, LCS_ERR_ARG, "xcorr_pss_device: IQ pointer not aligned to its sample size");
   if ((((uintptr_t)d_single | (uintptr_t)d_pow | (uintptr_t)d_frq | (uintptr_t)d_inc) & 15) != 0)
     return fail(ctx, LCS_ERR_ARG, "xcorr_pss_device: single, pow, frq and incoherent need 16-byte aligned pointers");

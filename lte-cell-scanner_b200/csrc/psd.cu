@@ -1,7 +1,7 @@
 // psd.cu - Welch power spectral density of a wideband recording (DESIGN.md section 4.8; contract in include/lcs_psd.h).
 // Built into liblcs_psd.so, which uses the lcs_ctx of liblcs_b200.so.
 //
-// Every segment (N samples, hop N/2) is staged from the raw recording with the format conversion of iq_load.cuh, windowed
+// Every segment (N samples, hop N/2) is staged from the raw recording with the format conversion of iq_format.cuh, windowed
 // by the periodic Hann window and transformed by an FP32 FFT in shared memory; |X|^2 per bin goes to a scratch row per
 // segment, and one thread per bin adds the rows of a launch to the FP64 accumulator in segment order.
 //
@@ -17,7 +17,7 @@
 #include <vector>
 
 #include "../../include/lcs_psd.h"
-#include "iq_load.cuh"
+#include "iq_format.cuh"
 #include "lcs_ctx.hpp"
 
 namespace lcs {
@@ -211,14 +211,16 @@ namespace {
 
 lcs_status pfail(const lcs_psd* p, const char* msg) { return fail(p ? p->ctx : nullptr, LCS_ERR_ARG, msg); }
 
-template <int FMT>
-void launch_fft(const lcs_psd* p, const Params& P, cudaStream_t st) {
-  if (!p->lg1) {
-    psd_fft_kernel<FMT><<<(P.n_seg + (TILE >> p->lg) - 1) / (TILE >> p->lg), THREADS, 0, st>>>(P);
-  } else {
-    psd_col_kernel<FMT><<<dim3((1u << p->lg2) >> (LG_TILE - p->lg1), P.n_seg), THREADS, 0, st>>>(P);
-    psd_row_kernel<<<dim3((1u << p->lg1) >> (LG_TILE - p->lg2), P.n_seg), THREADS, 0, st>>>(P);
-  }
+// The transform kernels of a launch chunk; LCS_ERR_ARG, and no launch, for a format the spectrum does not take.
+lcs_status launch_fft(const lcs_psd* p, const Params& P, cudaStream_t st) {
+  return StreamFormats::dispatch(p->fmt, [&](auto FMT) {
+    if (!p->lg1) {
+      psd_fft_kernel<FMT><<<(P.n_seg + (TILE >> p->lg) - 1) / (TILE >> p->lg), THREADS, 0, st>>>(P);
+    } else {
+      psd_col_kernel<FMT><<<dim3((1u << p->lg2) >> (LG_TILE - p->lg1), P.n_seg), THREADS, 0, st>>>(P);
+      psd_row_kernel<<<dim3((1u << p->lg1) >> (LG_TILE - p->lg2), P.n_seg), THREADS, 0, st>>>(P);
+    }
+  });
 }
 
 // Segments [0, n) of the virtual input carry ++ b, whose sample 0 is the first sample of segment 0.
@@ -240,12 +242,7 @@ lcs_status run(lcs_psd* p, const unsigned char* b, uint64_t n) {
     P.y = p->d_y.p;
     P.pw = p->d_pw.p;
     LCS_CUDA(ctx, p->clock.begin(st));
-    switch (p->fmt) {
-      case LCS_IQ_CI16: launch_fft<LCS_IQ_CI16>(p, P, st); break;
-      case LCS_IQ_CS8: launch_fft<LCS_IQ_CS8>(p, P, st); break;
-      case LCS_IQ_CU8: launch_fft<LCS_IQ_CU8>(p, P, st); break;
-      default: launch_fft<LCS_IQ_CF32>(p, P, st); break;
-    }
+    if (launch_fft(p, P, st) != LCS_OK) return fail(ctx, LCS_ERR_ARG, "lcs_psd: bad iq_format");
     psd_accum_kernel<<<(p->N + ACC_THREADS - 1) / ACC_THREADS, ACC_THREADS, 0, st>>>(p->d_pw.p, (int)ns, (int)p->N, p->d_acc.p);
     const int launches = p->lg1 ? 3 : 2;
     ctx->launches += launches;
@@ -266,7 +263,7 @@ lcs_status lcs_psd_create(lcs_ctx* ctx, double fs_in, int iq_format, uint32_t nf
   const double r = std::round(fs_in);
   if (!std::isfinite(fs_in) || std::fabs(fs_in - r) > 1e-6 || !(r > 0) || r > 250e6)
     return fail(ctx, LCS_ERR_ARG, "lcs_psd_create: fs_in must be an integer number of Hz in (0, 250] MHz");
-  if (!stream_sample_bytes(iq_format))
+  if (!StreamFormats::has(iq_format))
     return fail(ctx, LCS_ERR_ARG, "lcs_psd_create: iq_format must be LCS_IQ_CI16, CS8, CU8 or CF32");
   int lg = 0;
   while (lg <= LG_MAX && (1u << lg) < nfft) lg++;
@@ -276,7 +273,7 @@ lcs_status lcs_psd_create(lcs_ctx* ctx, double fs_in, int iq_format, uint32_t nf
   if (!p) return fail(ctx, LCS_ERR_STATE, "lcs_psd_create: out of memory");
   p->ctx = ctx;
   p->fmt = iq_format;
-  p->carry.esz = stream_sample_bytes(iq_format);
+  p->carry.esz = sample_bytes(iq_format);
   p->fs = (long long)r;
   p->N = nfft;
   p->lg = lg;

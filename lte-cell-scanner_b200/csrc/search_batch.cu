@@ -13,6 +13,7 @@
 
 #include "chain_gpu.hpp"
 #include "chain_host.hpp"
+#include "iq_format.cuh"
 #include "lcs_ctx.hpp"
 
 namespace lcs {
@@ -146,8 +147,8 @@ static lcs_status search_chunks(lcs_ctx* ctx, PlanSet& ps, int kernel, lcs_xcorr
                                 int iq_format, uint32_t batch, uint32_t chunk, const uint32_t* d_buf_plan, const uint32_t* h_buf_plan,
                                 F&& per_buffer, bool device_input = false) {
   const XcorrGeom& g = ps.geom;
-  const size_t samp_bytes = iq_sample_bytes(iq_format);
-  if (!samp_bytes) return fail(ctx, LCS_ERR_ARG, "search_batch: bad iq_format");
+  if (!SearchFormats::has(iq_format)) return fail(ctx, LCS_ERR_ARG, "search_batch: bad iq_format");
+  const size_t samp_bytes = sample_bytes(iq_format);
   if (batch == 0) return LCS_OK;
   LCS_CUDA(ctx, cudaSetDevice(ctx->device));
   chunk = std::max<uint32_t>(1, std::min<uint32_t>(chunk, batch));

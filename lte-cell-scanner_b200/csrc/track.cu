@@ -18,6 +18,7 @@
 
 #include "chain_host.hpp"
 #include "fft128.cuh"
+#include "iq_format.cuh"
 #include "lcs_ctx.hpp"
 
 namespace lcs {

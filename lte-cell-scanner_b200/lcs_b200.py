@@ -611,26 +611,30 @@ def chan_design_rational(fs_in):
     return up.value, down.value, h
 
 
-# sample format name -> (lcs format, numpy dtype of the [n][2] components)
-CHAN_FORMATS = {"ci16": (IQ_CI16, np.int16), "cs8": (IQ_CS8, np.int8), "cu8": (IQ_CU8, np.uint8),
-                "cf32": (IQ_CF32, np.float32)}
+# sample format name -> (lcs format, numpy dtype of the [...][2] components)
+IQ_FORMATS = {"cf32": (IQ_CF32, np.float32), "cu8": (IQ_CU8, np.uint8), "c128": (IQ_C128, np.float64),
+              "ci16": (IQ_CI16, np.int16), "cs8": (IQ_CS8, np.int8)}
+SEARCH_FORMATS = ("cf32", "cu8", "c128")             # what the correlator, the search and the cell measurement take
+STREAM_FORMATS = ("ci16", "cs8", "cu8", "cf32")      # what the channelizer and the spectrum take
 
 
 def _iq_format(fmt):
-    """The lcs format of a sample format name of CHAN_FORMATS."""
-    if fmt not in CHAN_FORMATS:
-        raise ValueError("fmt must be one of %s" % ", ".join(CHAN_FORMATS))
-    return CHAN_FORMATS[fmt][0]
+    """The lcs format of a sample format name of STREAM_FORMATS."""
+    if fmt not in STREAM_FORMATS:
+        raise ValueError("fmt must be one of %s" % ", ".join(STREAM_FORMATS))
+    return IQ_FORMATS[fmt][0]
 
 
-def _samples(iq, fmt):
-    """iq as a contiguous [n][2] array of fmt's dtype (complex64 [n] is accepted for cf32)."""
-    dtype = CHAN_FORMATS[fmt][1]
+def _samples(iq, fmt, ndims=(2,)):
+    """iq as contiguous [...][2] components of fmt's dtype with one of `ndims` dimensions; complex64 / complex128 arrays
+    (one dimension fewer) are accepted for cf32 / c128."""
+    dtype = IQ_FORMATS[fmt][1]
     iq = np.asarray(iq)
-    if fmt == "cf32" and iq.dtype == np.complex64 and iq.ndim == 1:
-        iq = iq.view(np.float32).reshape(-1, 2)
-    if iq.dtype != dtype or iq.ndim != 2 or iq.shape[1] != 2:
-        raise ValueError("expected %s samples: %s [n][2]" % (fmt, np.dtype(dtype).name))
+    if iq.dtype in (np.complex64, np.complex128):
+        iq = iq.view(iq.real.dtype).reshape(iq.shape + (2,))
+    if iq.dtype != dtype or iq.ndim not in ndims or iq.shape[-1] != 2:
+        raise ValueError("expected %s samples: %s, %s dimensions, the last of 2" % (fmt, np.dtype(dtype).name,
+                                                                                  " or ".join(map(str, ndims))))
     return np.ascontiguousarray(iq)
 
 
@@ -713,10 +717,7 @@ class Channelizer(RationalChannelizer):
 
     def _samples(self, iq):
         """iq as contiguous int16 [n][2], cast from other integer types."""
-        iq = np.ascontiguousarray(iq, np.int16)
-        if iq.ndim != 2 or iq.shape[1] != 2:
-            raise ValueError("expected ci16 samples [n][2]")
-        return iq
+        return _samples(np.asarray(iq, np.int16), "ci16")
 
     push_ci16 = RationalChannelizer.push
     push_ci16_device = RationalChannelizer.push_device
@@ -761,7 +762,6 @@ class Spectrum(_Handle):
 # lcs_cell_meas as a numpy record
 CELL_MEAS = np.dtype([("rsrp", np.float64, 4), ("noise", np.float64, 4), ("sinr", np.float64, 4), ("rssi", np.float64),
                       ("rsrq", np.float64), ("n_pairs", np.uint32, 4)], align=True)
-MEAS_FORMATS = {"cu8": (IQ_CU8, np.uint8), "cf32": (IQ_CF32, np.float32), "c128": (IQ_C128, np.float64)}
 
 
 class CellMeasure(_Handle):
@@ -781,7 +781,9 @@ class CellMeasure(_Handle):
         one channel) of format fmt: cu8 (uint8), cf32 (float32) or c128 (float64); complex64 / complex128 [n_ch][n_cap]
         are accepted for cf32 / c128.  iq may be a contiguous CUDA tensor (read in place; its stream is synchronised
         first).  ch[i] is the channel of cell i (default 0).  Returns a CELL_MEAS record array, one row per cell."""
-        iq_format, dtype = MEAS_FORMATS[fmt]
+        if fmt not in SEARCH_FORMATS:
+            raise KeyError(fmt)
+        iq_format = IQ_FORMATS[fmt][0]
         cells = list(cells)
         n = len(cells)
         arr = (Cell * max(n, 1))()
@@ -800,12 +802,7 @@ class CellMeasure(_Handle):
             torch.cuda.current_stream(iq.device).synchronize()
             ptr, on_device = iq.data_ptr(), 1
         else:
-            iq = np.asarray(iq)
-            if iq.dtype in (np.complex64, np.complex128):
-                iq = iq.view(iq.real.dtype).reshape(iq.shape + (2,))
-            if iq.dtype != dtype:
-                raise ValueError("expected %s samples: %s [n_ch][n_cap][2]" % (fmt, np.dtype(dtype).name))
-            iq = np.ascontiguousarray(iq)
+            iq = _samples(iq, fmt, (2, 3))
             shape, ptr, on_device = iq.shape, iq.ctypes.data, 0
         if len(shape) == 2:
             shape = (1,) + shape
