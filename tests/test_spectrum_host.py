@@ -28,6 +28,7 @@ class WelchOracle:
     def __init__(self, fs, N):
         self.fs, self.N = fs, N
         self.w = hann(N)
+        self.ws = np.sum(self.w ** 2)                          # the normalisation's sum of w[n]^2
         self.carry = np.zeros(0, complex)
         self.acc = np.zeros(N)
         self.S = 0
@@ -44,7 +45,7 @@ class WelchOracle:
 
     def read(self):
         """(P in fftshift order, S); the accumulator restarts."""
-        P = np.fft.fftshift(self.acc / (self.S * self.fs * np.sum(self.w ** 2))) if self.S else np.zeros(self.N)
+        P = np.fft.fftshift(self.acc / (self.S * self.fs * self.ws)) if self.S else np.zeros(self.N)
         S, self.acc, self.S = self.S, np.zeros(self.N), 0
         return P, S
 
