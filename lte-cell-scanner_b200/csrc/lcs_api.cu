@@ -210,9 +210,8 @@ lcs_status lcs_xcorr_pss_device(lcs_xcorr_plan* plan, const void* d_iq, int iq_f
                     (cudaStream_t)stream);
 }
 
-// Host-buffer batched call: chunks of the batch rotate over the context's three streams so that the
-// copies of the neighbouring chunks overlap the kernels of chunk i (with two streams the upload of chunk
-// i+2 sits behind the download of chunk i on the same stream and only just fits behind one chunk's kernels).
+// Host-buffer batched call: chunks of the batch rotate over the context's streams (rotate_chunks), so that the copies
+// of the neighbouring chunks overlap the kernels of a chunk; the host waits only once, for every stream at the end.
 lcs_status lcs_xcorr_pss_batch_host(lcs_xcorr_plan* p, const void* h_iq, int iq_format, uint32_t batch,
                                     float* h_single, double* h_pow, int32_t* h_frq, double* h_spi) {
   if (!p) return fail(nullptr, LCS_ERR_ARG, "xcorr_pss_batch_host: null plan");
@@ -223,20 +222,10 @@ lcs_status lcs_xcorr_pss_batch_host(lcs_xcorr_plan* p, const void* h_iq, int iq_
   if (!SearchFormats::has(iq_format)) return fail(ctx, LCS_ERR_ARG, "xcorr_pss_batch_host: bad iq_format");
   const size_t samp_bytes = sample_bytes(iq_format);
   LCS_CUDA(ctx, cudaSetDevice(ctx->device));
-  // chunk: large enough that the persistent correlator CTAs get many tiles each (64 buffers x 38 tiles = 16.4 tiles per
-  // CTA, 3 % rounding loss), small enough that the copies of neighbouring chunks overlap the kernels
-  const uint32_t chunk = std::min<uint32_t>(std::min<uint32_t>(p->max_batch, 64u), batch);
+  const uint32_t chunk = std::min<uint32_t>(std::min<uint32_t>(p->max_batch, BATCH_CHUNK), batch);
   const size_t n_single = (size_t)3 * g.n_f_stride * LCS_N_FOLD;
-  constexpr int NS = lcs_ctx::N_STREAMS;
-  for (int s = 0; s < NS; s++) {
-    LCS_CUDA(ctx, p->hb[s].iq.ensure((size_t)chunk * g.n_cap * samp_bytes + 16));
-    LCS_CUDA(ctx, p->hb[s].single.ensure(chunk * n_single));
-    LCS_CUDA(ctx, p->hb[s].pow.ensure((size_t)chunk * 3 * LCS_N_FOLD));
-    LCS_CUDA(ctx, p->hb[s].frq.ensure((size_t)chunk * 3 * LCS_N_FOLD));
-    LCS_CUDA(ctx, p->hb[s].spi.ensure((size_t)chunk * LCS_N_FOLD));
-  }
-  int s = 0;
-  for (uint32_t b0 = 0; b0 < batch; b0 += chunk, s = (s + 1) % NS) {
+  for (auto& hb : p->hb) LCS_CUDA(ctx, hb.ensure(g, chunk, samp_bytes, true, false));
+  auto issue = [&](uint32_t b0, int s) -> lcs_status {
     const uint32_t nb = std::min(chunk, batch - b0);
     cudaStream_t st = ctx->streams[s];
     auto& hb = p->hb[s];
@@ -249,8 +238,11 @@ lcs_status lcs_xcorr_pss_batch_host(lcs_xcorr_plan* p, const void* h_iq, int iq_
     LCS_CUDA(ctx, cudaMemcpyAsync(h_pow + (size_t)b0 * 3 * LCS_N_FOLD, hb.pow.p, (size_t)nb * 3 * LCS_N_FOLD * 8, cudaMemcpyDeviceToHost, st));
     LCS_CUDA(ctx, cudaMemcpyAsync(h_frq + (size_t)b0 * 3 * LCS_N_FOLD, hb.frq.p, (size_t)nb * 3 * LCS_N_FOLD * 4, cudaMemcpyDeviceToHost, st));
     LCS_CUDA(ctx, cudaMemcpyAsync(h_spi + (size_t)b0 * LCS_N_FOLD, hb.spi.p, (size_t)nb * LCS_N_FOLD * 8, cudaMemcpyDeviceToHost, st));
-  }
-  for (int i = 0; i < NS; i++) LCS_CUDA(ctx, cudaStreamSynchronize(ctx->streams[i]));
+    return LCS_OK;
+  };
+  lcs_status rc = rotate_chunks(batch, chunk, issue, [](uint32_t, int) { return LCS_OK; });
+  if (rc != LCS_OK) return rc;
+  for (cudaStream_t st : ctx->streams) LCS_CUDA(ctx, cudaStreamSynchronize(st));
   return LCS_OK;
 }
 
@@ -270,12 +262,9 @@ lcs_status lcs_xcorr_pss(lcs_ctx* ctx, const double* capbuf, uint32_t n_cap, con
   const size_t n_single = (size_t)3 * n_f * LCS_N_FOLD;
   auto& hb = p->hb[0];
   LCS_CUDA(ctx, ctx->d_capbuf.ensure((size_t)n_cap * 2));
-  LCS_CUDA(ctx, hb.single.ensure(n_single));
+  LCS_CUDA(ctx, hb.ensure(g, 1, 0, false, false));
   LCS_CUDA(ctx, ctx->d_ref.ensure(n_single));
   LCS_CUDA(ctx, ctx->d_inc.ensure(n_single));
-  LCS_CUDA(ctx, hb.pow.ensure(3 * LCS_N_FOLD));
-  LCS_CUDA(ctx, hb.frq.ensure(3 * LCS_N_FOLD));
-  LCS_CUDA(ctx, hb.spi.ensure(LCS_N_FOLD));
   LCS_CUDA(ctx, cudaMemcpyAsync(ctx->d_capbuf.p, capbuf, (size_t)n_cap * 16, cudaMemcpyHostToDevice, st));
   // 8-bit exact input (an rtl-sdr capture, capbuf.cpp:172-175) goes to the tensor-core correlator
   const void* d_in = ctx->d_capbuf.p;

@@ -236,10 +236,40 @@ struct lcs_xcorr_plan {
     lcs::DevBuf<int32_t> npeaks;
     lcs::PinBuf<unsigned char> h_peaks;   // page-locked landing zones of the peak lists
     lcs::PinBuf<int32_t> h_npeaks;
+    // Room for `chunk` capture buffers of geometry g: the correlator's outputs, the IQ bytes copied from the host
+    // (host_iq) and the device peak search's buffers (with_peaks).  Defined in search_batch.cu.
+    cudaError_t ensure(const lcs::XcorrGeom& g, uint32_t chunk, size_t samp_bytes, bool host_iq, bool with_peaks);
   } hb[lcs_ctx::N_STREAMS];
 };
 
 namespace lcs {
+
+// Capture buffers per chunk of the host-batch calls: large enough that the persistent correlator CTAs get many tiles
+// each (64 buffers x 38 tiles = 16.4 tiles per CTA, 3 % rounding loss), small enough that the copies of neighbouring
+// chunks overlap the kernels.
+constexpr uint32_t BATCH_CHUNK = 64;
+
+// The chunk pipeline of the host-batch calls: issue(b0, s) enqueues chunk k, which starts at buffer b0, on stream
+// s = k % N_STREAMS; after issuing chunk k the host calls finish(b0, s) of chunk k - (N_STREAMS - 1).  So N_STREAMS - 1
+// chunks are in flight while the oldest one is finished, and the copies of the neighbouring chunks overlap the kernels of
+// a chunk (with two streams the upload of chunk i+2 would sit behind the download of chunk i).
+template <class Issue, class Finish>
+lcs_status rotate_chunks(uint32_t batch, uint32_t chunk, Issue&& issue, Finish&& finish) {
+  constexpr uint32_t NS = lcs_ctx::N_STREAMS;
+  const uint32_t n_chunks = (batch + chunk - 1) / chunk;
+  for (uint32_t k = 0; k < n_chunks + (NS - 1); k++) {
+    if (k < n_chunks) {
+      lcs_status rc = issue(k * chunk, (int)(k % NS));
+      if (rc != LCS_OK) return rc;
+    }
+    if (k >= NS - 1) {
+      const uint32_t kf = k - (NS - 1);
+      lcs_status rc = finish(kf * chunk, (int)(kf % NS));
+      if (rc != LCS_OK) return rc;
+    }
+  }
+  return LCS_OK;
+}
 
 lcs_status fail(lcs_ctx* ctx, lcs_status st, const std::string& msg);
 #define LCS_CUDA(ctx, expr)                                                                         \

@@ -445,11 +445,11 @@ def test_device_peak_search_vs_oracle(ctx, lcs, capbuf0000, capbuf_chain):
     plan.close()
 
 
-def test_peak_list_overflow_falls_back_to_host(ctx, lcs, oracle):
-    """A buffer with more PSS peaks than the device peak list holds (32) has its peak_search redone on the host: 16
-    copies of every root's pss_td, 600 samples apart within a root and 200 samples between roots so that no two overlap,
-    repeated in every half frame so that they fold coherently, over weak noise.  The batched peak search (the buffer
-    second in its chunk) and the single-buffer cell search report exactly the host list, which matches the oracle's."""
+def test_peak_list_holds_more_than_32_peaks(ctx, lcs, oracle):
+    """A buffer with 48 PSS peaks: 16 copies of every root's pss_td, 600 samples apart within a root and 200 samples
+    between roots so that no two overlap, repeated in every half frame so that they fold coherently, over weak noise.
+    The device peak list holds 102 entries, the most a buffer can have, so the batched peak search (the buffer second in
+    its chunk) and the single-buffer cell search report exactly the host peak_search list, which matches the oracle's."""
     fc = 739e6
     f = lcs.f_search_set(fc, 120.0)
     half = np.zeros(9600, np.complex128)
