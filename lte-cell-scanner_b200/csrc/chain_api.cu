@@ -9,23 +9,6 @@
 
 namespace lcs {
 
-// per-context scratch of the companion kernels, owned by the context (one thread per context, see lcs_b200.h)
-ChainScratch& chain_scratch(lcs_ctx* ctx) {
-  if (!ctx->chain) ctx->chain = new ChainScratch();
-  return *static_cast<ChainScratch*>(ctx->chain);
-}
-void chain_scratch_release(lcs_ctx* ctx) {
-  delete static_cast<ChainScratch*>(ctx->chain);
-  ctx->chain = nullptr;
-}
-
-static lcs_status upload_c128(lcs_ctx* ctx, const double* capbuf, uint32_t n_cap) {
-  LCS_CUDA(ctx, cudaSetDevice(ctx->device));
-  LCS_CUDA(ctx, ctx->d_capbuf.ensure((size_t)n_cap * 2));
-  LCS_CUDA(ctx, cudaMemcpyAsync(ctx->d_capbuf.p, capbuf, (size_t)n_cap * 16, cudaMemcpyHostToDevice, ctx->streams[0]));
-  return LCS_OK;
-}
-
 static void to_colmajor(const std::vector<cd>& rowmajor, int n_rows, int n_cols, double* out) {
   cd* o = reinterpret_cast<cd*>(out);
   for (int r = 0; r < n_rows; r++)
@@ -41,16 +24,14 @@ static std::vector<cd> from_colmajor(const double* in, int n_rows, int n_cols) {
 
 // Per-peak stages of CellSearch.cpp:510-558 (sss_detect -> pss_sss_foe -> extract_tfg -> tfoec -> decode_mib) on a
 // device-resident capture buffer; cells that fail the SSS or MIB tests are dropped like in the reference.
-// Two phases: the device stages run peak by peak on the context's stream; the host stages (tfoec, chan_est, PBCH decoding
+// Two phases: the device stages run on sc.st, each for all peaks at once; the host stages (tfoec, chan_est, PBCH decoding
 // with its 12 tail-biting Viterbi attempts - milliseconds per cell) of all surviving peaks then run on parallel threads.
-lcs_status cell_chain_dev(lcs_ctx* ctx, const void* d_cap, int fmt, uint32_t n_cap, const std::vector<lcs_cell>& pk, double fc_req,
-                          double fc_prog, double fs_prog, lcs_cell* cells, uint32_t max_cells, uint32_t* n_cells,
-                          const int32_t* tracked, uint32_t n_tracked, bool tracker_cycle) {
+lcs_status cell_chain_dev(const StageCall& sc, const std::vector<lcs_cell>& pk, lcs_cell* cells, uint32_t max_cells,
+                          uint32_t* n_cells, const int32_t* tracked, uint32_t n_tracked, bool tracker_cycle) {
   const double THRESH2_N_SIGMA = 3;     // CellSearch.cpp:528
   lcs_status rc = LCS_OK;
   if (n_cells) *n_cells = 0;
   if (pk.empty()) return LCS_OK;
-  ChainScratch& cs = chain_scratch(ctx);
   struct Pending {
     lcs_cell c;                      // after pss_sss_foe
     std::vector<cd> tfg;
@@ -60,7 +41,7 @@ lcs_status cell_chain_dev(lcs_ctx* ctx, const void* d_cap, int fmt, uint32_t n_c
   // device stages, each for all peaks at once
   std::vector<lcs_cell> det;
   std::vector<lcs_status> st1;
-  rc = dev_sss_detect_batch(ctx, cs, d_cap, fmt, n_cap, pk, THRESH2_N_SIGMA, fc_req, fc_prog, fs_prog, det, st1, nullptr);
+  rc = dev_sss_detect_batch(sc, pk, THRESH2_N_SIGMA, det, st1, nullptr);
   if (rc != LCS_OK) return rc;
   std::vector<lcs_cell> surv;
   for (size_t i = 0; i < pk.size(); i++) {
@@ -73,12 +54,12 @@ lcs_status cell_chain_dev(lcs_ctx* ctx, const void* d_cap, int fmt, uint32_t n_c
     surv.push_back(det[i]);
   }
   std::vector<lcs_cell> foe;
-  rc = dev_pss_sss_foe_batch(ctx, cs, d_cap, fmt, n_cap, surv, fc_req, fc_prog, fs_prog, foe);
+  rc = dev_pss_sss_foe_batch(sc, surv, foe);
   if (rc != LCS_OK) return rc;
   std::vector<std::vector<cd>> tfgs;
   std::vector<std::vector<double>> tss;
   std::vector<lcs_status> st3;
-  rc = dev_extract_tfg_batch(ctx, cs, d_cap, fmt, n_cap, foe, fc_req, fc_prog, fs_prog, tfgs, tss, st3);
+  rc = dev_extract_tfg_batch(sc, foe, tfgs, tss, st3);
   if (rc != LCS_OK) return rc;
   std::vector<Pending> pend;
   pend.reserve(foe.size());
@@ -95,7 +76,7 @@ lcs_status cell_chain_dev(lcs_ctx* ctx, const void* d_cap, int fmt, uint32_t n_c
     std::vector<cd> tfg_comp(q.tfg.size());
     std::vector<double> ts_comp(q.ts.size());
     lcs_cell o;
-    tfoec(q.c, q.tfg.data(), q.ts.data(), (int)q.ts.size(), fc_req, fc_prog, rs, tfg_comp.data(), ts_comp.data(), o);
+    tfoec(q.c, q.tfg.data(), q.ts.data(), (int)q.ts.size(), sc.cfg.fc_req, sc.cfg.fc_prog, rs, tfg_comp.data(), ts_comp.data(), o);
     decode_mib(o, tfg_comp.data(), (int)q.ts.size(), rs, q.out);
   };
   if (pend.size() <= 1) {
@@ -159,12 +140,17 @@ lcs_status lcs_sss_detect(lcs_ctx* ctx, const lcs_cell* cell, const double* capb
                           double* h1_np, double* h2_np, double* h1_nrm, double* h2_nrm, double* h1_ext, double* h2_ext,
                           double* log_lik_nrm, double* log_lik_ext) {
   if (!ctx || !cell || !capbuf || !cell_out) return fail(ctx, LCS_ERR_ARG, "sss_detect: null argument");
-  lcs_status rc = upload_c128(ctx, capbuf, n_cap);
+  const cudaStream_t st = ctx->streams[0];
+  lcs_status rc = upload_c128(ctx, capbuf, n_cap, st);
   if (rc != LCS_OK) return rc;
+  const PlanCfg cfg{fc_requested, fc_programmed, fs_programmed};
+  std::vector<lcs_cell> out;
+  std::vector<lcs_status> status;
   SssDebugHost d;
-  rc = dev_sss_detect(ctx, chain_scratch(ctx), ctx->d_capbuf.p, LCS_IQ_C128, n_cap, *cell, thresh2_n_sigma, fc_requested,
-                      fc_programmed, fs_programmed, *cell_out, &d);
+  rc = dev_sss_detect_batch(StageCall{ctx, ctx->d_capbuf.p, LCS_IQ_C128, n_cap, cfg, st}, {*cell}, thresh2_n_sigma, out, status, &d);
   if (rc != LCS_OK) return rc;
+  if (status[0] != LCS_OK) return fail(ctx, status[0], "sss_detect: DFT window outside the capture buffer");
+  *cell_out = out[0];
   if (h1_np) std::memcpy(h1_np, &d.est[0], 62 * 8);
   if (h2_np) std::memcpy(h2_np, &d.est[62], 62 * 8);
   if (h1_nrm) std::memcpy(h1_nrm, &d.est[124], 62 * 16);
@@ -179,26 +165,34 @@ lcs_status lcs_sss_detect(lcs_ctx* ctx, const lcs_cell* cell, const double* capb
 lcs_status lcs_pss_sss_foe(lcs_ctx* ctx, const lcs_cell* cell_in, const double* capbuf, uint32_t n_cap, double fc_requested,
                            double fc_programmed, double fs_programmed, lcs_cell* cell_out) {
   if (!ctx || !cell_in || !capbuf || !cell_out) return fail(ctx, LCS_ERR_ARG, "pss_sss_foe: null argument");
-  lcs_status rc = upload_c128(ctx, capbuf, n_cap);
+  const cudaStream_t st = ctx->streams[0];
+  lcs_status rc = upload_c128(ctx, capbuf, n_cap, st);
   if (rc != LCS_OK) return rc;
-  return dev_pss_sss_foe(ctx, chain_scratch(ctx), ctx->d_capbuf.p, LCS_IQ_C128, n_cap, *cell_in, fc_requested, fc_programmed,
-                         fs_programmed, *cell_out);
+  const PlanCfg cfg{fc_requested, fc_programmed, fs_programmed};
+  std::vector<lcs_cell> out;
+  rc = dev_pss_sss_foe_batch(StageCall{ctx, ctx->d_capbuf.p, LCS_IQ_C128, n_cap, cfg, st}, {*cell_in}, out);
+  if (rc != LCS_OK) return rc;
+  *cell_out = out[0];
+  return LCS_OK;
 }
 
 lcs_status lcs_extract_tfg(lcs_ctx* ctx, const lcs_cell* cell, const double* capbuf, uint32_t n_cap, double fc_requested,
                            double fc_programmed, double fs_programmed, double* tfg, double* tfg_timestamp,
                            uint32_t* n_ofdm_out) {
   if (!ctx || !cell || !capbuf || !tfg || !tfg_timestamp) return fail(ctx, LCS_ERR_ARG, "extract_tfg: null argument");
-  lcs_status rc = upload_c128(ctx, capbuf, n_cap);
+  const cudaStream_t st = ctx->streams[0];
+  lcs_status rc = upload_c128(ctx, capbuf, n_cap, st);
   if (rc != LCS_OK) return rc;
-  std::vector<cd> g;
-  std::vector<double> ts;
-  rc = dev_extract_tfg(ctx, chain_scratch(ctx), ctx->d_capbuf.p, LCS_IQ_C128, n_cap, *cell, fc_requested, fc_programmed,
-                       fs_programmed, g, ts);
+  const PlanCfg cfg{fc_requested, fc_programmed, fs_programmed};
+  std::vector<std::vector<cd>> g;
+  std::vector<std::vector<double>> ts;
+  std::vector<lcs_status> status;
+  rc = dev_extract_tfg_batch(StageCall{ctx, ctx->d_capbuf.p, LCS_IQ_C128, n_cap, cfg, st}, {*cell}, g, ts, status);
   if (rc != LCS_OK) return rc;
-  to_colmajor(g, (int)ts.size(), 72, tfg);
-  std::memcpy(tfg_timestamp, ts.data(), ts.size() * 8);
-  if (n_ofdm_out) *n_ofdm_out = (uint32_t)ts.size();
+  if (status[0] != LCS_OK) return fail(ctx, status[0], "extract_tfg: DFT window outside the capture buffer");
+  to_colmajor(g[0], (int)ts[0].size(), 72, tfg);
+  std::memcpy(tfg_timestamp, ts[0].data(), ts[0].size() * 8);
+  if (n_ofdm_out) *n_ofdm_out = (uint32_t)ts[0].size();
   return LCS_OK;
 }
 

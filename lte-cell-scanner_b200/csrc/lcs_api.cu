@@ -143,7 +143,6 @@ void lcs_ctx_destroy(lcs_ctx* ctx) {
   cudaDeviceSynchronize();
   for (auto* p : ctx->cached_plans) lcs_xcorr_plan_destroy(p);
   ctx->cached_plans.clear();
-  chain_scratch_release(ctx);
   for (int i = 0; i < lcs_ctx::N_STREAMS; i++)
     if (ctx->streams[i]) cudaStreamDestroy(ctx->streams[i]);
   delete ctx;
@@ -261,11 +260,11 @@ lcs_status lcs_xcorr_pss(lcs_ctx* ctx, const double* capbuf, uint32_t n_cap, con
   cudaStream_t st = ctx->streams[0];
   const size_t n_single = (size_t)3 * n_f * LCS_N_FOLD;
   auto& hb = p->hb[0];
-  LCS_CUDA(ctx, ctx->d_capbuf.ensure((size_t)n_cap * 2));
+  rc = upload_c128(ctx, capbuf, n_cap, st);
+  if (rc != LCS_OK) return rc;
   LCS_CUDA(ctx, hb.ensure(g, 1, 0, false, false));
   LCS_CUDA(ctx, ctx->d_ref.ensure(n_single));
   LCS_CUDA(ctx, ctx->d_inc.ensure(n_single));
-  LCS_CUDA(ctx, cudaMemcpyAsync(ctx->d_capbuf.p, capbuf, (size_t)n_cap * 16, cudaMemcpyHostToDevice, st));
   // 8-bit exact input (an rtl-sdr capture, capbuf.cpp:172-175) goes to the tensor-core correlator
   const void* d_in = ctx->d_capbuf.p;
   int fmt = LCS_IQ_C128;
@@ -324,6 +323,13 @@ lcs_status lcs_xcorr_pss(lcs_ctx* ctx, const double* capbuf, uint32_t n_cap, con
 }  // extern "C"
 
 namespace lcs {
+lcs_status upload_c128(lcs_ctx* ctx, const double* capbuf, uint32_t n_cap, cudaStream_t st) {
+  LCS_CUDA(ctx, cudaSetDevice(ctx->device));
+  LCS_CUDA(ctx, ctx->d_capbuf.ensure((size_t)n_cap * 2));
+  LCS_CUDA(ctx, cudaMemcpyAsync(ctx->d_capbuf.p, capbuf, (size_t)n_cap * 16, cudaMemcpyHostToDevice, st));
+  return LCS_OK;
+}
+
 lcs_status get_cached_plan(lcs_ctx* ctx, uint32_t n_cap, const double* f_search_set, uint32_t n_f, uint8_t arm,
                            double fc_req, double fc_prog, double fs_prog, lcs_xcorr_plan** out) {
   for (auto* q : ctx->cached_plans) {

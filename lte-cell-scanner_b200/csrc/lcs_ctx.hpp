@@ -24,6 +24,7 @@ struct DevBuf {   // owning device allocation
     return cudaMalloc((void**)&p, std::max<size_t>(count, 1) * sizeof(T));
   }
   cudaError_t ensure(size_t count) { return (p && n >= count) ? cudaSuccess : alloc(count); }
+  void swap(DevBuf& o) { std::swap(p, o.p); std::swap(n, o.n); }
 };
 
 template <class T>
@@ -40,6 +41,36 @@ struct PinBuf {   // owning page-locked host allocation (asynchronous copies nee
     n = count;
     return cudaMallocHost((void**)&p, std::max<size_t>(count, 1) * sizeof(T));
   }
+};
+
+// The small host tables of a launch, staged in page-locked memory and uploaded with one asynchronous copy.  reset(bytes)
+// makes room for slices of `bytes` in all, counting 16 bytes of alignment per slice; take() and put() hand out host
+// slices, upload() copies every slice taken since the reset, and dev() is the device address of a host slice.  A slice
+// may be written again once the stream its copy went to has been synchronised.
+struct Staging {
+  PinBuf<unsigned char> h;
+  DevBuf<unsigned char> d;
+  size_t off = 0;
+  cudaError_t reset(size_t bytes) {
+    off = 0;
+    cudaError_t e = h.ensure(bytes);
+    return e == cudaSuccess ? d.ensure(bytes) : e;
+  }
+  template <class T> T* take(size_t n) {
+    off = (off + 15) & ~(size_t)15;
+    T* p = reinterpret_cast<T*>(h.p + off);
+    off += n * sizeof(T);
+    return p;
+  }
+  template <class T> T* put(const std::vector<T>& v) {
+    T* p = take<T>(v.size());
+    std::copy(v.begin(), v.end(), p);
+    return p;
+  }
+  template <class T> T* dev(T* host) const {
+    return reinterpret_cast<T*>(d.p + (reinterpret_cast<const unsigned char*>(host) - h.p));
+  }
+  cudaError_t upload(cudaStream_t st) const { return cudaMemcpyAsync(d.p, h.p, off, cudaMemcpyHostToDevice, st); }
 };
 
 // Kernel time of a handle: CUDA event pairs recorded around groups of launches, each committed with the number of kernels
@@ -193,6 +224,19 @@ struct PlanSet {
   ~PlanSet() { if (staged) cudaEventDestroy(staged); }
 };
 
+// Scratch of the per-peak stages (chain_gpu.cu).  Every stage synchronises its stream before it returns, so the next
+// stage, on any stream, may reuse the staging.
+struct ChainScratch {
+  DevBuf<signed char> d_sss_tab;   // [168][3][2][62] +-1
+  DevBuf<double2> d_pss_fd;        // [3][62]
+  Staging up;                      // per stage: segment starts and shifts, peak parameters or the cells' grid geometry
+  PinBuf<unsigned char> h_down;    // page-locked landing zone of the results
+  DevBuf<double2> d_psss;          // [n_seg][62]
+  DevBuf<double> d_est;            // [124] np + 4x62 complex
+  DevBuf<double> d_ll;             // [4][168]
+  DevBuf<double2> d_tfg;           // [cell][TFG_MAX][72]
+};
+
 }  // namespace lcs
 
 struct lcs_xcorr_plan;
@@ -202,7 +246,6 @@ struct lcs_ctx {
   int n_sm = 0;
   static constexpr int N_STREAMS = 3;           // chunks of the host-batch calls rotate over these
   cudaStream_t streams[N_STREAMS] = {nullptr, nullptr, nullptr};
-  cudaStream_t chain_stream = nullptr;         // stream of the per-peak stages (NULL: streams[0]); the chunked search sets it to the idle stream of the chunk it examines
   std::string last_error;
   uint64_t launches = 0;
   std::vector<lcs_xcorr_plan*> cached_plans;   // for the plan-less drop-in calls
@@ -214,7 +257,7 @@ struct lcs_ctx {
   lcs::DevBuf<float> d_ref, d_inc;
   lcs::DevBuf<unsigned char> d_cu8;
   lcs::DevBuf<int> d_flag8;                    // 8-bit exactness probe of lcs_xcorr_pss
-  void* chain = nullptr;                       // lcs::ChainScratch (chain_api.cu), owned
+  lcs::ChainScratch chain;                     // one thread per context (lcs_b200.h)
 };
 
 struct lcs_xcorr_plan {
@@ -298,10 +341,8 @@ lcs_status planset_run(PlanSet& ps, int kernel, const void* d_iq, int iq_format,
 
 lcs_status get_cached_plan(lcs_ctx* ctx, uint32_t n_cap, const double* f_search_set, uint32_t n_f, uint8_t arm,
                            double fc_req, double fc_prog, double fs_prog, lcs_xcorr_plan** out);
-void chain_scratch_release(lcs_ctx* ctx);   // chain_api.cu
-lcs_status cell_chain_dev(lcs_ctx* ctx, const void* d_cap, int fmt, uint32_t n_cap, const std::vector<lcs_cell>& pk, double fc_req,
-                          double fc_prog, double fs_prog, lcs_cell* cells, uint32_t max_cells, uint32_t* n_cells,
-                          const int32_t* tracked = nullptr, uint32_t n_tracked = 0, bool tracker_cycle = false);   // chain_api.cu
+// The c128 capture buffer of a drop-in call into ctx->d_capbuf, on the context's device, asynchronously on st.
+lcs_status upload_c128(lcs_ctx* ctx, const double* capbuf, uint32_t n_cap, cudaStream_t st);
 // ---- xcorr_tc.cu ----
 lcs_status tc_init(lcs_ctx* ctx);           // one-time function attributes
 int launch_xcorr_fold_tc(PlanSet& ps, const void* d_iq_cu8, uint32_t batch, const uint32_t* d_buf_plan,

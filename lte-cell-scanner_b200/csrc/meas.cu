@@ -2,12 +2,13 @@
 // contract in include/lcs_meas.h).
 //
 // One call measures every cell it is given with two launches on the context's stream:
-//   1. tfg_kernel (chain_gpu.cu, through launch_tfg): each cell's 72-subcarrier grid, exactly as lcs_extract_tfg makes it
+//   1. tfg_kernel (chain_gpu.cu, through launch_grids): each cell's 72-subcarrier grid, exactly as lcs_extract_tfg makes it
 //      for the cell with freq_fine = freq_superfine; the cells may sit in different channels of one [n_ch][n_cap] buffer.
 //   2. meas_kernel: one CTA per cell.  Each thread sums a fixed, strided subset of the cell's CRS pairs (and of its RSSI
 //      resource elements) in FP64; the warps then reduce with a fixed shuffle tree and thread 0 adds the warps in order.
 //      The result is thus the same on every run and independent of the other cells of the call.
-// The CRS values and their subcarrier shifts come from the host tables (RsDl, chain_host.cpp), uploaded per call.
+// The CRS values and their subcarrier shifts come from the host tables (RsDl, chain_host.cpp), staged with the grid
+// geometry and uploaded with it in one copy per call.
 #include <cmath>
 #include <limits>
 #include <new>
@@ -108,13 +109,8 @@ using namespace lcs;
 struct lcs_meas {
   lcs_ctx* ctx = nullptr;
   DevBuf<unsigned char> d_iq;              // host input, uploaded
-  DevBuf<uint64_t> d_base;                 // [cell] first sample of the cell's channel
-  DevBuf<int> d_pos, d_nofdm;
-  DevBuf<double> d_late, d_k;
+  Staging up;                              // per call: the grid geometry, the CRS and shift tables and the cell parameters
   DevBuf<double2> d_tfg;                   // [cell][TFG_MAX][72]
-  DevBuf<double2> d_rs;                    // [cell][20][3][12]
-  DevBuf<unsigned char> d_shift;           // [cell][20][3][4]
-  DevBuf<int4> d_par;
   DevBuf<lcs_cell_meas> d_out;
   KernelClock clock;                       // both launches of each call
 };
@@ -154,13 +150,16 @@ lcs_status lcs_meas_cells(lcs_meas* m, const void* iq, int iq_format, int on_dev
   if (!(std::isfinite(fs_programmed) && fs_programmed > 0)) return mfail(m, "fs_programmed must be finite and positive");
   if (!n_cells) return LCS_OK;
   // host tables of every cell, and every argument checked, before any device work
+  lcs_ctx* ctx = m->ctx;
+  LCS_CUDA(ctx, cudaSetDevice(ctx->device));
   const size_t L = n_cells;
-  std::vector<int> pos(L * TFG_MAX, 0), nofdm(L);
-  std::vector<double> late(L * TFG_MAX, 0.0), kc(L), ts(TFG_MAX);
-  std::vector<uint64_t> base(L);
-  std::vector<cd> rs_tab(L * meas::N_SLOT_TAB * 3 * 12);
-  std::vector<unsigned char> shift_tab(L * meas::N_SLOT_TAB * 3 * 4);
-  std::vector<int4> par(L);
+  const size_t n_tab = L * meas::N_SLOT_TAB * 3;
+  LCS_CUDA(ctx, m->up.reset(GridTables::bytes(L) + n_tab * (12 * sizeof(cd) + 4) + L * sizeof(int4) + 3 * 16));
+  const GridTables g(m->up, L, true);
+  cd* rs_tab = m->up.take<cd>(n_tab * 12);                         // [cell][20][3][12]
+  unsigned char* shift_tab = m->up.take<unsigned char>(n_tab * 4);  // [cell][20][3][4]
+  int4* par = m->up.take<int4>(L);
+  std::vector<double> ts(TFG_MAX);
   for (size_t i = 0; i < L; i++) {
     const lcs_cell& c = cells[i];
     const std::string who = "cell " + std::to_string(i) + ": ";
@@ -172,13 +171,12 @@ lcs_status lcs_meas_cells(lcs_meas* m, const void* iq, int iq_format, int on_dev
       return mfail(m, who + "frame_start and freq_superfine must be finite");
     if (!(std::isfinite(c.fc_requested) && c.fc_requested > 0 && std::isfinite(c.fc_programmed) && c.fc_programmed > 0))
       return mfail(m, who + "fc_requested and fc_programmed must be finite and positive");
-    lcs_cell g = c;
-    g.freq_fine = c.freq_superfine;
+    lcs_cell gc = c;
+    gc.freq_fine = c.freq_superfine;
     const char* why = "";
-    if (tfg_geometry(g, c.fc_requested, c.fc_programmed, fs_programmed, n_cap, &pos[i * TFG_MAX], &late[i * TFG_MAX],
-                     ts.data(), &kc[i], &nofdm[i], &why) != LCS_OK)
+    if (tfg_geometry(gc, c.fc_requested, c.fc_programmed, fs_programmed, n_cap, g, i, ts.data(), &why) != LCS_OK)
       return mfail(m, who + "grid does not fit in the capture buffer (" + why + ")");
-    base[i] = (uint64_t)ch[i] * n_cap;
+    g.base[i] = (uint64_t)ch[i] * n_cap;
     const RsDl rs(c.n_id_2 + 3 * c.n_id_1, c.cp_type);
     for (int sl = 0; sl < meas::N_SLOT_TAB; sl++)
       for (int s3 = 0; s3 < 3; s3++) {
@@ -187,11 +185,9 @@ lcs_status lcs_meas_cells(lcs_meas* m, const void* iq, int iq_format, int on_dev
         for (int k = 0; k < 12; k++) rs_tab[((i * meas::N_SLOT_TAB + sl) * 3 + s3) * 12 + k] = r[k];
         for (int p = 0; p < 4; p++) shift_tab[((i * meas::N_SLOT_TAB + sl) * 3 + s3) * 4 + p] = (unsigned char)rs.shift(sl, sym, p);
       }
-    par[i] = make_int4(rs.n_symb, c.n_ports, nofdm[i], 0);
+    par[i] = make_int4(rs.n_symb, c.n_ports, g.n_ofdm[i], 0);
   }
-  lcs_ctx* ctx = m->ctx;
   cudaStream_t st = ctx->streams[0];
-  LCS_CUDA(ctx, cudaSetDevice(ctx->device));
   const void* d_iq = iq;
   if (!on_device) {
     const size_t bytes = (size_t)n_ch * n_cap * esz;
@@ -199,29 +195,15 @@ lcs_status lcs_meas_cells(lcs_meas* m, const void* iq, int iq_format, int on_dev
     LCS_CUDA(ctx, cudaMemcpyAsync(m->d_iq.p, iq, bytes, cudaMemcpyHostToDevice, st));
     d_iq = m->d_iq.p;
   }
-  LCS_CUDA(ctx, m->d_base.ensure(L));
-  LCS_CUDA(ctx, m->d_pos.ensure(L * TFG_MAX));
-  LCS_CUDA(ctx, m->d_late.ensure(L * TFG_MAX));
-  LCS_CUDA(ctx, m->d_k.ensure(L));
-  LCS_CUDA(ctx, m->d_nofdm.ensure(L));
   LCS_CUDA(ctx, m->d_tfg.ensure(L * TFG_MAX * 72));
-  LCS_CUDA(ctx, m->d_rs.ensure(rs_tab.size()));
-  LCS_CUDA(ctx, m->d_shift.ensure(shift_tab.size()));
-  LCS_CUDA(ctx, m->d_par.ensure(L));
   LCS_CUDA(ctx, m->d_out.ensure(L));
-  LCS_CUDA(ctx, cudaMemcpyAsync(m->d_base.p, base.data(), L * sizeof(uint64_t), cudaMemcpyHostToDevice, st));
-  LCS_CUDA(ctx, cudaMemcpyAsync(m->d_pos.p, pos.data(), pos.size() * sizeof(int), cudaMemcpyHostToDevice, st));
-  LCS_CUDA(ctx, cudaMemcpyAsync(m->d_late.p, late.data(), late.size() * sizeof(double), cudaMemcpyHostToDevice, st));
-  LCS_CUDA(ctx, cudaMemcpyAsync(m->d_k.p, kc.data(), L * sizeof(double), cudaMemcpyHostToDevice, st));
-  LCS_CUDA(ctx, cudaMemcpyAsync(m->d_nofdm.p, nofdm.data(), L * sizeof(int), cudaMemcpyHostToDevice, st));
-  LCS_CUDA(ctx, cudaMemcpyAsync(m->d_rs.p, rs_tab.data(), rs_tab.size() * sizeof(cd), cudaMemcpyHostToDevice, st));
-  LCS_CUDA(ctx, cudaMemcpyAsync(m->d_shift.p, shift_tab.data(), shift_tab.size(), cudaMemcpyHostToDevice, st));
-  LCS_CUDA(ctx, cudaMemcpyAsync(m->d_par.p, par.data(), L * sizeof(int4), cudaMemcpyHostToDevice, st));
+  LCS_CUDA(ctx, m->up.upload(st));
   LCS_CUDA(ctx, m->clock.begin(st));
-  if (launch_tfg(d_iq, iq_format, m->d_base.p, m->d_pos.p, m->d_late.p, m->d_k.p, m->d_nofdm.p, n_cells, m->d_tfg.p, st) != LCS_OK)
-    return mfail(m, "no grid kernel for this iq_format");
-  meas::meas_kernel<<<n_cells, meas::THREADS, 0, st>>>(m->d_tfg.p, m->d_rs.p, m->d_shift.p, m->d_par.p, m->d_out.p);
-  ctx->launches += 2;
+  lcs_status rc = launch_grids(ctx, m->up, g, n_cells, d_iq, iq_format, m->d_tfg.p, st, "lcs_meas_cells: no grid kernel for this iq_format");
+  if (rc != LCS_OK) return rc;
+  meas::meas_kernel<<<n_cells, meas::THREADS, 0, st>>>(m->d_tfg.p, reinterpret_cast<const double2*>(m->up.dev(rs_tab)),
+                                                       m->up.dev(shift_tab), m->up.dev(par), m->d_out.p);
+  ctx->launches++;
   LCS_CUDA(ctx, cudaGetLastError());
   LCS_CUDA(ctx, m->clock.end(st, 2));
   LCS_CUDA(ctx, cudaMemcpyAsync(out, m->d_out.p, L * sizeof(lcs_cell_meas), cudaMemcpyDeviceToHost, st));

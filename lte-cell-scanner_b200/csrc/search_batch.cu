@@ -138,9 +138,10 @@ static lcs_status launch_peak_search(lcs_ctx* ctx, const XcorrGeom& g, uint32_t 
 }
 
 // Shared driver: xcorr_pss + threshold + peak_search for `batch` host capture buffers in chunks on the context's streams
-// (rotate_chunks); `per_buffer(buffer index, device pointer of the buffer's IQ bytes, the buffer's PlanCfg, its PSS
-// peaks)` runs on the host after the chunk's kernels finished while the next chunks are already in flight on the other
-// streams.
+// (rotate_chunks); `per_buffer(buffer index, StageCall of the buffer, its PSS peaks)` runs on the host after the chunk's
+// kernels finished while the next chunks are already in flight on the other streams.  The StageCall names the buffer's
+// IQ bytes on the device, its PlanCfg and the chunk's stream, which is idle by then: the per-peak kernels do not queue
+// behind later chunks.
 // d_buf_plan == NULL: every buffer is searched with plan 0 of `ps`; otherwise buffer b uses plan d_buf_plan[b] and
 // h_buf_plan[b] names the same plan on the host.
 // device_input: h_iq is device memory; each chunk is searched in place there (no host-to-device copy).
@@ -200,9 +201,8 @@ static lcs_status search_chunks(lcs_ctx* ctx, PlanSet& ps, int kernel, lcs_xcorr
         c.n_id_2 = (int8_t)d.row;
         pk.push_back(c);
       }
-      ctx->chain_stream = ctx->streams[s];        // this chunk's stream is idle now: the per-peak kernels do not queue behind later chunks
-      lcs_status rc = per_buffer(b0 + i, (const void*)(chunk_iq(b0, s) + (size_t)i * g.n_cap * samp_bytes), cfg, pk);
-      ctx->chain_stream = nullptr;
+      const StageCall sc{ctx, chunk_iq(b0, s) + (size_t)i * g.n_cap * samp_bytes, iq_format, g.n_cap, cfg, ctx->streams[s]};
+      lcs_status rc = per_buffer(b0 + i, sc, pk);
       if (rc != LCS_OK) return rc;
     }
     return LCS_OK;
@@ -219,16 +219,15 @@ struct TrackerCycle {
 };
 
 // The per-buffer step of the cell-search entry points: the per-peak chain (CellSearch.cpp:510-558) on buffer b of a
-// search_chunks call with the buffer's plan configuration; writes cells[b * max_cells ...] and n_cells[b].
-static lcs_status chain_step(lcs_ctx* ctx, uint32_t n_cap, int fmt, uint32_t b, const void* d_cap, const PlanCfg& cfg,
-                             const std::vector<lcs_cell>& pk, lcs_cell* cells, uint32_t max_cells, uint32_t* n_cells,
-                             const TrackerCycle* tc = nullptr) {
+// search_chunks call; writes cells[b * max_cells ...] and n_cells[b].
+static lcs_status chain_step(uint32_t b, const StageCall& sc, const std::vector<lcs_cell>& pk, lcs_cell* cells, uint32_t max_cells,
+                             uint32_t* n_cells, const TrackerCycle* tc = nullptr) {
   lcs_cell* out = cells ? cells + (size_t)b * max_cells : nullptr;
   uint32_t found = 0;
-  const lcs_status rc = cell_chain_dev(ctx, d_cap, fmt, n_cap, pk, cfg.fc_req, cfg.fc_prog, cfg.fs_prog, out, max_cells, &found,
-                                       tc ? tc->tracked : nullptr, tc ? tc->n_tracked : 0, tc != nullptr);
+  const lcs_status rc = cell_chain_dev(sc, pk, out, max_cells, &found, tc ? tc->tracked : nullptr, tc ? tc->n_tracked : 0, tc != nullptr);
   n_cells[b] = found;
   if (tc) {
+    const PlanCfg& cfg = sc.cfg;
     const double k_factor = (cfg.fc_req - cfg.f[0]) / cfg.fc_prog;
     for (uint32_t i = 0; i < found && i < max_cells; i++)                                  // searcher_thread.cpp:214
       tc->frame_timing[(size_t)b * max_cells + i] = out[i].frame_start * (30720000.0 / 16) / (cfg.fs_prog * k_factor) + tc->late;
@@ -246,10 +245,10 @@ static lcs_status search_one(lcs_ctx* ctx, const void* capbuf, int fmt, uint32_t
   if (rc != LCS_OK) return rc;
   uint32_t found = 0;
   rc = search_chunks(ctx, p->ps, p->kernel, p->hb, capbuf, fmt, 1, 1, nullptr, nullptr,
-                     [&](uint32_t b, const void* d_cap, const PlanCfg& cfg, const std::vector<lcs_cell>& pk) {
+                     [&](uint32_t b, const StageCall& sc, const std::vector<lcs_cell>& pk) {
                        if (n_peaks) *n_peaks = (uint32_t)pk.size();
                        for (size_t i = 0; peaks && i < pk.size() && i < max_cells; i++) peaks[i] = pk[i];
-                       return chain_step(ctx, n_cap, fmt, b, d_cap, cfg, pk, cells, max_cells, &found, tc);
+                       return chain_step(b, sc, pk, cells, max_cells, &found, tc);
                      });
   if (n_cells) *n_cells = found;
   return rc;
@@ -318,7 +317,7 @@ lcs_status lcs_xcorr_peaks_batch_host(lcs_xcorr_plan* p, const void* iq_host, in
   if (!p) return fail(nullptr, LCS_ERR_ARG, "xcorr_peaks_batch_host: null plan");
   if (!iq_host || !n_peaks || (!peaks && max_peaks)) return fail(p->ctx, LCS_ERR_ARG, "xcorr_peaks_batch_host: null pointer");
   return search_chunks(p->ctx, p->ps, p->kernel, p->hb, iq_host, iq_format, batch, std::min<uint32_t>(p->max_batch, BATCH_CHUNK), nullptr,
-                       nullptr, [&](uint32_t b, const void*, const PlanCfg&, const std::vector<lcs_cell>& pk) {
+                       nullptr, [&](uint32_t b, const StageCall&, const std::vector<lcs_cell>& pk) {
                          n_peaks[b] = (uint32_t)pk.size();
                          for (size_t k = 0; k < pk.size() && k < max_peaks; k++) peaks[(size_t)b * max_peaks + k] = pk[k];
                          return LCS_OK;
@@ -330,8 +329,8 @@ lcs_status lcs_cell_search_batch_cu8(lcs_xcorr_plan* p, const uint8_t* iq_host, 
   if (!p) return fail(nullptr, LCS_ERR_ARG, "cell_search_batch_cu8: null plan");
   if (!iq_host || !n_cells || (!cells && max_cells)) return fail(p->ctx, LCS_ERR_ARG, "cell_search_batch_cu8: null pointer");
   return search_chunks(p->ctx, p->ps, p->kernel, p->hb, iq_host, LCS_IQ_CU8, batch, std::min<uint32_t>(p->max_batch, BATCH_CHUNK), nullptr,
-                       nullptr, [&](uint32_t b, const void* d_cap, const PlanCfg& cfg, const std::vector<lcs_cell>& pk) {
-                         return chain_step(p->ctx, p->ps.geom.n_cap, LCS_IQ_CU8, b, d_cap, cfg, pk, cells, max_cells, n_cells);
+                       nullptr, [&](uint32_t b, const StageCall& sc, const std::vector<lcs_cell>& pk) {
+                         return chain_step(b, sc, pk, cells, max_cells, n_cells);
                        });
 }
 
@@ -436,8 +435,8 @@ static lcs_status sweep_search(lcs_sweep* sw, const uint8_t* iq, bool device_inp
   if (rc != LCS_OK) return rc;
   // chunks of 64 channels: 128 units of 38+ tiles keep every persistent correlator CTA busy for >30 tiles
   return search_chunks(ctx, sw->ps, LCS_KERNEL_AUTO, sw->hb, iq, LCS_IQ_CU8, n_ch, BATCH_CHUNK, sw->d_ident.p, sw->h_ident.data(),
-                       [&](uint32_t b, const void* d_cap, const PlanCfg& cfg, const std::vector<lcs_cell>& pk) {
-                         return chain_step(ctx, sw->n_cap, LCS_IQ_CU8, b, d_cap, cfg, pk, cells, max_cells, n_cells);
+                       [&](uint32_t b, const StageCall& sc, const std::vector<lcs_cell>& pk) {
+                         return chain_step(b, sc, pk, cells, max_cells, n_cells);
                        },
                        device_input);
 }
@@ -485,10 +484,10 @@ lcs_status lcs_sweep_track_cu8(lcs_sweep* sw, const uint8_t* iq_host, uint32_t n
   lcs_status rc = sweep_prepare(sw, cfgs, 2, true);
   if (rc != LCS_OK) return rc;
   return search_chunks(ctx, sw->ps, LCS_KERNEL_AUTO, sw->hb, iq_host, LCS_IQ_CU8, n_ch, BATCH_CHUNK, sw->d_ident.p, sw->h_ident.data(),
-                       [&](uint32_t b, const void* d_cap, const PlanCfg& cfg, const std::vector<lcs_cell>& pk) {
+                       [&](uint32_t b, const StageCall& sc, const std::vector<lcs_cell>& pk) {
                          const TrackerCycle tc{n_tracked ? tracked_n_id_cell + (size_t)b * tracked_stride : nullptr,
                                                n_tracked ? n_tracked[b] : 0, late ? late[b] : 0.0, frame_timing};
-                         return chain_step(ctx, sw->n_cap, LCS_IQ_CU8, b, d_cap, cfg, pk, cells, max_cells, n_cells, &tc);
+                         return chain_step(b, sc, pk, cells, max_cells, n_cells, &tc);
                        });
 }
 
