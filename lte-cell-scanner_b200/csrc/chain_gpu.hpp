@@ -45,6 +45,8 @@ struct GridTables {
   uint64_t* base;
   static size_t bytes(size_t n_cells) { return n_cells * (TFG_MAX * 12 + 20) + 5 * 16; }   // Staging::reset
   GridTables(Staging& up, size_t n_cells, bool with_base);
+  // Over caller-owned host arrays, for geometry that is not uploaded: pos / late [n_cells][TFG_MAX], k / n_ofdm [n_cells].
+  GridTables(int* pos_, double* late_, double* k_, int* n_ofdm_) : pos(pos_), late(late_), k(k_), n_ofdm(n_ofdm_), base(nullptr) {}
 };
 // The host geometry of extract_tfg (searcher.cpp:871-928) for one cell, into slot `slot` of g: pos / late and ts [n_ofdm]
 // of every DFT window, the FOC constant k and n_ofdm.  LCS_ERR_ARG (cp_type unknown, frame_start / freq_fine not finite)

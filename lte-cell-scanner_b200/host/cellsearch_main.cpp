@@ -56,6 +56,13 @@ static void print_usage() {
   cout << "     --measure                   add RSRP[dBFS] RSRQ[dB] SINR[dB] columns (antenna port 0) to the cell table," << endl;
   cout << "                                 measured on the GPU from the CRS of each cell's central 6 RBs over 60 ms of the" << endl;
   cout << "                                 capture (with --wideband, RSRP in the recording's full scale)" << endl;
+  cout << "     --measure-carrier           with --wideband: add RSRPc[dBFS] RSRQc[dB] SINRc[dB] columns (antenna port 0)," << endl;
+  cout << "                                 measured on the GPU from the CRS of all n_rb_dl RBs of each cell, taken from the" << endl;
+  cout << "                                 recording itself; --fs-in must be D * 1.92 MHz with D in {2, 4, 8, 16, 32}.  A" << endl;
+  cout << "                                 cell whose carrier the recording does not hold whole shows -" << endl;
+  cout << "     --carrier-csv OUT.csv       with --measure-carrier: one line per cell, port and RB," << endl;
+  cout << "                                 n_id_cell,fc_hz,port,rb,rsrp_dbfs,noise_dbfs,rssi_dbfs (- for a power <= 0:" << endl;
+  cout << "                                 an RB's noise estimate can come out zero or negative at high SNR)" << endl;
   cout << "  -r --record / -i --device-index need a live rtl-sdr dongle: not supported by this build" << endl;
 }
 
@@ -124,6 +131,15 @@ static const lcs_cell_meas* measurement_of(const Cell& c, double freq_start, con
   return nullptr;
 }
 
+// A power as dB for the carrier CSV, or "-" when it is not positive: an RB's noise is the difference of two near-equal
+// sums and can come out zero or negative at high SNR.
+static string csv_db(double v) {
+  if (!(v > 0)) return "-";
+  char b[32];
+  std::snprintf(b, sizeof(b), "%.17g", 10 * std::log10(v));
+  return b;
+}
+
 // 10 log10 of the power in the bins whose centre lies within n_rb_dl * 90 kHz of the cell's carrier fc_requested +
 // freq_superfine, in full-scale^2 (dBFS).
 static double carrier_power_dbfs(const vector<double>& psd, double fs_in, double fc_in, const Cell& c) {
@@ -142,8 +158,8 @@ int main(int argc, char* const argv[]) {
   bool save_cap = false, use_recorded_data = false, raw = false, batched = false;
   string data_dir = ".", wideband, format = "ci16";
   double fs_in = -1, fc_in = -1;
-  bool resample = false, measure = false;
-  string spectrum;
+  bool resample = false, measure = false, measure_carrier = false;
+  string spectrum, carrier_csv;
   long nfft = 4096;
   static struct option long_options[] = {
       {"help", no_argument, 0, 'h'},          {"verbose", no_argument, 0, 'v'},       {"brief", no_argument, 0, 'b'},
@@ -153,6 +169,7 @@ int main(int argc, char* const argv[]) {
       {"wideband", required_argument, 0, 'B'},   {"fs-in", required_argument, 0, 'F'},   {"fc-in", required_argument, 0, 'C'},
       {"resample", no_argument, 0, 'S'},         {"format", required_argument, 0, 'T'},
       {"spectrum", required_argument, 0, 'P'},   {"nfft", required_argument, 0, 'N'},   {"measure", no_argument, 0, 'M'},
+      {"measure-carrier", no_argument, 0, 'K'}, {"carrier-csv", required_argument, 0, 'V'},
       {0, 0, 0, 0}};
   for (;;) {
     int idx = 0;
@@ -180,6 +197,8 @@ int main(int argc, char* const argv[]) {
       case 'P': spectrum = optarg; break;
       case 'N': nfft = strtol(optarg, &endp, 10); if (optarg == endp || *endp) { cerr << "Error: could not parse --nfft" << endl; return -1; } break;
       case 'M': measure = true; break;
+      case 'K': measure_carrier = true; break;
+      case 'V': carrier_csv = optarg; break;
       case 'i': break;
       default: return -1;
     }
@@ -188,6 +207,9 @@ int main(int argc, char* const argv[]) {
   const bool spec = !spectrum.empty(), search = !spec || freq_start != -1;   // --spectrum alone: no search
   if (spec && wideband.empty()) { cerr << "Error: --spectrum needs --wideband" << endl; return -1; }
   if (measure && !search) { cerr << "Error: --measure needs a search (-s)" << endl; return -1; }
+  if (!carrier_csv.empty() && !measure_carrier) { cerr << "Error: --carrier-csv needs --measure-carrier" << endl; return -1; }
+  if (measure_carrier && wideband.empty()) { cerr << "Error: --measure-carrier needs --wideband" << endl; return -1; }
+  if (measure_carrier && !search) { cerr << "Error: --measure-carrier needs a search (-s)" << endl; return -1; }
   if (nfft < 64 || nfft > 65536 || (nfft & (nfft - 1))) { cerr << "Error: --nfft must be a power of two in [64, 65536]" << endl; return -1; }
   const bool wide = !wideband.empty();
   int wide_format = LCS_IQ_CI16;   // --format, for the spectrum and the search
@@ -250,6 +272,13 @@ int main(int argc, char* const argv[]) {
     } else {
       down = (uint32_t)std::lround(fs_in / 1.92e6);
     }
+    if (measure_carrier) {
+      const long D = std::lround(fs_in / 1.92e6);
+      if (!((D == 2 || D == 4 || D == 8 || D == 16 || D == 32) && std::fabs(fs_in - D * 1.92e6) <= 1e-6)) {
+        cerr << "Error: --measure-carrier needs --fs-in = D * 1.92 MHz with D in {2, 4, 8, 16, 32}" << endl;
+        return -1;
+      }
+    }
     const uint64_t M = (n_taps - 1) / 2;
     const int n_fc = (int)floor((freq_end - freq_start) / 100e3) + 1;                     // the raster of the search loop
     for (int fci = 0; fci < n_fc; fci++) {
@@ -274,6 +303,8 @@ int main(int argc, char* const argv[]) {
     }
   }
   if (spec && !(spec_file = open_output(spectrum))) return -1;
+  FILE* carrier_file = nullptr;
+  if (!carrier_csv.empty() && !(carrier_file = open_output(carrier_csv))) return -1;
   if (verbosity >= 1) {
     cout << "LTE CellSearch (GPU drop-in, " << lcs_version() << ") beginning" << endl;
     if (freq_start == freq_end) cout << "  Search frequency: " << freq_start / 1e6 << " MHz" << endl;
@@ -404,14 +435,34 @@ int main(int argc, char* const argv[]) {
     }
     list<Cell> cells_final;
     dedup(detected_cells, cells_final);
+    vector<lcs_carrier_meas> cmeas;   // --measure-carrier: that of the k-th final cell, if cok[k]
+    vector<bool> cok;
+    if (measure_carrier) {
+      measure_carriers(wide_iq.data(), wide_format, wide_n, fs_in, fc_in, vector<Cell>(cells_final.begin(), cells_final.end()),
+                       fs_programmed, cmeas, cok);
+      if (carrier_file) {
+        bool ok = std::fprintf(carrier_file, "n_id_cell,fc_hz,port,rb,rsrp_dbfs,noise_dbfs,rssi_dbfs\n") > 0;
+        size_t k = 0;
+        for (list<Cell>::iterator it = cells_final.begin(); it != cells_final.end(); ++it, ++k)
+          for (int p = 0; cok[k] && p < (int)(*it).n_ports; p++)
+            for (uint32_t b = 0; b < cmeas[k].n_rb; b++)
+              ok = ok && std::fprintf(carrier_file, "%d,%.17g,%d,%u,%s,%s,%s\n", (int)(*it).n_id_cell(), (*it).fc_requested, p,
+                                      b, csv_db(cmeas[k].rb_rsrp[p][b]).c_str(), csv_db(cmeas[k].rb_noise[p][b]).c_str(),
+                                      csv_db(cmeas[k].rb_rssi[b]).c_str()) > 0;
+        ok = std::fclose(carrier_file) == 0 && ok;
+        if (!ok) throw("cannot write the carrier CSV file");
+      }
+    }
     if (cells_final.size() == 0) {
       cout << "No LTE cells were found..." << endl;
     } else {   // CellSearch.cpp:579-613
       cout << "Detected the following cells:" << endl;
       cout << "A: #antenna ports C: CP type ; P: PHICH duration ; PR: PHICH resource type" << endl;
       cout << "CID A      fc   foff RXPWR C nRB P  PR CrystalCorrectionFactor" << (spec ? " CarrierPower[dBFS]" : "")
-           << (measure ? " RSRP[dBFS] RSRQ[dB] SINR[dB]" : "") << endl;
-      for (list<Cell>::iterator it = cells_final.begin(); it != cells_final.end(); ++it) {
+           << (measure ? " RSRP[dBFS] RSRQ[dB] SINR[dB]" : "") << (measure_carrier ? " RSRPc[dBFS] RSRQc[dB] SINRc[dB]" : "")
+           << endl;
+      size_t k = 0;
+      for (list<Cell>::iterator it = cells_final.begin(); it != cells_final.end(); ++it, ++k) {
         stringstream ss;
         ss << setw(3) << (*it).n_id_cell();
         ss << setw(2) << (int)(*it).n_ports;
@@ -437,6 +488,13 @@ int main(int argc, char* const argv[]) {
           if (!m) throw("--measure: a listed cell has no measurement");
           ss << " " << fixed << setprecision(2) << 10 * log10(m->rsrp[0]) << " " << 10 * log10(m->rsrq) << " "
              << 10 * log10(m->sinr[0]);
+        }
+        if (measure_carrier) {
+          if (cok[k])
+            ss << " " << fixed << setprecision(2) << 10 * log10(cmeas[k].rsrp[0]) << " " << 10 * log10(cmeas[k].rsrq) << " "
+               << 10 * log10(cmeas[k].sinr[0]);
+          else
+            ss << " - - -";
         }
         cout << ss.str() << endl;
       }

@@ -100,6 +100,29 @@ void measure_cells(const void* iq, int iq_format, uint32_t n_cap, const std::vec
   check(measure_lists(iq, iq_format, 0, n_cap, detected_cells, fs_programmed, meas, &where), where);
 }
 
+void measure_carriers(const void* iq, int iq_format, uint64_t n, double fs_in, double fc_in, const std::vector<Cell>& cells,
+                      const double& fs_programmed, std::vector<lcs_carrier_meas>& meas, std::vector<bool>& ok) {
+  std::vector<lcs_cell> flat;
+  for (const Cell& c : cells) flat.push_back(to_pod(c));
+  meas.assign(flat.size(), lcs_carrier_meas());
+  ok.assign(flat.size(), true);
+  if (flat.empty()) return;
+  lcs_carrier* h = nullptr;
+  check(lcs_carrier_create(lcs_dropin_ctx(), &h), "lcs_carrier_create");
+  lcs_status rc = lcs_carrier_cells(h, iq, iq_format, 0, n, fs_in, fc_in, flat.data(), (uint32_t)flat.size(), fs_programmed,
+                                    meas.data());
+  if (rc == LCS_ERR_ARG) {   // a cell was rejected: each on its own, so that only the rejected ones go unmeasured
+    rc = LCS_OK;
+    for (size_t i = 0; i < flat.size() && rc == LCS_OK; i++) {
+      const lcs_status r = lcs_carrier_cells(h, iq, iq_format, 0, n, fs_in, fc_in, &flat[i], 1, fs_programmed, &meas[i]);
+      ok[i] = r == LCS_OK;
+      if (r != LCS_ERR_ARG) rc = r;
+    }
+  }
+  lcs_carrier_destroy(h);
+  check(rc, "lcs_carrier_cells");
+}
+
 void sweep_search_cu8(const std::vector<unsigned char>& iq, uint32_t n_cap, const std::vector<double>& fc_requested,
                       const vec& f_search_set, const double& fs_programmed, std::vector<std::list<Cell> >& detected_cells) {
   const uint32_t n_ch = (uint32_t)fc_requested.size(), max_cells = 16;

@@ -1,6 +1,6 @@
-"""ctypes binding of liblcs_b200.so - the C ABI declared in include/lcs_b200.h - and of the two modules built on top of
-it: liblcs_psd.so, the Welch spectrum of include/lcs_psd.h, and liblcs_meas.so, the per-cell RSRP / RSRQ / SINR of
-include/lcs_meas.h.
+"""ctypes binding of liblcs_b200.so - the C ABI declared in include/lcs_b200.h - and of the three modules built on top of
+it: liblcs_psd.so, the Welch spectrum of include/lcs_psd.h, liblcs_meas.so, the per-cell RSRP / RSRQ / SINR of
+include/lcs_meas.h, and liblcs_carrier.so, the same over each cell's whole carrier, of include/lcs_carrier.h.
 
 This module is plumbing for tests/, bench.py and __graft_entry__.py: every call goes through the
 same `extern "C"` entry points a C++/IT++ host would bind (INTEGRATION.md).  lib() gives every
@@ -22,6 +22,8 @@ PSD_LIB_PATH = os.environ.get("LCS_PSD_LIB") or os.path.join(HERE, "liblcs_psd.s
 PSD_HEADER = os.path.join(HERE, "..", "include", "lcs_psd.h")
 MEAS_LIB_PATH = os.environ.get("LCS_MEAS_LIB") or os.path.join(HERE, "liblcs_meas.so")
 MEAS_HEADER = os.path.join(HERE, "..", "include", "lcs_meas.h")
+CARRIER_LIB_PATH = os.environ.get("LCS_CARRIER_LIB") or os.path.join(HERE, "liblcs_carrier.so")
+CARRIER_HEADER = os.path.join(HERE, "..", "include", "lcs_carrier.h")
 
 IQ_CF32, IQ_CU8, IQ_C128, IQ_CI16, IQ_CS8 = 0, 1, 2, 3, 4
 KERNEL_AUTO, KERNEL_FP32, KERNEL_TC = 0, 1, 2
@@ -128,6 +130,12 @@ def meas_lib():
     """liblcs_meas.so (include/lcs_meas.h); it takes the contexts of lib()."""
     lib()
     return _bind(MEAS_LIB_PATH, MEAS_HEADER)
+
+
+def carrier_lib():
+    """liblcs_carrier.so (include/lcs_carrier.h); it takes the contexts of lib()."""
+    lib()
+    return _bind(CARRIER_LIB_PATH, CARRIER_HEADER)
 
 
 def _p(a):
@@ -812,5 +820,55 @@ class CellMeasure(_Handle):
         self._iq = iq                                   # kept alive until the call has returned
         _chk(meas_lib().lcs_meas_cells(self._h, ptr, iq_format, on_device, shape[0], shape[1], arr, _p(chv), n,
                                        fs_programmed, _p(out)), self.ctx._h)
+        self._iq = None
+        return out
+
+
+# lcs_carrier_meas as a numpy record
+CARRIER_MEAS = np.dtype([("rsrp", np.float64, 4), ("noise", np.float64, 4), ("sinr", np.float64, 4), ("rssi", np.float64),
+                         ("rsrq", np.float64), ("rb_rsrp", np.float64, (4, 100)), ("rb_noise", np.float64, (4, 100)),
+                         ("rb_rssi", np.float64, 100), ("n_pairs", np.uint32, 4), ("n_rb", np.uint32)], align=True)
+CARRIER_CHUNK = 32                    # LCS_CARRIER_CHUNK: cells per chunk, two launches each
+
+
+class CarrierMeasure(_Handle):
+    """lcs_carrier: RSRP, RSRQ and SINR of found cells over all their resource blocks, and per resource block, measured on
+    the wideband recording they were found in (DESIGN.md section 4.10)."""
+    _destroy = "lcs_carrier_destroy"
+    _timing_read = "lcs_carrier_timing_read"
+    _lib = staticmethod(carrier_lib)
+
+    def __init__(self, ctx):
+        self.ctx = ctx
+        self._h = C.c_void_p()
+        _chk(carrier_lib().lcs_carrier_create(ctx._h, C.byref(self._h)), ctx._h)
+
+    def measure(self, iq, fmt, fs_in, fc_in, cells, fs_programmed):
+        """Measure `cells` (Cells, or any struct of lcs_cell's layout) in the recording iq [n_in][2] of format fmt (ci16,
+        cs8, cu8 or cf32; complex64 [n_in] is accepted for cf32) at fs_in, centred on fc_in.  iq may be a contiguous
+        CUDA tensor (read in place; its stream is synchronised first).  Returns a CARRIER_MEAS record array, one row per
+        cell."""
+        iq_format = _iq_format(fmt)
+        cells = list(cells)
+        n = len(cells)
+        arr = (Cell * max(n, 1))()
+        for i, c in enumerate(cells):
+            C.memmove(C.addressof(arr) + i * C.sizeof(Cell), C.byref(c), C.sizeof(Cell))
+        if hasattr(iq, "is_cuda"):
+            if not (iq.is_cuda and iq.is_contiguous()):
+                raise ValueError("measure: expected a contiguous CUDA tensor")
+            shape = tuple(iq.shape) + ((2,) if iq.is_complex() else ())
+            import torch
+            torch.cuda.current_stream(iq.device).synchronize()
+            ptr, on_device = iq.data_ptr(), 1
+        else:
+            iq = _samples(iq, fmt)
+            shape, ptr, on_device = iq.shape, iq.ctypes.data, 0
+        if len(shape) != 2 or shape[1] != 2:
+            raise ValueError("expected a recording [n_in][2]")
+        out = np.zeros(n, CARRIER_MEAS)
+        self._iq = iq                                   # kept alive until the call has returned
+        _chk(carrier_lib().lcs_carrier_cells(self._h, ptr, iq_format, on_device, shape[0], fs_in, fc_in, arr, n,
+                                             fs_programmed, _p(out)), self.ctx._h)
         self._iq = None
         return out

@@ -9,7 +9,15 @@ place, in one call, --reps times after a warm-up call.  One JSON line reports:
     RSSI resource elements read back), the achieved byte rate and the lower bound at 3.35 TB/s (H100 SXM data sheet);
   - the card name, power limit and SM clocks, read in the same run.
 
+With --carrier it times the full-carrier measurement (lcs_carrier_cells, DESIGN.md section 4.10) instead: a synthetic
+30.72 Msps ci16 recording with three 50-RB carriers of eight cells each, read in place from device memory, every cell
+measured --copies times in one call.  One JSON line reports the device time per cell (lcs_carrier_timing_read), the bytes
+the two kernels need per cell (the CRS windows' samples read, the 12 R grid columns of those windows written, and the CRS
+pairs and RSSI columns read back), the achieved byte rate, the lower bound at 3.35 TB/s, and the card, read in the same
+run.
+
 Usage: python tools/meas_bench.py [--channels 64] [--reps 20]
+       python tools/meas_bench.py --carrier [--copies 8] [--reps 20]
 """
 import argparse
 import json
@@ -50,11 +58,72 @@ def cell_bytes(c):
     return n_ofdm * 128 * 2 + n_ofdm * 72 * 16 + 2 * pairs * 16 + 244 * 72 * 16
 
 
+def gpu_name():
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"],
+                       capture_output=True, text=True).stdout.strip().splitlines()
+    return q[0] if q else "unknown"
+
+
+def carrier_bytes(c, D, esz=4):
+    """Bytes the two carrier kernels move for one cell: its CRS windows' N = 128 D samples, the 12 R grid columns of each
+    written (float2), and read back at the CRS pairs (two REs each) and the RSSI columns of the port-0 CRS symbols."""
+    R, nw = c.n_rb_dl, 3 if c.n_ports == 4 else 2
+    n_win = 122 * nw
+    pairs = sum([480 * R, 480 * R, 240 * R, 240 * R][:c.n_ports])
+    return n_win * 128 * D * esz + n_win * 12 * R * 8 + 2 * pairs * 8 + 244 * 12 * R * 8
+
+
+def carrier_main(a):
+    import torch
+    D, fs_in = 16, 16 * 1.92e6
+    carriers, cells = [], []
+    for j, off in enumerate((-10_000_000, 0, 10_000_000)):
+        cs = []
+        for i in range(8):
+            c = cell(3 * (8 * j + i) + i % 3, (1, 2, 4)[i % 3], 1 + (i % 4 == 3), 1000 + 517 * i)
+            c["n_rb_dl"] = 50
+            cs.append(c)
+        carriers.append((FC + off, cs))
+        for c in cs:
+            cells.append(L.new_cell(fc_requested=FC + off, fc_programmed=FC + off, n_id_1=c["n_id_cell"] // 3,
+                                    n_id_2=c["n_id_cell"] % 3, cp_type=c["cp_type"], n_ports=c["n_ports"],
+                                    frame_start=float(c["t0"]), freq_superfine=0.0, n_rb_dl=50))
+    x, _ = S.synth_wide_full(D * (5000 + 122 * 960 + 400), fs_in, FC, carriers, 30.0, 0)
+    iq = S.quantise(x, "ci16", 0.1 / np.sqrt(np.mean(np.abs(x) ** 2)))
+    cells = cells * a.copies
+    ctx = L.Context(0)
+    d_iq = torch.from_numpy(iq).cuda()
+    m = L.CarrierMeasure(ctx)
+    m.measure(d_iq, "ci16", fs_in, FC, cells, 1.92e6)              # warm-up
+    m.timing_read()
+    wall = []
+    for _ in range(a.reps):
+        t = time.perf_counter()
+        m.measure(d_iq, "ci16", fs_in, FC, cells, 1.92e6)
+        wall.append(time.perf_counter() - t)
+    ms, launches = m.timing_read()
+    m.close()
+    n = len(cells)
+    dev_s = ms / 1e3 / a.reps
+    bytes_ = sum(carrier_bytes(c, D) for c in cells)
+    print(json.dumps({
+        "carrier": True, "fs_in": fs_in, "cells": n, "reps": a.reps, "launches": launches,
+        "carrier_device_us_per_cell": 1e6 * dev_s / n, "carrier_host_us_per_cell": 1e6 * float(np.median(wall)) / n,
+        "carrier_bytes_per_cell": bytes_ / n, "carrier_gbytes_per_s": bytes_ / dev_s / 1e9,
+        "bound_hbm_us_per_cell": 1e6 * bytes_ / HBM_BPS / n, "gpu": gpu_name(),
+    }), flush=True)
+    ctx.close()
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--channels", type=int, default=64)
     ap.add_argument("--reps", type=int, default=20)
+    ap.add_argument("--carrier", action="store_true", help="time lcs_carrier_cells instead")
+    ap.add_argument("--copies", type=int, default=8, help="with --carrier: how often each of the 24 cells is measured per call")
     a = ap.parse_args()
+    if a.carrier:
+        return carrier_main(a)
     import torch
     bufs = [S.synth_cu8(153600, cs, fc=FC, snr_db=12.0, seed=i) for i, cs in enumerate(BUFFERS)]
     iq = np.stack([bufs[c % len(bufs)] for c in range(a.channels)])
@@ -83,14 +152,12 @@ def main():
     n = len(cells)
     dev_s = ms / 1e3 / a.reps
     bytes_ = sum(cell_bytes(c) for c in cells)
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True).stdout.strip().splitlines()
     print(json.dumps({
         "channels": a.channels, "cells": n, "reps": a.reps, "launches": launches,
         "meas_device_us_per_cell": 1e6 * dev_s / n, "meas_host_us_per_cell": 1e6 * float(np.median(wall)) / n,
         "search_host_us_per_cell": 1e6 * search_s / n, "search_host_ms": 1e3 * search_s,
         "meas_bytes_per_cell": bytes_ / n, "meas_gbytes_per_s": bytes_ / dev_s / 1e9,
-        "bound_hbm_us_per_cell": 1e6 * bytes_ / HBM_BPS / n, "gpu": q[0] if q else "unknown",
+        "bound_hbm_us_per_cell": 1e6 * bytes_ / HBM_BPS / n, "gpu": gpu_name(),
     }), flush=True)
     ctx.close()
 

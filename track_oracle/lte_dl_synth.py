@@ -218,3 +218,175 @@ def _eval_grid(Xc, n_symb, cp, rel):
 
 def to_c128(cu8):
     return ((cu8.astype(np.float64) - 127) / 128).view(np.complex128).reshape(-1)
+
+
+# ---- full-bandwidth carriers --------------------------------------------------------------------------------------------
+def crs_full(n_id_cell, cp_type, n_rb_dl):
+    """The CRS of all n_rb_dl RBs (36.211 6.10.1.1): [20 slots][n_symb][2 n_rb_dl], r(m') with m' = 110 - n_rb_dl + m;
+    rows of symbols without CRS are 0.  The subcarrier of r[.., m] for port p is 6 m + shift (O.rs_dl's shift table)."""
+    n_symb = 7 if cp_type == 1 else 6
+    n_cp = 1 if cp_type == 1 else 0
+    m = 110 - n_rb_dl + np.arange(2 * n_rb_dl)
+    r = np.zeros((20, n_symb, 2 * n_rb_dl), complex)
+    for slot in range(20):
+        for sym in (0, 1, n_symb - 3):
+            c = O.lte_pn((1 << 10) * (7 * (slot + 1) + sym + 1) * (2 * n_id_cell + 1) + 2 * n_id_cell + n_cp, 440)
+            r[slot, sym] = ((1 - 2 * c[2 * m].astype(float)) + 1j * (1 - 2 * c[2 * m + 1].astype(float))) / np.sqrt(2)
+    return r
+
+
+def subcarriers(n_rb_dl):
+    """Subcarrier number of each grid column c < 12 n_rb_dl: c - 6R below DC, c - 6R + 1 above (DC skipped)."""
+    R = n_rb_dl
+    return np.concatenate([np.arange(-6 * R, 0), np.arange(1, 6 * R + 1)])
+
+
+def _grid_full(cell, n_frames, rng):
+    """Transmitted grid of all n_rb_dl RBs per port, [n_ports][n_sym][12 R]: the 6-RB content of _grid in the centre,
+    full-band CRS, and QPSK times sqrt(cell["load"]) (default 1) on port 0 on every other RE outside the centre."""
+    R, P, cp = cell["n_rb_dl"], cell["n_ports"], cell["cp_type"]
+    X6, n_symb = _grid(cell, n_frames, cell.get("sfn0", 0), rng)
+    n_sym = X6.shape[1]
+    X = np.zeros((P, n_sym, 12 * R), complex)
+    load = np.sqrt(cell.get("load", 1.0))
+    X[0] = load * ((1 - 2 * rng.integers(0, 2, (n_sym, 12 * R))) + 1j * (1 - 2 * rng.integers(0, 2, (n_sym, 12 * R)))) / np.sqrt(2)
+    rs = crs_full(cell["n_id_cell"], cp, R)
+    _, shift = O.rs_dl(cell["n_id_cell"], cp)
+    for g in range(n_sym):
+        slot, sym = (g // n_symb) % 20, g % n_symb
+        for p in range(P):
+            sh = shift[slot * n_symb + sym, p]
+            if np.isnan(sh):
+                continue
+            idx = int(sh) + 6 * np.arange(2 * R)
+            X[:, g, idx] = 0
+            X[p, g, idx] = rs[slot, sym]
+    X[:, :, 6 * R - 36:6 * R + 36] = X6
+    return X, n_symb
+
+
+def channel_response(paths, f):
+    """H(f) of the paths [(delay_s, complex_gain), ...] at the frequencies f (Hz)."""
+    return sum(g * np.exp(-2j * np.pi * np.asarray(f) * d) for d, g in paths)
+
+
+def synth_wide_full(n, fs_in, fc_in, carriers, snr_db=30.0, seed=0):
+    """A wideband recording at the nominal clock as complex128 [n] in full-scale units: LTE carriers of all their RBs.
+
+    carriers: list of (fc_c, cells); fc_c - fc_in an integer number of Hz, fs_in = D * 1.92 MHz.  Each cell as in
+    synth_cu8 plus n_rb_dl RBs of content (_grid_full), an integer t0, optional `paths` [(delay_s, gain)] (each symbol's
+    subcarriers times H(f); exact while the delays stay inside the cyclic prefix) and an optional `interferer`
+    (rb_lo, rb_hi, power): complex Gaussian noise of power power * AMP^2 per RE on RBs [rb_lo, rb_hi) of the cell.
+    Every OFDM symbol is built by one N = 128 D point inverse FFT and its cyclic prefix, which is exact at these rates.
+    AWGN of variance D * AMP^2 / 10^(snr_db/10) over the band gives each RE the SNR snr_db.  Returns (x, grids):
+    grids[i] is the received grid [n_sym][12 R] of the i-th cell (port gains, channel and interferer applied, AMP
+    included, noise excluded), row 0 the frame starting at t0."""
+    rng = np.random.default_rng(seed)
+    D = int(round(fs_in / FS_LTE16))
+    N, fs = 128 * D, int(round(fs_in))
+    x = np.zeros(n, complex)
+    grids = []
+    for fc_c, cells in carriers:
+        delta = int(round(fc_c - fc_in))
+        xc = np.zeros(n, complex)
+        for cell in cells:
+            R, cp = cell["n_rb_dl"], cell["cp_type"]
+            start = D * int(cell["t0"])
+            n_frames = -(-(n - start) // (D * FRAME))
+            X, n_symb = _grid_full(cell, n_frames, rng)
+            gains = cell.get("gains", [1.0, 0.8 * np.exp(0.7j), 0.9 * np.exp(-1.1j), 0.7 * np.exp(2.2j)])[:cell["n_ports"]]
+            Y = AMP * np.tensordot(np.asarray(gains), X, axes=1)
+            k = subcarriers(R)
+            if "paths" in cell:
+                Y = Y * channel_response(cell["paths"], k * 15e3)[None, :]
+            if "interferer" in cell:
+                lo, hi, pw = cell["interferer"]
+                cols = slice(12 * lo, 12 * hi)
+                sh = (Y.shape[0], 12 * (hi - lo))
+                Y[:, cols] += AMP * np.sqrt(pw / 2) * (rng.standard_normal(sh) + 1j * rng.standard_normal(sh))
+            grids.append(Y)
+            V = np.zeros((Y.shape[0], N), complex)
+            V[:, k % N] = Y
+            u = np.fft.ifft(V, axis=1) * (N / np.sqrt(128))
+            pos = start
+            for g in range(Y.shape[0]):
+                sym = g % n_symb
+                ncp = D * (32 if cp == 2 else (10 if sym == 0 else 9))
+                seg = np.concatenate([u[g, N - ncp:], u[g]])
+                m = min(seg.size, n - pos)
+                if m <= 0:
+                    break
+                xc[pos:pos + m] += seg[:m]
+                pos += seg.size
+        p = (np.arange(n, dtype=np.int64) * (delta % fs)) % fs
+        x += xc * np.exp(2j * np.pi * p / fs)
+    sigma2 = D * AMP ** 2 / 10 ** (snr_db / 10)
+    x += np.sqrt(sigma2 / 2) * (rng.standard_normal(n) + 1j * rng.standard_normal(n))
+    return x, grids
+
+
+def quantise(x, fmt, scale):
+    """x * scale (full-scale units) as [n][2] samples of fmt: ci16 (/32768), cs8 (/128), cu8 ((v - 127) / 128) or cf32."""
+    v = np.stack([x.real, x.imag], axis=1) * scale
+    if fmt == "ci16":
+        return np.clip(np.rint(v * 32768), -32768, 32767).astype(np.int16)
+    if fmt == "cs8":
+        return np.clip(np.rint(v * 128), -128, 127).astype(np.int8)
+    if fmt == "cu8":
+        return np.clip(np.rint(v * 128 + 127), 0, 255).astype(np.uint8)
+    return v.astype(np.float32)
+
+
+def dequantise(iq, fmt):
+    """The samples of quantise() as complex128 in full-scale units, as the device reads them."""
+    v = iq.astype(np.float64)
+    v = {"ci16": v / 32768, "cs8": v / 128, "cu8": (v - 127) / 128, "cf32": v}[fmt]
+    return v[:, 0] + 1j * v[:, 1]
+
+
+def _eval_grid_full(Xc, n_symb, cp, rel, n_rb_dl):
+    """_eval_grid for a grid of all n_rb_dl RBs, Xc [n_sym][12 R]: the OFDM signal at rel (LTE samples after the cell's
+    frame start, any real value), evaluated directly; 0 outside the grid."""
+    x = np.zeros(rel.size, complex)
+    fr = np.floor(rel / FRAME)
+    p = rel - fr * FRAME
+    slot = np.floor(p / 960)
+    q = p - slot * 960
+    if cp == 1:
+        sym = np.where(q < 138, 0, 1 + np.floor((q - 138) / 137))
+        d = q - np.where(sym == 0, 0, 138 + (sym - 1) * 137) - np.where(sym == 0, 10, 9)
+    else:
+        sym = np.floor(q / 160)
+        d = q - sym * 160 - 32
+    g = (((fr + 1) * 20 + slot) * n_symb + sym).astype(np.int64) - 20 * n_symb
+    ok = (g >= 0) & (g < Xc.shape[0])
+    cn = subcarriers(n_rb_dl)
+    for c0 in range(0, rel.size, 8192):
+        sl = slice(c0, min(c0 + 8192, rel.size))
+        gg = np.where(ok[sl], g[sl], 0)
+        v = np.einsum("ij,ij->i", Xc[gg], np.exp(2j * np.pi * np.outer(d[sl], cn) / 128)) / np.sqrt(128)
+        x[sl] = np.where(ok[sl], v, 0)
+    return x
+
+
+def synth_wide_offset(n, fs_in, fc_in, fc_c, cell, clock_ratio, f_res, snr_db=30.0, seed=0):
+    """One cell of all its RBs in a wideband recording whose sample clock is off, by direct evaluation (the slow path,
+    for small cases).  Sample m is taken at t_m = m / (fs_in * clock_ratio); the carrier at fc_c (fc_c - fc_in an integer
+    number of Hz) turns by the exact nominal mixer phase (m (fc_c - fc_in) mod fs_in) / fs_in and by f_res t_m, so that
+    after the nominal mixer it sits f_res off with its clock clock_ratio times fast.  The search reports such a cell with
+    freq_superfine = f_res, fc_programmed = (fc_c - f_res) / clock_ratio (so k_factor = clock_ratio) and frame_start =
+    t0 * clock_ratio; t0 may be fractional.  AWGN as in synth_wide_full.  Returns (x complex128 [n], received grid)."""
+    rng = np.random.default_rng(seed)
+    D = int(round(fs_in / FS_LTE16))
+    fs, delta = int(round(fs_in)), int(round(fc_c - fc_in))
+    t = np.arange(n) / (fs_in * clock_ratio)
+    rel = t * FS_LTE16 - cell["t0"]
+    X, n_symb = _grid_full(cell, int(np.ceil((rel.max() + 1) / FRAME)) + 1, rng)
+    gains = cell.get("gains", [1.0, 0.8 * np.exp(0.7j), 0.9 * np.exp(-1.1j), 0.7 * np.exp(2.2j)])[:cell["n_ports"]]
+    Y = AMP * np.tensordot(np.asarray(gains), X, axes=1)
+    p = (np.arange(n, dtype=np.int64) * (delta % fs)) % fs
+    x = _eval_grid_full(Y, n_symb, cell["cp_type"], rel, cell["n_rb_dl"]) * np.exp(2j * np.pi * p / fs)
+    x *= np.exp(2j * np.pi * f_res * t)
+    sigma2 = D * AMP ** 2 / 10 ** (snr_db / 10)
+    x += np.sqrt(sigma2 / 2) * (rng.standard_normal(n) + 1j * rng.standard_normal(n))
+    return x, Y
