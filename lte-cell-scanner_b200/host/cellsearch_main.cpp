@@ -63,6 +63,13 @@ static void print_usage() {
   cout << "     --carrier-csv OUT.csv       with --measure-carrier: one line per cell, port and RB," << endl;
   cout << "                                 n_id_cell,fc_hz,port,rb,rsrp_dbfs,noise_dbfs,rssi_dbfs (- for a power <= 0:" << endl;
   cout << "                                 an RB's noise estimate can come out zero or negative at high SNR)" << endl;
+  cout << "     --cir                       with --wideband: add TOA[us] DS[ns] columns, the arrival of each cell's frame" << endl;
+  cout << "                                 (its first path, modulo 10 ms, from the recording's first sample) and the RMS" << endl;
+  cout << "                                 delay spread of antenna port 0, from the power delay profile of all n_rb_dl RBs" << endl;
+  cout << "                                 of the cell, taken from the recording itself; --fs-in as for --measure-carrier." << endl;
+  cout << "                                 A cell whose carrier the recording does not hold whole shows -" << endl;
+  cout << "     --cir-csv OUT.csv           with --cir: the power delay profile, one line per cell, port and delay tap," << endl;
+  cout << "                                 n_id_cell,fc_hz,port,delay_ns,pdp_dbfs (- for a power <= 0)" << endl;
   cout << "  -r --record / -i --device-index need a live rtl-sdr dongle: not supported by this build" << endl;
 }
 
@@ -158,8 +165,8 @@ int main(int argc, char* const argv[]) {
   bool save_cap = false, use_recorded_data = false, raw = false, batched = false;
   string data_dir = ".", wideband, format = "ci16";
   double fs_in = -1, fc_in = -1;
-  bool resample = false, measure = false, measure_carrier = false;
-  string spectrum, carrier_csv;
+  bool resample = false, measure = false, measure_carrier = false, cir = false;
+  string spectrum, carrier_csv, cir_csv;
   long nfft = 4096;
   static struct option long_options[] = {
       {"help", no_argument, 0, 'h'},          {"verbose", no_argument, 0, 'v'},       {"brief", no_argument, 0, 'b'},
@@ -170,6 +177,7 @@ int main(int argc, char* const argv[]) {
       {"resample", no_argument, 0, 'S'},         {"format", required_argument, 0, 'T'},
       {"spectrum", required_argument, 0, 'P'},   {"nfft", required_argument, 0, 'N'},   {"measure", no_argument, 0, 'M'},
       {"measure-carrier", no_argument, 0, 'K'}, {"carrier-csv", required_argument, 0, 'V'},
+      {"cir", no_argument, 0, 'X'},             {"cir-csv", required_argument, 0, 'Y'},
       {0, 0, 0, 0}};
   for (;;) {
     int idx = 0;
@@ -199,6 +207,8 @@ int main(int argc, char* const argv[]) {
       case 'M': measure = true; break;
       case 'K': measure_carrier = true; break;
       case 'V': carrier_csv = optarg; break;
+      case 'X': cir = true; break;
+      case 'Y': cir_csv = optarg; break;
       case 'i': break;
       default: return -1;
     }
@@ -210,6 +220,9 @@ int main(int argc, char* const argv[]) {
   if (!carrier_csv.empty() && !measure_carrier) { cerr << "Error: --carrier-csv needs --measure-carrier" << endl; return -1; }
   if (measure_carrier && wideband.empty()) { cerr << "Error: --measure-carrier needs --wideband" << endl; return -1; }
   if (measure_carrier && !search) { cerr << "Error: --measure-carrier needs a search (-s)" << endl; return -1; }
+  if (!cir_csv.empty() && !cir) { cerr << "Error: --cir-csv needs --cir" << endl; return -1; }
+  if (cir && wideband.empty()) { cerr << "Error: --cir needs --wideband" << endl; return -1; }
+  if (cir && !search) { cerr << "Error: --cir needs a search (-s)" << endl; return -1; }
   if (nfft < 64 || nfft > 65536 || (nfft & (nfft - 1))) { cerr << "Error: --nfft must be a power of two in [64, 65536]" << endl; return -1; }
   const bool wide = !wideband.empty();
   int wide_format = LCS_IQ_CI16;   // --format, for the spectrum and the search
@@ -272,10 +285,11 @@ int main(int argc, char* const argv[]) {
     } else {
       down = (uint32_t)std::lround(fs_in / 1.92e6);
     }
-    if (measure_carrier) {
+    if (measure_carrier || cir) {
       const long D = std::lround(fs_in / 1.92e6);
       if (!((D == 2 || D == 4 || D == 8 || D == 16 || D == 32) && std::fabs(fs_in - D * 1.92e6) <= 1e-6)) {
-        cerr << "Error: --measure-carrier needs --fs-in = D * 1.92 MHz with D in {2, 4, 8, 16, 32}" << endl;
+        cerr << "Error: " << (measure_carrier ? "--measure-carrier" : "--cir")
+             << " needs --fs-in = D * 1.92 MHz with D in {2, 4, 8, 16, 32}" << endl;
         return -1;
       }
     }
@@ -305,6 +319,8 @@ int main(int argc, char* const argv[]) {
   if (spec && !(spec_file = open_output(spectrum))) return -1;
   FILE* carrier_file = nullptr;
   if (!carrier_csv.empty() && !(carrier_file = open_output(carrier_csv))) return -1;
+  FILE* cir_file = nullptr;
+  if (!cir_csv.empty() && !(cir_file = open_output(cir_csv))) return -1;
   if (verbosity >= 1) {
     cout << "LTE CellSearch (GPU drop-in, " << lcs_version() << ") beginning" << endl;
     if (freq_start == freq_end) cout << "  Search frequency: " << freq_start / 1e6 << " MHz" << endl;
@@ -453,6 +469,23 @@ int main(int argc, char* const argv[]) {
         if (!ok) throw("cannot write the carrier CSV file");
       }
     }
+    vector<lcs_cir_meas> tmeas;   // --cir: that of the k-th final cell, if tok[k]
+    vector<bool> tok;
+    if (cir) {
+      measure_cirs(wide_iq.data(), wide_format, wide_n, fs_in, fc_in, vector<Cell>(cells_final.begin(), cells_final.end()),
+                   fs_programmed, tmeas, tok);
+      if (cir_file) {
+        bool ok = std::fprintf(cir_file, "n_id_cell,fc_hz,port,delay_ns,pdp_dbfs\n") > 0;
+        size_t k = 0;
+        for (list<Cell>::iterator it = cells_final.begin(); it != cells_final.end(); ++it, ++k)
+          for (int p = 0; tok[k] && p < (int)(*it).n_ports; p++)
+            for (int j = 0; j < LCS_CIR_TAPS; j++)
+              ok = ok && std::fprintf(cir_file, "%d,%.17g,%d,%.17g,%s\n", (int)(*it).n_id_cell(), (*it).fc_requested, p,
+                                      (j - 64) * 1e9 / 30.72e6, csv_db(tmeas[k].pdp[p][j]).c_str()) > 0;
+        ok = std::fclose(cir_file) == 0 && ok;
+        if (!ok) throw("cannot write the CIR CSV file");
+      }
+    }
     if (cells_final.size() == 0) {
       cout << "No LTE cells were found..." << endl;
     } else {   // CellSearch.cpp:579-613
@@ -460,7 +493,7 @@ int main(int argc, char* const argv[]) {
       cout << "A: #antenna ports C: CP type ; P: PHICH duration ; PR: PHICH resource type" << endl;
       cout << "CID A      fc   foff RXPWR C nRB P  PR CrystalCorrectionFactor" << (spec ? " CarrierPower[dBFS]" : "")
            << (measure ? " RSRP[dBFS] RSRQ[dB] SINR[dB]" : "") << (measure_carrier ? " RSRPc[dBFS] RSRQc[dB] SINRc[dB]" : "")
-           << endl;
+           << (cir ? " TOA[us] DS[ns]" : "") << endl;
       size_t k = 0;
       for (list<Cell>::iterator it = cells_final.begin(); it != cells_final.end(); ++it, ++k) {
         stringstream ss;
@@ -495,6 +528,13 @@ int main(int argc, char* const argv[]) {
                << 10 * log10(cmeas[k].sinr[0]);
           else
             ss << " - - -";
+        }
+        if (cir) {
+          if (tok[k])
+            ss << " " << fixed << setprecision(3) << 1e6 * std::fmod(tmeas[k].frame_arrival, 10e-3) << " " << setprecision(1)
+               << 1e9 * tmeas[k].rms_spread[0];
+          else
+            ss << " - -";
         }
         cout << ss.str() << endl;
       }

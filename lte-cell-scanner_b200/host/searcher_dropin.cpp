@@ -100,27 +100,43 @@ void measure_cells(const void* iq, int iq_format, uint32_t n_cap, const std::vec
   check(measure_lists(iq, iq_format, 0, n_cap, detected_cells, fs_programmed, meas, &where), where);
 }
 
-void measure_carriers(const void* iq, int iq_format, uint64_t n, double fs_in, double fc_in, const std::vector<Cell>& cells,
-                      const double& fs_programmed, std::vector<lcs_carrier_meas>& meas, std::vector<bool>& ok) {
+// One measurement of the wideband recording (lcs_carrier_cells or lcs_cir_cells, through handle type H) of every cell of
+// `cells`: all in one call, and when a cell is rejected each on its own, so that only the rejected ones go unmeasured.
+template <class H, class M, class Create, class Cells, class Destroy>
+static void measure_recording(Create create, Cells cells_fn, Destroy destroy, const char* what, const void* iq, int iq_format,
+                              uint64_t n, double fs_in, double fc_in, const std::vector<Cell>& cells,
+                              const double& fs_programmed, std::vector<M>& meas, std::vector<bool>& ok) {
   std::vector<lcs_cell> flat;
   for (const Cell& c : cells) flat.push_back(to_pod(c));
-  meas.assign(flat.size(), lcs_carrier_meas());
+  meas.assign(flat.size(), M());
   ok.assign(flat.size(), true);
   if (flat.empty()) return;
-  lcs_carrier* h = nullptr;
-  check(lcs_carrier_create(lcs_dropin_ctx(), &h), "lcs_carrier_create");
-  lcs_status rc = lcs_carrier_cells(h, iq, iq_format, 0, n, fs_in, fc_in, flat.data(), (uint32_t)flat.size(), fs_programmed,
-                                    meas.data());
-  if (rc == LCS_ERR_ARG) {   // a cell was rejected: each on its own, so that only the rejected ones go unmeasured
+  H* h = nullptr;
+  check(create(lcs_dropin_ctx(), &h), (std::string(what) + "_create").c_str());
+  lcs_status rc = cells_fn(h, iq, iq_format, 0, n, fs_in, fc_in, flat.data(), (uint32_t)flat.size(), fs_programmed,
+                           meas.data());
+  if (rc == LCS_ERR_ARG) {
     rc = LCS_OK;
     for (size_t i = 0; i < flat.size() && rc == LCS_OK; i++) {
-      const lcs_status r = lcs_carrier_cells(h, iq, iq_format, 0, n, fs_in, fc_in, &flat[i], 1, fs_programmed, &meas[i]);
+      const lcs_status r = cells_fn(h, iq, iq_format, 0, n, fs_in, fc_in, &flat[i], 1, fs_programmed, &meas[i]);
       ok[i] = r == LCS_OK;
       if (r != LCS_ERR_ARG) rc = r;
     }
   }
-  lcs_carrier_destroy(h);
-  check(rc, "lcs_carrier_cells");
+  destroy(h);
+  check(rc, (std::string(what) + "_cells").c_str());
+}
+
+void measure_carriers(const void* iq, int iq_format, uint64_t n, double fs_in, double fc_in, const std::vector<Cell>& cells,
+                      const double& fs_programmed, std::vector<lcs_carrier_meas>& meas, std::vector<bool>& ok) {
+  measure_recording<lcs_carrier>(lcs_carrier_create, lcs_carrier_cells, lcs_carrier_destroy, "lcs_carrier", iq, iq_format, n,
+                                 fs_in, fc_in, cells, fs_programmed, meas, ok);
+}
+
+void measure_cirs(const void* iq, int iq_format, uint64_t n, double fs_in, double fc_in, const std::vector<Cell>& cells,
+                  const double& fs_programmed, std::vector<lcs_cir_meas>& meas, std::vector<bool>& ok) {
+  measure_recording<lcs_cir>(lcs_cir_create, lcs_cir_cells, lcs_cir_destroy, "lcs_cir", iq, iq_format, n, fs_in, fc_in, cells,
+                             fs_programmed, meas, ok);
 }
 
 void sweep_search_cu8(const std::vector<unsigned char>& iq, uint32_t n_cap, const std::vector<double>& fc_requested,

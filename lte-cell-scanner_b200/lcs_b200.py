@@ -1,6 +1,7 @@
 """ctypes binding of liblcs_b200.so - the C ABI declared in include/lcs_b200.h - and of the three modules built on top of
 it: liblcs_psd.so, the Welch spectrum of include/lcs_psd.h, liblcs_meas.so, the per-cell RSRP / RSRQ / SINR of
-include/lcs_meas.h, and liblcs_carrier.so, the same over each cell's whole carrier, of include/lcs_carrier.h.
+include/lcs_meas.h, liblcs_carrier.so, the same over each cell's whole carrier, of include/lcs_carrier.h, and
+liblcs_cir.so, the power delay profile of each cell over its whole carrier, of include/lcs_cir.h.
 
 This module is plumbing for tests/, bench.py and __graft_entry__.py: every call goes through the
 same `extern "C"` entry points a C++/IT++ host would bind (INTEGRATION.md).  lib() gives every
@@ -24,6 +25,8 @@ MEAS_LIB_PATH = os.environ.get("LCS_MEAS_LIB") or os.path.join(HERE, "liblcs_mea
 MEAS_HEADER = os.path.join(HERE, "..", "include", "lcs_meas.h")
 CARRIER_LIB_PATH = os.environ.get("LCS_CARRIER_LIB") or os.path.join(HERE, "liblcs_carrier.so")
 CARRIER_HEADER = os.path.join(HERE, "..", "include", "lcs_carrier.h")
+CIR_LIB_PATH = os.environ.get("LCS_CIR_LIB") or os.path.join(HERE, "liblcs_cir.so")
+CIR_HEADER = os.path.join(HERE, "..", "include", "lcs_cir.h")
 
 IQ_CF32, IQ_CU8, IQ_C128, IQ_CI16, IQ_CS8 = 0, 1, 2, 3, 4
 KERNEL_AUTO, KERNEL_FP32, KERNEL_TC = 0, 1, 2
@@ -136,6 +139,12 @@ def carrier_lib():
     """liblcs_carrier.so (include/lcs_carrier.h); it takes the contexts of lib()."""
     lib()
     return _bind(CARRIER_LIB_PATH, CARRIER_HEADER)
+
+
+def cir_lib():
+    """liblcs_cir.so (include/lcs_cir.h); it takes the contexts of lib()."""
+    lib()
+    return _bind(CIR_LIB_PATH, CIR_HEADER)
 
 
 def _p(a):
@@ -824,6 +833,34 @@ class CellMeasure(_Handle):
         return out
 
 
+def _measure_recording(h, fn, dtype, iq, fmt, fs_in, fc_in, cells, fs_programmed):
+    """fn (lcs_carrier_cells or lcs_cir_cells) of handle h on the recording iq: a record array of dtype, one row per
+    cell."""
+    iq_format = _iq_format(fmt)
+    cells = list(cells)
+    n = len(cells)
+    arr = (Cell * max(n, 1))()
+    for i, c in enumerate(cells):
+        C.memmove(C.addressof(arr) + i * C.sizeof(Cell), C.byref(c), C.sizeof(Cell))
+    if hasattr(iq, "is_cuda"):
+        if not (iq.is_cuda and iq.is_contiguous()):
+            raise ValueError("measure: expected a contiguous CUDA tensor")
+        shape = tuple(iq.shape) + ((2,) if iq.is_complex() else ())
+        import torch
+        torch.cuda.current_stream(iq.device).synchronize()
+        ptr, on_device = iq.data_ptr(), 1
+    else:
+        iq = _samples(iq, fmt)
+        shape, ptr, on_device = iq.shape, iq.ctypes.data, 0
+    if len(shape) != 2 or shape[1] != 2:
+        raise ValueError("expected a recording [n_in][2]")
+    out = np.zeros(n, dtype)
+    h._iq = iq                                          # kept alive until the call has returned
+    _chk(fn(h._h, ptr, iq_format, on_device, shape[0], fs_in, fc_in, arr, n, fs_programmed, _p(out)), h.ctx._h)
+    h._iq = None
+    return out
+
+
 # lcs_carrier_meas as a numpy record
 CARRIER_MEAS = np.dtype([("rsrp", np.float64, 4), ("noise", np.float64, 4), ("sinr", np.float64, 4), ("rssi", np.float64),
                          ("rsrq", np.float64), ("rb_rsrp", np.float64, (4, 100)), ("rb_noise", np.float64, (4, 100)),
@@ -848,27 +885,36 @@ class CarrierMeasure(_Handle):
         cs8, cu8 or cf32; complex64 [n_in] is accepted for cf32) at fs_in, centred on fc_in.  iq may be a contiguous
         CUDA tensor (read in place; its stream is synchronised first).  Returns a CARRIER_MEAS record array, one row per
         cell."""
-        iq_format = _iq_format(fmt)
-        cells = list(cells)
-        n = len(cells)
-        arr = (Cell * max(n, 1))()
-        for i, c in enumerate(cells):
-            C.memmove(C.addressof(arr) + i * C.sizeof(Cell), C.byref(c), C.sizeof(Cell))
-        if hasattr(iq, "is_cuda"):
-            if not (iq.is_cuda and iq.is_contiguous()):
-                raise ValueError("measure: expected a contiguous CUDA tensor")
-            shape = tuple(iq.shape) + ((2,) if iq.is_complex() else ())
-            import torch
-            torch.cuda.current_stream(iq.device).synchronize()
-            ptr, on_device = iq.data_ptr(), 1
-        else:
-            iq = _samples(iq, fmt)
-            shape, ptr, on_device = iq.shape, iq.ctypes.data, 0
-        if len(shape) != 2 or shape[1] != 2:
-            raise ValueError("expected a recording [n_in][2]")
-        out = np.zeros(n, CARRIER_MEAS)
-        self._iq = iq                                   # kept alive until the call has returned
-        _chk(carrier_lib().lcs_carrier_cells(self._h, ptr, iq_format, on_device, shape[0], fs_in, fc_in, arr, n,
-                                             fs_programmed, _p(out)), self.ctx._h)
-        self._iq = None
-        return out
+        return _measure_recording(self, carrier_lib().lcs_carrier_cells, CARRIER_MEAS, iq, fmt, fs_in, fc_in, cells,
+                                  fs_programmed)
+
+
+# lcs_cir_meas as a numpy record
+CIR_TAPS = 320                        # LCS_CIR_TAPS: tap j is (j - 64) / 30.72 MHz
+CIR_MEAS = np.dtype([("pdp", np.float64, (4, CIR_TAPS)), ("floor", np.float64, 4), ("peak_delay", np.float64, 4),
+                     ("first_delay", np.float64, 4), ("mean_delay", np.float64, 4), ("rms_spread", np.float64, 4),
+                     ("frame_arrival", np.float64), ("n_pairs", np.uint32, 4), ("n_taps", np.uint32, 4)], align=True)
+CIR_CHUNK = 32                        # LCS_CIR_CHUNK: cells per chunk, two launches each
+
+
+def cir_delays():
+    """The delay of every tap of CIR_MEAS.pdp, seconds."""
+    return (np.arange(CIR_TAPS) - 64) * (1 / 30.72e6)
+
+
+class CellImpulse(_Handle):
+    """lcs_cir: the power delay profile of found cells over their whole carrier, with its first-path and peak delay, mean
+    delay, RMS delay spread and the frame's arrival time, measured on the wideband recording they were found in (DESIGN.md
+    section 4.11)."""
+    _destroy = "lcs_cir_destroy"
+    _timing_read = "lcs_cir_timing_read"
+    _lib = staticmethod(cir_lib)
+
+    def __init__(self, ctx):
+        self.ctx = ctx
+        self._h = C.c_void_p()
+        _chk(cir_lib().lcs_cir_create(ctx._h, C.byref(self._h)), ctx._h)
+
+    def measure(self, iq, fmt, fs_in, fc_in, cells, fs_programmed):
+        """As CarrierMeasure.measure; returns a CIR_MEAS record array, one row per cell."""
+        return _measure_recording(self, cir_lib().lcs_cir_cells, CIR_MEAS, iq, fmt, fs_in, fc_in, cells, fs_programmed)

@@ -16,8 +16,14 @@ the two kernels need per cell (the CRS windows' samples read, the 12 R grid colu
 pairs and RSSI columns read back), the achieved byte rate, the lower bound at 3.35 TB/s, and the card, read in the same
 run.
 
+With --cir it times the power delay profile (lcs_cir_cells, DESIGN.md section 4.11) on the same recording and cells in
+the same way: one JSON line with the device time per cell (lcs_cir_timing_read), the complex multiply-adds of the delay
+transform per cell (2 R CRS x 320 taps for every CRS symbol of every port), their FP64 rate, and the card, read in the
+same run.
+
 Usage: python tools/meas_bench.py [--channels 64] [--reps 20]
        python tools/meas_bench.py --carrier [--copies 8] [--reps 20]
+       python tools/meas_bench.py --cir [--copies 8] [--reps 20]
 """
 import argparse
 import json
@@ -73,6 +79,12 @@ def carrier_bytes(c, D, esz=4):
     return n_win * 128 * D * esz + n_win * 12 * R * 8 + 2 * pairs * 8 + 244 * 12 * R * 8
 
 
+def cir_macs(c):
+    """Complex multiply-adds of cir_kernel's transform for one cell: 2 R CRS times 320 taps in each of the 244 symbols of
+    ports 0 and 1 and the 122 of ports 2 and 3."""
+    return sum([244, 244, 122, 122][:c.n_ports]) * 2 * c.n_rb_dl * 320
+
+
 def carrier_main(a):
     import torch
     D, fs_in = 16, 16 * 1.92e6
@@ -93,7 +105,7 @@ def carrier_main(a):
     cells = cells * a.copies
     ctx = L.Context(0)
     d_iq = torch.from_numpy(iq).cuda()
-    m = L.CarrierMeasure(ctx)
+    m = L.CellImpulse(ctx) if a.cir else L.CarrierMeasure(ctx)
     m.measure(d_iq, "ci16", fs_in, FC, cells, 1.92e6)              # warm-up
     m.timing_read()
     wall = []
@@ -105,6 +117,15 @@ def carrier_main(a):
     m.close()
     n = len(cells)
     dev_s = ms / 1e3 / a.reps
+    if a.cir:
+        macs = sum(cir_macs(c) for c in cells)
+        print(json.dumps({
+            "cir": True, "fs_in": fs_in, "cells": n, "reps": a.reps, "launches": launches,
+            "cir_device_us_per_cell": 1e6 * dev_s / n, "cir_host_us_per_cell": 1e6 * float(np.median(wall)) / n,
+            "cir_cmacs_per_cell": macs / n, "cir_fp64_tflops": 8 * macs / dev_s / 1e12, "gpu": gpu_name(),
+        }), flush=True)
+        ctx.close()
+        return
     bytes_ = sum(carrier_bytes(c, D) for c in cells)
     print(json.dumps({
         "carrier": True, "fs_in": fs_in, "cells": n, "reps": a.reps, "launches": launches,
@@ -120,9 +141,11 @@ def main():
     ap.add_argument("--channels", type=int, default=64)
     ap.add_argument("--reps", type=int, default=20)
     ap.add_argument("--carrier", action="store_true", help="time lcs_carrier_cells instead")
-    ap.add_argument("--copies", type=int, default=8, help="with --carrier: how often each of the 24 cells is measured per call")
+    ap.add_argument("--cir", action="store_true", help="time lcs_cir_cells instead")
+    ap.add_argument("--copies", type=int, default=8, help="with --carrier or --cir: how often each of the 24 cells is measured "
+                    "per call")
     a = ap.parse_args()
-    if a.carrier:
+    if a.carrier or a.cir:
         return carrier_main(a)
     import torch
     bufs = [S.synth_cu8(153600, cs, fc=FC, snr_db=12.0, seed=i) for i, cs in enumerate(BUFFERS)]
