@@ -70,6 +70,12 @@ static void print_usage() {
   cout << "                                 A cell whose carrier the recording does not hold whole shows -" << endl;
   cout << "     --cir-csv OUT.csv           with --cir: the power delay profile, one line per cell, port and delay tap," << endl;
   cout << "                                 n_id_cell,fc_hz,port,delay_ns,pdp_dbfs (- for a power <= 0)" << endl;
+  cout << "     --cfi                       with --wideband: add a CFI column, the control format indicator each cell sends" << endl;
+  cout << "                                 most often, decoded from its PCFICH in every subframe over all n_rb_dl RBs," << endl;
+  cout << "                                 taken from the recording itself; --fs-in as for --measure-carrier.  A cell whose" << endl;
+  cout << "                                 carrier the recording does not hold whole shows -" << endl;
+  cout << "     --cfi-csv OUT.csv           with --cfi: one line per cell and subframe," << endl;
+  cout << "                                 n_id_cell,fc_hz,subframe,cfi,metric1,metric2,metric3,sinr_db" << endl;
   cout << "  -r --record / -i --device-index need a live rtl-sdr dongle: not supported by this build" << endl;
 }
 
@@ -165,8 +171,8 @@ int main(int argc, char* const argv[]) {
   bool save_cap = false, use_recorded_data = false, raw = false, batched = false;
   string data_dir = ".", wideband, format = "ci16";
   double fs_in = -1, fc_in = -1;
-  bool resample = false, measure = false, measure_carrier = false, cir = false;
-  string spectrum, carrier_csv, cir_csv;
+  bool resample = false, measure = false, measure_carrier = false, cir = false, cfi = false;
+  string spectrum, carrier_csv, cir_csv, cfi_csv;
   long nfft = 4096;
   static struct option long_options[] = {
       {"help", no_argument, 0, 'h'},          {"verbose", no_argument, 0, 'v'},       {"brief", no_argument, 0, 'b'},
@@ -178,6 +184,7 @@ int main(int argc, char* const argv[]) {
       {"spectrum", required_argument, 0, 'P'},   {"nfft", required_argument, 0, 'N'},   {"measure", no_argument, 0, 'M'},
       {"measure-carrier", no_argument, 0, 'K'}, {"carrier-csv", required_argument, 0, 'V'},
       {"cir", no_argument, 0, 'X'},             {"cir-csv", required_argument, 0, 'Y'},
+      {"cfi", no_argument, 0, 'Q'},             {"cfi-csv", required_argument, 0, 'Z'},
       {0, 0, 0, 0}};
   for (;;) {
     int idx = 0;
@@ -209,6 +216,8 @@ int main(int argc, char* const argv[]) {
       case 'V': carrier_csv = optarg; break;
       case 'X': cir = true; break;
       case 'Y': cir_csv = optarg; break;
+      case 'Q': cfi = true; break;
+      case 'Z': cfi_csv = optarg; break;
       case 'i': break;
       default: return -1;
     }
@@ -223,6 +232,9 @@ int main(int argc, char* const argv[]) {
   if (!cir_csv.empty() && !cir) { cerr << "Error: --cir-csv needs --cir" << endl; return -1; }
   if (cir && wideband.empty()) { cerr << "Error: --cir needs --wideband" << endl; return -1; }
   if (cir && !search) { cerr << "Error: --cir needs a search (-s)" << endl; return -1; }
+  if (!cfi_csv.empty() && !cfi) { cerr << "Error: --cfi-csv needs --cfi" << endl; return -1; }
+  if (cfi && wideband.empty()) { cerr << "Error: --cfi needs --wideband" << endl; return -1; }
+  if (cfi && !search) { cerr << "Error: --cfi needs a search (-s)" << endl; return -1; }
   if (nfft < 64 || nfft > 65536 || (nfft & (nfft - 1))) { cerr << "Error: --nfft must be a power of two in [64, 65536]" << endl; return -1; }
   const bool wide = !wideband.empty();
   int wide_format = LCS_IQ_CI16;   // --format, for the spectrum and the search
@@ -285,10 +297,10 @@ int main(int argc, char* const argv[]) {
     } else {
       down = (uint32_t)std::lround(fs_in / 1.92e6);
     }
-    if (measure_carrier || cir) {
+    if (measure_carrier || cir || cfi) {
       const long D = std::lround(fs_in / 1.92e6);
       if (!((D == 2 || D == 4 || D == 8 || D == 16 || D == 32) && std::fabs(fs_in - D * 1.92e6) <= 1e-6)) {
-        cerr << "Error: " << (measure_carrier ? "--measure-carrier" : "--cir")
+        cerr << "Error: " << (measure_carrier ? "--measure-carrier" : (cir ? "--cir" : "--cfi"))
              << " needs --fs-in = D * 1.92 MHz with D in {2, 4, 8, 16, 32}" << endl;
         return -1;
       }
@@ -321,6 +333,8 @@ int main(int argc, char* const argv[]) {
   if (!carrier_csv.empty() && !(carrier_file = open_output(carrier_csv))) return -1;
   FILE* cir_file = nullptr;
   if (!cir_csv.empty() && !(cir_file = open_output(cir_csv))) return -1;
+  FILE* cfi_file = nullptr;
+  if (!cfi_csv.empty() && !(cfi_file = open_output(cfi_csv))) return -1;
   if (verbosity >= 1) {
     cout << "LTE CellSearch (GPU drop-in, " << lcs_version() << ") beginning" << endl;
     if (freq_start == freq_end) cout << "  Search frequency: " << freq_start / 1e6 << " MHz" << endl;
@@ -486,6 +500,24 @@ int main(int argc, char* const argv[]) {
         if (!ok) throw("cannot write the CIR CSV file");
       }
     }
+    vector<lcs_pcfich_meas> fmeas;   // --cfi: that of the k-th final cell, if fok[k]
+    vector<bool> fok;
+    if (cfi) {
+      measure_pcfich(wide_iq.data(), wide_format, wide_n, fs_in, fc_in, vector<Cell>(cells_final.begin(), cells_final.end()),
+                     fs_programmed, fmeas, fok);
+      if (cfi_file) {
+        bool ok = std::fprintf(cfi_file, "n_id_cell,fc_hz,subframe,cfi,metric1,metric2,metric3,sinr_db\n") > 0;
+        size_t k = 0;
+        for (list<Cell>::iterator it = cells_final.begin(); it != cells_final.end(); ++it, ++k)
+          for (int s = 0; fok[k] && s < (int)fmeas[k].n_subframes; s++) {
+            const lcs_pcfich_meas& m = fmeas[k];
+            ok = ok && std::fprintf(cfi_file, "%d,%.17g,%d,%u,%.17g,%.17g,%.17g,%s\n", (int)(*it).n_id_cell(), (*it).fc_requested,
+                                    s, m.cfi[s], m.metric[s][0], m.metric[s][1], m.metric[s][2], csv_db(m.sinr[s]).c_str()) > 0;
+          }
+        ok = std::fclose(cfi_file) == 0 && ok;
+        if (!ok) throw("cannot write the CFI CSV file");
+      }
+    }
     if (cells_final.size() == 0) {
       cout << "No LTE cells were found..." << endl;
     } else {   // CellSearch.cpp:579-613
@@ -493,7 +525,7 @@ int main(int argc, char* const argv[]) {
       cout << "A: #antenna ports C: CP type ; P: PHICH duration ; PR: PHICH resource type" << endl;
       cout << "CID A      fc   foff RXPWR C nRB P  PR CrystalCorrectionFactor" << (spec ? " CarrierPower[dBFS]" : "")
            << (measure ? " RSRP[dBFS] RSRQ[dB] SINR[dB]" : "") << (measure_carrier ? " RSRPc[dBFS] RSRQc[dB] SINRc[dB]" : "")
-           << (cir ? " TOA[us] DS[ns]" : "") << endl;
+           << (cir ? " TOA[us] DS[ns]" : "") << (cfi ? " CFI" : "") << endl;
       size_t k = 0;
       for (list<Cell>::iterator it = cells_final.begin(); it != cells_final.end(); ++it, ++k) {
         stringstream ss;
@@ -535,6 +567,12 @@ int main(int argc, char* const argv[]) {
                << 1e9 * tmeas[k].rms_spread[0];
           else
             ss << " - -";
+        }
+        if (cfi) {
+          if (fok[k])
+            ss << " " << fmeas[k].cfi_mode;
+          else
+            ss << " -";
         }
         cout << ss.str() << endl;
       }

@@ -23,6 +23,7 @@
 #include "../../include/lcs_meas.h"
 #include "../../include/lcs_carrier.h"
 #include "../../include/lcs_cir.h"
+#include "../../include/lcs_pcfich.h"
 
 // --- include/common.h.in ---
 typedef char int8;
@@ -126,6 +127,10 @@ void measure_carriers(const void* iq, int iq_format, uint64_t n, double fs_in, d
 // measure_carriers: meas[i] is that of cells[i], and ok[i] is false for a cell lcs_cir_cells rejects.
 void measure_cirs(const void* iq, int iq_format, uint64_t n, double fs_in, double fc_in, const std::vector<Cell>& cells,
                   const double& fs_programmed, std::vector<lcs_cir_meas>& meas, std::vector<bool>& ok);
+// The control format indicator in every subframe (lcs_pcfich of liblcs_pcfich.so, DESIGN.md section 4.12) of every cell
+// of `cells`, as measure_carriers: meas[i] is that of cells[i], and ok[i] is false for a cell lcs_pcfich_cells rejects.
+void measure_pcfich(const void* iq, int iq_format, uint64_t n, double fs_in, double fc_in, const std::vector<Cell>& cells,
+                    const double& fs_programmed, std::vector<lcs_pcfich_meas>& meas, std::vector<bool>& ok);
 // Welch power spectral density (lcs_psd of liblcs_psd.so, DESIGN.md section 4.8) of the whole recording in `path` ([n][2] in iq_format,
 // sample_bytes per sample, at fs_in, read in blocks): psd [nfft] in fftshift order, full-scale^2 per Hz, over n_segments segments.
 void wideband_psd(const std::string& path, int iq_format, size_t sample_bytes, double fs_in, uint32_t nfft,

@@ -1,7 +1,8 @@
 """ctypes binding of liblcs_b200.so - the C ABI declared in include/lcs_b200.h - and of the three modules built on top of
 it: liblcs_psd.so, the Welch spectrum of include/lcs_psd.h, liblcs_meas.so, the per-cell RSRP / RSRQ / SINR of
-include/lcs_meas.h, liblcs_carrier.so, the same over each cell's whole carrier, of include/lcs_carrier.h, and
-liblcs_cir.so, the power delay profile of each cell over its whole carrier, of include/lcs_cir.h.
+include/lcs_meas.h, liblcs_carrier.so, the same over each cell's whole carrier, of include/lcs_carrier.h,
+liblcs_cir.so, the power delay profile of each cell over its whole carrier, of include/lcs_cir.h, and liblcs_pcfich.so,
+the control format indicator of each cell in every subframe, of include/lcs_pcfich.h.
 
 This module is plumbing for tests/, bench.py and __graft_entry__.py: every call goes through the
 same `extern "C"` entry points a C++/IT++ host would bind (INTEGRATION.md).  lib() gives every
@@ -27,6 +28,8 @@ CARRIER_LIB_PATH = os.environ.get("LCS_CARRIER_LIB") or os.path.join(HERE, "libl
 CARRIER_HEADER = os.path.join(HERE, "..", "include", "lcs_carrier.h")
 CIR_LIB_PATH = os.environ.get("LCS_CIR_LIB") or os.path.join(HERE, "liblcs_cir.so")
 CIR_HEADER = os.path.join(HERE, "..", "include", "lcs_cir.h")
+PCFICH_LIB_PATH = os.environ.get("LCS_PCFICH_LIB") or os.path.join(HERE, "liblcs_pcfich.so")
+PCFICH_HEADER = os.path.join(HERE, "..", "include", "lcs_pcfich.h")
 
 IQ_CF32, IQ_CU8, IQ_C128, IQ_CI16, IQ_CS8 = 0, 1, 2, 3, 4
 KERNEL_AUTO, KERNEL_FP32, KERNEL_TC = 0, 1, 2
@@ -145,6 +148,12 @@ def cir_lib():
     """liblcs_cir.so (include/lcs_cir.h); it takes the contexts of lib()."""
     lib()
     return _bind(CIR_LIB_PATH, CIR_HEADER)
+
+
+def pcfich_lib():
+    """liblcs_pcfich.so (include/lcs_pcfich.h); it takes the contexts of lib()."""
+    lib()
+    return _bind(PCFICH_LIB_PATH, PCFICH_HEADER)
 
 
 def _p(a):
@@ -834,7 +843,7 @@ class CellMeasure(_Handle):
 
 
 def _measure_recording(h, fn, dtype, iq, fmt, fs_in, fc_in, cells, fs_programmed):
-    """fn (lcs_carrier_cells or lcs_cir_cells) of handle h on the recording iq: a record array of dtype, one row per
+    """fn (lcs_carrier_cells, lcs_cir_cells or lcs_pcfich_cells) of handle h on the recording iq: a record array of dtype, one row per
     cell."""
     iq_format = _iq_format(fmt)
     cells = list(cells)
@@ -918,3 +927,29 @@ class CellImpulse(_Handle):
     def measure(self, iq, fmt, fs_in, fc_in, cells, fs_programmed):
         """As CarrierMeasure.measure; returns a CIR_MEAS record array, one row per cell."""
         return _measure_recording(self, cir_lib().lcs_cir_cells, CIR_MEAS, iq, fmt, fs_in, fc_in, cells, fs_programmed)
+
+
+# lcs_pcfich_meas as a numpy record
+PCFICH_SUBFRAMES = 61                 # LCS_PCFICH_SUBFRAMES
+PCFICH_MEAS = np.dtype([("metric", np.float64, (PCFICH_SUBFRAMES, 3)), ("sinr", np.float64, PCFICH_SUBFRAMES),
+                        ("cfi", np.uint32, PCFICH_SUBFRAMES), ("count", np.uint32, 4), ("cfi_mode", np.uint32),
+                        ("n_ctrl_symbols", np.uint32), ("n_subframes", np.uint32)], align=True)
+PCFICH_CHUNK = 32                     # LCS_PCFICH_CHUNK: cells per chunk, two launches each
+
+
+class ControlFormat(_Handle):
+    """lcs_pcfich: the control format indicator of found cells in every subframe, decoded from their PCFICH over the
+    whole carrier of the wideband recording they were found in (DESIGN.md section 4.12)."""
+    _destroy = "lcs_pcfich_destroy"
+    _timing_read = "lcs_pcfich_timing_read"
+    _lib = staticmethod(pcfich_lib)
+
+    def __init__(self, ctx):
+        self.ctx = ctx
+        self._h = C.c_void_p()
+        _chk(pcfich_lib().lcs_pcfich_create(ctx._h, C.byref(self._h)), ctx._h)
+
+    def measure(self, iq, fmt, fs_in, fc_in, cells, fs_programmed):
+        """As CarrierMeasure.measure; returns a PCFICH_MEAS record array, one row per cell."""
+        return _measure_recording(self, pcfich_lib().lcs_pcfich_cells, PCFICH_MEAS, iq, fmt, fs_in, fc_in, cells,
+                                  fs_programmed)

@@ -21,9 +21,14 @@ the same way: one JSON line with the device time per cell (lcs_cir_timing_read),
 transform per cell (2 R CRS x 320 taps for every CRS symbol of every port), their FP64 rate, and the card, read in the
 same run.
 
+With --pcfich it times the CFI decoder (lcs_pcfich_cells, DESIGN.md section 4.12) on the same recording and cells in
+the same way: one JSON line with the device time per cell (lcs_pcfich_timing_read), the launches and the card, read in
+the same run.
+
 Usage: python tools/meas_bench.py [--channels 64] [--reps 20]
        python tools/meas_bench.py --carrier [--copies 8] [--reps 20]
        python tools/meas_bench.py --cir [--copies 8] [--reps 20]
+       python tools/meas_bench.py --pcfich [--copies 8] [--reps 20]
 """
 import argparse
 import json
@@ -105,7 +110,7 @@ def carrier_main(a):
     cells = cells * a.copies
     ctx = L.Context(0)
     d_iq = torch.from_numpy(iq).cuda()
-    m = L.CellImpulse(ctx) if a.cir else L.CarrierMeasure(ctx)
+    m = L.ControlFormat(ctx) if a.pcfich else (L.CellImpulse(ctx) if a.cir else L.CarrierMeasure(ctx))
     m.measure(d_iq, "ci16", fs_in, FC, cells, 1.92e6)              # warm-up
     m.timing_read()
     wall = []
@@ -117,6 +122,14 @@ def carrier_main(a):
     m.close()
     n = len(cells)
     dev_s = ms / 1e3 / a.reps
+    if a.pcfich:
+        print(json.dumps({
+            "pcfich": True, "fs_in": fs_in, "cells": n, "reps": a.reps, "launches": launches,
+            "pcfich_device_us_per_cell": 1e6 * dev_s / n, "pcfich_host_us_per_cell": 1e6 * float(np.median(wall)) / n,
+            "gpu": gpu_name(),
+        }), flush=True)
+        ctx.close()
+        return
     if a.cir:
         macs = sum(cir_macs(c) for c in cells)
         print(json.dumps({
@@ -142,10 +155,11 @@ def main():
     ap.add_argument("--reps", type=int, default=20)
     ap.add_argument("--carrier", action="store_true", help="time lcs_carrier_cells instead")
     ap.add_argument("--cir", action="store_true", help="time lcs_cir_cells instead")
-    ap.add_argument("--copies", type=int, default=8, help="with --carrier or --cir: how often each of the 24 cells is measured "
-                    "per call")
+    ap.add_argument("--pcfich", action="store_true", help="time lcs_pcfich_cells instead")
+    ap.add_argument("--copies", type=int, default=8, help="with --carrier, --cir or --pcfich: how often each of the 24 cells "
+                    "is measured per call")
     a = ap.parse_args()
-    if a.carrier or a.cir:
+    if a.carrier or a.cir or a.pcfich:
         return carrier_main(a)
     import torch
     bufs = [S.synth_cu8(153600, cs, fc=FC, snr_db=12.0, seed=i) for i, cs in enumerate(BUFFERS)]

@@ -241,9 +241,40 @@ def subcarriers(n_rb_dl):
     return np.concatenate([np.arange(-6 * R, 0), np.arange(1, 6 * R + 1)])
 
 
+def pcfich_res(n_id_cell, n_rb_dl):
+    """The 16 columns of the PCFICH in symbol 0 (36.211 6.7.4): quadruplet i in the REG at 6 (n_id_cell mod 2R) +
+    6 floor(i R / 2) (mod 12 R), on its 4 REs off the CRS of ports 0 and 1."""
+    R = n_rb_dl
+    cols = []
+    for i in range(4):
+        k0 = (6 * (n_id_cell % (2 * R)) + 6 * (i * R // 2)) % (12 * R)
+        cols += [k0 + o for o in range(6) if o % 3 != n_id_cell % 3]
+    return np.array(cols)
+
+
+def pcfich_symbols(n_id_cell, n_ports, subframe, cfi):
+    """The PCFICH of CFI cfi in subframe number `subframe` per port, [n_ports][16]: the codeword of 36.212 Table 5.3.4-1
+    scrambled (36.211 6.7.1), QPSK-mapped and precoded for transmit diversity (6.3.4.3), as _grid's PBCH."""
+    cw = (np.arange(32) % 3 != cfi - 1).astype(np.uint8)
+    c = O.lte_pn((subframe + 1) * (2 * n_id_cell + 1) * 512 + n_id_cell, 32).astype(np.uint8)
+    e = (cw ^ c).astype(float)
+    d = ((1 - 2 * e[0::2]) + 1j * (1 - 2 * e[1::2])) / np.sqrt(2)
+    y = np.zeros((n_ports, 16), complex)
+    if n_ports == 1:
+        y[0] = d
+        return y
+    for j in range(8):                                  # pair j: ports (0, 1), or (0, 2) / (1, 3) for four ports
+        a, b = (0, 1) if n_ports == 2 else ((0, 2) if j % 2 == 0 else (1, 3))
+        y[a, 2 * j], y[a, 2 * j + 1] = d[2 * j] / np.sqrt(2), d[2 * j + 1] / np.sqrt(2)
+        y[b, 2 * j], y[b, 2 * j + 1] = -np.conj(d[2 * j + 1]) / np.sqrt(2), np.conj(d[2 * j]) / np.sqrt(2)
+    return y
+
+
 def _grid_full(cell, n_frames, rng):
     """Transmitted grid of all n_rb_dl RBs per port, [n_ports][n_sym][12 R]: the 6-RB content of _grid in the centre,
-    full-band CRS, and QPSK times sqrt(cell["load"]) (default 1) on port 0 on every other RE outside the centre."""
+    full-band CRS, and QPSK times sqrt(cell["load"]) (default 1) on port 0 on every other RE outside the centre.  With
+    cell["cfi"], a sequence of CFIs, subframe u (counted from the grid's first) carries the PCFICH of cfi[u mod len] in
+    its symbol 0, written last."""
     R, P, cp = cell["n_rb_dl"], cell["n_ports"], cell["cp_type"]
     X6, n_symb = _grid(cell, n_frames, cell.get("sfn0", 0), rng)
     n_sym = X6.shape[1]
@@ -262,6 +293,10 @@ def _grid_full(cell, n_frames, rng):
             X[:, g, idx] = 0
             X[p, g, idx] = rs[slot, sym]
     X[:, :, 6 * R - 36:6 * R + 36] = X6
+    if "cfi" in cell:
+        cols, seq = pcfich_res(cell["n_id_cell"], R), list(cell["cfi"])
+        for u in range(n_sym // (2 * n_symb)):
+            X[:, 2 * n_symb * u, cols] = pcfich_symbols(cell["n_id_cell"], P, u % 10, seq[u % len(seq)])
     return X, n_symb
 
 
