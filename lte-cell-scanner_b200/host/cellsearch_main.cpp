@@ -76,6 +76,13 @@ static void print_usage() {
   cout << "                                 carrier the recording does not hold whole shows -" << endl;
   cout << "     --cfi-csv OUT.csv           with --cfi: one line per cell and subframe," << endl;
   cout << "                                 n_id_cell,fc_hz,subframe,cfi,metric1,metric2,metric3,sinr_db" << endl;
+  cout << "     --pdcch                     with --wideband: add an SI column, the number of System Information DCIs" << endl;
+  cout << "                                 (SI-RNTI) decoded from each cell's PDCCH common search space in every subframe" << endl;
+  cout << "                                 over all n_rb_dl RBs, taken from the recording itself; --fs-in as for" << endl;
+  cout << "                                 --measure-carrier.  A cell whose carrier the recording does not hold whole shows -" << endl;
+  cout << "     --pdcch-csv OUT.csv         with --pdcch: one line per decoded DCI (SI-, P- and RA-RNTI, formats 1A and 1C)," << endl;
+  cout << "                                 n_id_cell,fc_hz,subframe,cfi,format,agg,cce,rnti,n_bits,payload_hex,quality," << endl;
+  cout << "                                 rb_start,n_rb,mcs,rv (- for a field the format does not have)" << endl;
   cout << "  -r --record / -i --device-index need a live rtl-sdr dongle: not supported by this build" << endl;
 }
 
@@ -171,8 +178,8 @@ int main(int argc, char* const argv[]) {
   bool save_cap = false, use_recorded_data = false, raw = false, batched = false;
   string data_dir = ".", wideband, format = "ci16";
   double fs_in = -1, fc_in = -1;
-  bool resample = false, measure = false, measure_carrier = false, cir = false, cfi = false;
-  string spectrum, carrier_csv, cir_csv, cfi_csv;
+  bool resample = false, measure = false, measure_carrier = false, cir = false, cfi = false, pdcch = false;
+  string spectrum, carrier_csv, cir_csv, cfi_csv, pdcch_csv;
   long nfft = 4096;
   static struct option long_options[] = {
       {"help", no_argument, 0, 'h'},          {"verbose", no_argument, 0, 'v'},       {"brief", no_argument, 0, 'b'},
@@ -185,6 +192,7 @@ int main(int argc, char* const argv[]) {
       {"measure-carrier", no_argument, 0, 'K'}, {"carrier-csv", required_argument, 0, 'V'},
       {"cir", no_argument, 0, 'X'},             {"cir-csv", required_argument, 0, 'Y'},
       {"cfi", no_argument, 0, 'Q'},             {"cfi-csv", required_argument, 0, 'Z'},
+      {"pdcch", no_argument, 0, 'H'},           {"pdcch-csv", required_argument, 0, 'J'},
       {0, 0, 0, 0}};
   for (;;) {
     int idx = 0;
@@ -218,6 +226,8 @@ int main(int argc, char* const argv[]) {
       case 'Y': cir_csv = optarg; break;
       case 'Q': cfi = true; break;
       case 'Z': cfi_csv = optarg; break;
+      case 'H': pdcch = true; break;
+      case 'J': pdcch_csv = optarg; break;
       case 'i': break;
       default: return -1;
     }
@@ -235,6 +245,9 @@ int main(int argc, char* const argv[]) {
   if (!cfi_csv.empty() && !cfi) { cerr << "Error: --cfi-csv needs --cfi" << endl; return -1; }
   if (cfi && wideband.empty()) { cerr << "Error: --cfi needs --wideband" << endl; return -1; }
   if (cfi && !search) { cerr << "Error: --cfi needs a search (-s)" << endl; return -1; }
+  if (!pdcch_csv.empty() && !pdcch) { cerr << "Error: --pdcch-csv needs --pdcch" << endl; return -1; }
+  if (pdcch && wideband.empty()) { cerr << "Error: --pdcch needs --wideband" << endl; return -1; }
+  if (pdcch && !search) { cerr << "Error: --pdcch needs a search (-s)" << endl; return -1; }
   if (nfft < 64 || nfft > 65536 || (nfft & (nfft - 1))) { cerr << "Error: --nfft must be a power of two in [64, 65536]" << endl; return -1; }
   const bool wide = !wideband.empty();
   int wide_format = LCS_IQ_CI16;   // --format, for the spectrum and the search
@@ -297,10 +310,10 @@ int main(int argc, char* const argv[]) {
     } else {
       down = (uint32_t)std::lround(fs_in / 1.92e6);
     }
-    if (measure_carrier || cir || cfi) {
+    if (measure_carrier || cir || cfi || pdcch) {
       const long D = std::lround(fs_in / 1.92e6);
       if (!((D == 2 || D == 4 || D == 8 || D == 16 || D == 32) && std::fabs(fs_in - D * 1.92e6) <= 1e-6)) {
-        cerr << "Error: " << (measure_carrier ? "--measure-carrier" : (cir ? "--cir" : "--cfi"))
+        cerr << "Error: " << (measure_carrier ? "--measure-carrier" : (cir ? "--cir" : (cfi ? "--cfi" : "--pdcch")))
              << " needs --fs-in = D * 1.92 MHz with D in {2, 4, 8, 16, 32}" << endl;
         return -1;
       }
@@ -335,6 +348,8 @@ int main(int argc, char* const argv[]) {
   if (!cir_csv.empty() && !(cir_file = open_output(cir_csv))) return -1;
   FILE* cfi_file = nullptr;
   if (!cfi_csv.empty() && !(cfi_file = open_output(cfi_csv))) return -1;
+  FILE* pdcch_file = nullptr;
+  if (!pdcch_csv.empty() && !(pdcch_file = open_output(pdcch_csv))) return -1;
   if (verbosity >= 1) {
     cout << "LTE CellSearch (GPU drop-in, " << lcs_version() << ") beginning" << endl;
     if (freq_start == freq_end) cout << "  Search frequency: " << freq_start / 1e6 << " MHz" << endl;
@@ -518,6 +533,30 @@ int main(int argc, char* const argv[]) {
         if (!ok) throw("cannot write the CFI CSV file");
       }
     }
+    vector<lcs_pdcch_meas> pmeas;   // --pdcch: that of the k-th final cell, if pok[k]
+    vector<bool> pok;
+    if (pdcch) {
+      measure_pdcch(wide_iq.data(), wide_format, wide_n, fs_in, fc_in, vector<Cell>(cells_final.begin(), cells_final.end()),
+                    fs_programmed, pmeas, pok);
+      if (pdcch_file) {
+        bool ok = std::fprintf(pdcch_file, "n_id_cell,fc_hz,subframe,cfi,format,agg,cce,rnti,n_bits,payload_hex,quality,"
+                                           "rb_start,n_rb,mcs,rv\n") > 0;
+        size_t k = 0;
+        for (list<Cell>::iterator it = cells_final.begin(); it != cells_final.end(); ++it, ++k)
+          for (int s = 0; pok[k] && s < (int)pmeas[k].n_subframes; s++)
+            for (uint32_t i = 0; i < pmeas[k].n_dci[s]; i++) {
+              const lcs_pdcch_dci& d = pmeas[k].dci[s][i];
+              const bool a = d.format == LCS_DCI_1A;
+              const string rb = a && d.n_rb > 0 ? std::to_string(d.rb_start) + "," + std::to_string(d.n_rb) : "-,-";
+              const string mr = a ? std::to_string(d.mcs) + "," + std::to_string(d.rv) : "-,-";
+              ok = ok && std::fprintf(pdcch_file, "%d,%.17g,%d,%u,%s,%u,%u,%u,%u,%llx,%.17g,%s,%s\n", (int)(*it).n_id_cell(),
+                                      (*it).fc_requested, s, pmeas[k].cfi[s], a ? "1A" : "1C", d.agg, d.cce, d.rnti, d.n_bits,
+                                      (unsigned long long)d.payload, d.quality, rb.c_str(), mr.c_str()) > 0;
+            }
+        ok = std::fclose(pdcch_file) == 0 && ok;
+        if (!ok) throw("cannot write the PDCCH CSV file");
+      }
+    }
     if (cells_final.size() == 0) {
       cout << "No LTE cells were found..." << endl;
     } else {   // CellSearch.cpp:579-613
@@ -525,7 +564,7 @@ int main(int argc, char* const argv[]) {
       cout << "A: #antenna ports C: CP type ; P: PHICH duration ; PR: PHICH resource type" << endl;
       cout << "CID A      fc   foff RXPWR C nRB P  PR CrystalCorrectionFactor" << (spec ? " CarrierPower[dBFS]" : "")
            << (measure ? " RSRP[dBFS] RSRQ[dB] SINR[dB]" : "") << (measure_carrier ? " RSRPc[dBFS] RSRQc[dB] SINRc[dB]" : "")
-           << (cir ? " TOA[us] DS[ns]" : "") << (cfi ? " CFI" : "") << endl;
+           << (cir ? " TOA[us] DS[ns]" : "") << (cfi ? " CFI" : "") << (pdcch ? " SI" : "") << endl;
       size_t k = 0;
       for (list<Cell>::iterator it = cells_final.begin(); it != cells_final.end(); ++it, ++k) {
         stringstream ss;
@@ -571,6 +610,12 @@ int main(int argc, char* const argv[]) {
         if (cfi) {
           if (fok[k])
             ss << " " << fmeas[k].cfi_mode;
+          else
+            ss << " -";
+        }
+        if (pdcch) {
+          if (pok[k])
+            ss << " " << pmeas[k].count[0];
           else
             ss << " -";
         }

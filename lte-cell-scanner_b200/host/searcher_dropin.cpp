@@ -100,8 +100,8 @@ void measure_cells(const void* iq, int iq_format, uint32_t n_cap, const std::vec
   check(measure_lists(iq, iq_format, 0, n_cap, detected_cells, fs_programmed, meas, &where), where);
 }
 
-// One measurement of the wideband recording (lcs_carrier_cells, lcs_cir_cells or lcs_pcfich_cells, through handle type H)
-// of every cell of `cells`: all in one call, and when a cell is rejected each on its own, so that only the rejected ones go
+// One measurement of the wideband recording (lcs_carrier_cells, lcs_cir_cells, lcs_pcfich_cells or lcs_pdcch_cells, through
+// handle type H) of every cell of `cells`: all in one call, and when a cell is rejected each on its own, so that only the rejected ones go
 // unmeasured.
 template <class H, class M, class Create, class Cells, class Destroy>
 static void measure_recording(Create create, Cells cells_fn, Destroy destroy, const char* what, const void* iq, int iq_format,
@@ -144,6 +144,12 @@ void measure_pcfich(const void* iq, int iq_format, uint64_t n, double fs_in, dou
                     const double& fs_programmed, std::vector<lcs_pcfich_meas>& meas, std::vector<bool>& ok) {
   measure_recording<lcs_pcfich>(lcs_pcfich_create, lcs_pcfich_cells, lcs_pcfich_destroy, "lcs_pcfich", iq, iq_format, n, fs_in,
                                 fc_in, cells, fs_programmed, meas, ok);
+}
+
+void measure_pdcch(const void* iq, int iq_format, uint64_t n, double fs_in, double fc_in, const std::vector<Cell>& cells,
+                   const double& fs_programmed, std::vector<lcs_pdcch_meas>& meas, std::vector<bool>& ok) {
+  measure_recording<lcs_pdcch>(lcs_pdcch_create, lcs_pdcch_cells, lcs_pdcch_destroy, "lcs_pdcch", iq, iq_format, n, fs_in,
+                               fc_in, cells, fs_programmed, meas, ok);
 }
 
 void sweep_search_cu8(const std::vector<unsigned char>& iq, uint32_t n_cap, const std::vector<double>& fc_requested,

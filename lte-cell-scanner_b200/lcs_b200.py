@@ -1,8 +1,9 @@
 """ctypes binding of liblcs_b200.so - the C ABI declared in include/lcs_b200.h - and of the three modules built on top of
 it: liblcs_psd.so, the Welch spectrum of include/lcs_psd.h, liblcs_meas.so, the per-cell RSRP / RSRQ / SINR of
 include/lcs_meas.h, liblcs_carrier.so, the same over each cell's whole carrier, of include/lcs_carrier.h,
-liblcs_cir.so, the power delay profile of each cell over its whole carrier, of include/lcs_cir.h, and liblcs_pcfich.so,
-the control format indicator of each cell in every subframe, of include/lcs_pcfich.h.
+liblcs_cir.so, the power delay profile of each cell over its whole carrier, of include/lcs_cir.h, liblcs_pcfich.so,
+the control format indicator of each cell in every subframe, of include/lcs_pcfich.h, and liblcs_pdcch.so, the
+common-search-space DCIs of each cell in every subframe, of include/lcs_pdcch.h.
 
 This module is plumbing for tests/, bench.py and __graft_entry__.py: every call goes through the
 same `extern "C"` entry points a C++/IT++ host would bind (INTEGRATION.md).  lib() gives every
@@ -30,6 +31,8 @@ CIR_LIB_PATH = os.environ.get("LCS_CIR_LIB") or os.path.join(HERE, "liblcs_cir.s
 CIR_HEADER = os.path.join(HERE, "..", "include", "lcs_cir.h")
 PCFICH_LIB_PATH = os.environ.get("LCS_PCFICH_LIB") or os.path.join(HERE, "liblcs_pcfich.so")
 PCFICH_HEADER = os.path.join(HERE, "..", "include", "lcs_pcfich.h")
+PDCCH_LIB_PATH = os.environ.get("LCS_PDCCH_LIB") or os.path.join(HERE, "liblcs_pdcch.so")
+PDCCH_HEADER = os.path.join(HERE, "..", "include", "lcs_pdcch.h")
 
 IQ_CF32, IQ_CU8, IQ_C128, IQ_CI16, IQ_CS8 = 0, 1, 2, 3, 4
 KERNEL_AUTO, KERNEL_FP32, KERNEL_TC = 0, 1, 2
@@ -154,6 +157,12 @@ def pcfich_lib():
     """liblcs_pcfich.so (include/lcs_pcfich.h); it takes the contexts of lib()."""
     lib()
     return _bind(PCFICH_LIB_PATH, PCFICH_HEADER)
+
+
+def pdcch_lib():
+    """liblcs_pdcch.so (include/lcs_pdcch.h); it takes the contexts of lib()."""
+    lib()
+    return _bind(PDCCH_LIB_PATH, PDCCH_HEADER)
 
 
 def _p(a):
@@ -843,7 +852,7 @@ class CellMeasure(_Handle):
 
 
 def _measure_recording(h, fn, dtype, iq, fmt, fs_in, fc_in, cells, fs_programmed):
-    """fn (lcs_carrier_cells, lcs_cir_cells or lcs_pcfich_cells) of handle h on the recording iq: a record array of dtype, one row per
+    """fn (lcs_carrier_cells, lcs_cir_cells, lcs_pcfich_cells or lcs_pdcch_cells) of handle h on the recording iq: a record array of dtype, one row per
     cell."""
     iq_format = _iq_format(fmt)
     cells = list(cells)
@@ -952,4 +961,40 @@ class ControlFormat(_Handle):
     def measure(self, iq, fmt, fs_in, fc_in, cells, fs_programmed):
         """As CarrierMeasure.measure; returns a PCFICH_MEAS record array, one row per cell."""
         return _measure_recording(self, pcfich_lib().lcs_pcfich_cells, PCFICH_MEAS, iq, fmt, fs_in, fc_in, cells,
+                                  fs_programmed)
+
+
+# lcs_pdcch_dci and lcs_pdcch_meas as numpy records
+PDCCH_SUBFRAMES = 61                  # LCS_PDCCH_SUBFRAMES
+PDCCH_MAX_DCI = 6                     # LCS_PDCCH_MAX_DCI
+DCI_1A, DCI_1C = 1, 2                 # LCS_DCI_1A, LCS_DCI_1C
+RNTI_SI, RNTI_P = 0xFFFF, 0xFFFE      # LCS_RNTI_SI, LCS_RNTI_P
+PDCCH_DCI = np.dtype([("quality", np.float64), ("payload", np.uint64), ("format", np.uint32), ("agg", np.uint32),
+                      ("cce", np.uint32), ("rnti", np.uint32), ("n_bits", np.uint32), ("riv", np.uint32),
+                      ("rb_start", np.int32), ("n_rb", np.int32), ("localized", np.uint32), ("mcs", np.uint32),
+                      ("harq", np.uint32), ("ndi", np.uint32), ("rv", np.uint32), ("tpc", np.uint32), ("gap", np.uint32),
+                      ("tbs_index", np.uint32)], align=True)
+PDCCH_MEAS = np.dtype([("dci", PDCCH_DCI, (PDCCH_SUBFRAMES, PDCCH_MAX_DCI)), ("cfi", np.uint32, PDCCH_SUBFRAMES),
+                       ("n_ctrl", np.uint32, PDCCH_SUBFRAMES), ("n_reg", np.uint32, PDCCH_SUBFRAMES),
+                       ("n_cce", np.uint32, PDCCH_SUBFRAMES), ("n_dci", np.uint32, PDCCH_SUBFRAMES), ("count", np.uint32, 3),
+                       ("si_subframes", np.uint32), ("n_subframes", np.uint32)], align=True)
+PDCCH_CHUNK = 32                      # LCS_PDCCH_CHUNK: cells per chunk, three launches each
+
+
+class ControlChannel(_Handle):
+    """lcs_pdcch: the common-search-space DCIs (SI-, P- and RA-RNTI, formats 1A and 1C) of found cells in every
+    subframe, decoded from their PDCCH over the whole carrier of the wideband recording they were found in (DESIGN.md
+    section 4.13)."""
+    _destroy = "lcs_pdcch_destroy"
+    _timing_read = "lcs_pdcch_timing_read"
+    _lib = staticmethod(pdcch_lib)
+
+    def __init__(self, ctx):
+        self.ctx = ctx
+        self._h = C.c_void_p()
+        _chk(pdcch_lib().lcs_pdcch_create(ctx._h, C.byref(self._h)), ctx._h)
+
+    def measure(self, iq, fmt, fs_in, fc_in, cells, fs_programmed):
+        """As CarrierMeasure.measure; returns a PDCCH_MEAS record array, one row per cell."""
+        return _measure_recording(self, pdcch_lib().lcs_pdcch_cells, PDCCH_MEAS, iq, fmt, fs_in, fc_in, cells,
                                   fs_programmed)

@@ -25,10 +25,15 @@ With --pcfich it times the CFI decoder (lcs_pcfich_cells, DESIGN.md section 4.12
 the same way: one JSON line with the device time per cell (lcs_pcfich_timing_read), the launches and the card, read in
 the same run.
 
+With --pdcch it times the common-search-space DCI decoder (lcs_pdcch_cells, DESIGN.md section 4.13) on the same
+recording and cells in the same way (PHICH duration normal, N_g = 1): one JSON line with the device time per cell
+(lcs_pdcch_timing_read), the launches and the card, read in the same run.
+
 Usage: python tools/meas_bench.py [--channels 64] [--reps 20]
        python tools/meas_bench.py --carrier [--copies 8] [--reps 20]
        python tools/meas_bench.py --cir [--copies 8] [--reps 20]
        python tools/meas_bench.py --pcfich [--copies 8] [--reps 20]
+       python tools/meas_bench.py --pdcch [--copies 8] [--reps 20]
 """
 import argparse
 import json
@@ -104,13 +109,15 @@ def carrier_main(a):
         for c in cs:
             cells.append(L.new_cell(fc_requested=FC + off, fc_programmed=FC + off, n_id_1=c["n_id_cell"] // 3,
                                     n_id_2=c["n_id_cell"] % 3, cp_type=c["cp_type"], n_ports=c["n_ports"],
-                                    frame_start=float(c["t0"]), freq_superfine=0.0, n_rb_dl=50))
+                                    frame_start=float(c["t0"]), freq_superfine=0.0, n_rb_dl=50, phich_duration=1,
+                                    phich_resource=3))
     x, _ = S.synth_wide_full(D * (5000 + 122 * 960 + 400), fs_in, FC, carriers, 30.0, 0)
     iq = S.quantise(x, "ci16", 0.1 / np.sqrt(np.mean(np.abs(x) ** 2)))
     cells = cells * a.copies
     ctx = L.Context(0)
     d_iq = torch.from_numpy(iq).cuda()
-    m = L.ControlFormat(ctx) if a.pcfich else (L.CellImpulse(ctx) if a.cir else L.CarrierMeasure(ctx))
+    m = (L.ControlChannel(ctx) if a.pdcch else L.ControlFormat(ctx) if a.pcfich else
+         L.CellImpulse(ctx) if a.cir else L.CarrierMeasure(ctx))
     m.measure(d_iq, "ci16", fs_in, FC, cells, 1.92e6)              # warm-up
     m.timing_read()
     wall = []
@@ -122,6 +129,14 @@ def carrier_main(a):
     m.close()
     n = len(cells)
     dev_s = ms / 1e3 / a.reps
+    if a.pdcch:
+        print(json.dumps({
+            "pdcch": True, "fs_in": fs_in, "cells": n, "reps": a.reps, "launches": launches,
+            "pdcch_device_us_per_cell": 1e6 * dev_s / n, "pdcch_host_us_per_cell": 1e6 * float(np.median(wall)) / n,
+            "gpu": gpu_name(),
+        }), flush=True)
+        ctx.close()
+        return
     if a.pcfich:
         print(json.dumps({
             "pcfich": True, "fs_in": fs_in, "cells": n, "reps": a.reps, "launches": launches,
@@ -156,10 +171,11 @@ def main():
     ap.add_argument("--carrier", action="store_true", help="time lcs_carrier_cells instead")
     ap.add_argument("--cir", action="store_true", help="time lcs_cir_cells instead")
     ap.add_argument("--pcfich", action="store_true", help="time lcs_pcfich_cells instead")
-    ap.add_argument("--copies", type=int, default=8, help="with --carrier, --cir or --pcfich: how often each of the 24 cells "
-                    "is measured per call")
+    ap.add_argument("--pdcch", action="store_true", help="time lcs_pdcch_cells instead")
+    ap.add_argument("--copies", type=int, default=8, help="with --carrier, --cir, --pcfich or --pdcch: how often each of "
+                    "the 24 cells is measured per call")
     a = ap.parse_args()
-    if a.carrier or a.cir or a.pcfich:
+    if a.carrier or a.cir or a.pcfich or a.pdcch:
         return carrier_main(a)
     import torch
     bufs = [S.synth_cu8(153600, cs, fc=FC, snr_db=12.0, seed=i) for i, cs in enumerate(BUFFERS)]

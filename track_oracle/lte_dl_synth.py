@@ -274,7 +274,7 @@ def _grid_full(cell, n_frames, rng):
     """Transmitted grid of all n_rb_dl RBs per port, [n_ports][n_sym][12 R]: the 6-RB content of _grid in the centre,
     full-band CRS, and QPSK times sqrt(cell["load"]) (default 1) on port 0 on every other RE outside the centre.  With
     cell["cfi"], a sequence of CFIs, subframe u (counted from the grid's first) carries the PCFICH of cfi[u mod len] in
-    its symbol 0, written last."""
+    its symbol 0, written last; with cell["pdcch"] as well, its control region carries those DCIs (_write_control)."""
     R, P, cp = cell["n_rb_dl"], cell["n_ports"], cell["cp_type"]
     X6, n_symb = _grid(cell, n_frames, cell.get("sfn0", 0), rng)
     n_sym = X6.shape[1]
@@ -293,11 +293,133 @@ def _grid_full(cell, n_frames, rng):
             X[:, g, idx] = 0
             X[p, g, idx] = rs[slot, sym]
     X[:, :, 6 * R - 36:6 * R + 36] = X6
+    if "pdcch" in cell:
+        _write_control(X, cell, n_symb)
     if "cfi" in cell:
         cols, seq = pcfich_res(cell["n_id_cell"], R), list(cell["cfi"])
         for u in range(n_sym // (2 * n_symb)):
             X[:, 2 * n_symb * u, cols] = pcfich_symbols(cell["n_id_cell"], P, u % 10, seq[u % len(seq)])
     return X, n_symb
+
+
+# ---- the control region: PHICH and PDCCH REGs (36.211 6.2.4, 6.8.5, 6.9.3) -------------------------------------------------
+DCI_SIZES_1A = {6: 21, 15: 22, 25: 25, 50: 27, 75: 27, 100: 28}      # 36.212 5.3.3.1.3, FDD, with its padding bit
+DCI_SIZES_1C = {6: 8, 15: 10, 25: 12, 50: 13, 75: 14, 100: 15}       # 36.212 5.3.3.1.4
+
+
+def reg_is_six(l, n_ports, cp_type):
+    """True when the REGs of control symbol l are 6 REs (2 of them CRS), else 4."""
+    return l == 0 or (l == 1 and n_ports == 4) or (l == 3 and cp_type == 2)
+
+
+def reg_data_cols(l, k0, n_id_cell, n_ports, cp_type):
+    """The 4 data columns of the REG of symbol l starting at k0, in increasing k."""
+    if reg_is_six(l, n_ports, cp_type):
+        return [k0 + o for o in range(6) if (k0 + o) % 3 != n_id_cell % 3]
+    return [k0 + o for o in range(4)]
+
+
+def n_ctrl_of(cfi, R, phich_duration):
+    """Symbols of the control region: CFI (+1 at R <= 10), at least 3 with extended PHICH duration."""
+    n = cfi + (R <= 10)
+    return max(n, 3) if phich_duration == 2 else n
+
+
+def control_regs(R, n_ports, cp_type, n_id_cell, phich_duration, phich_resource, n_ctrl):
+    """The REGs of a control region of n_ctrl symbols: dict with `pcfich` and `phich` (sets of (l, k0)), `pdcch` (the
+    PDCCH REGs (l, k0) in the order m' of 6.8.5) and `quad_reg` (quadruplet j is on REG pdcch[quad_reg[j]])."""
+    W = 12 * R
+    pcf = {(0, (6 * (n_id_cell % (2 * R)) + 6 * (i * R // 2)) % W) for i in range(4)}
+    avail = [[k0 for k0 in range(0, W, 6 if reg_is_six(l, n_ports, cp_type) else 4) if (l, k0) not in pcf] for l in range(4)]
+    ng = {1: (1, 6), 2: (1, 2), 3: (1, 1), 4: (2, 1)}[phich_resource]
+    m_u = -(-ng[0] * R // (8 * ng[1]))
+    n0 = len(avail[0])
+    phich = set()
+    for m in range(m_u):
+        for i in range(3):
+            l = i if phich_duration == 2 else 0
+            nl = len(avail[l])
+            phich.add((l, avail[l][(n_id_cell * nl // n0 + m + i * nl // 3) % nl]))
+    regs = [(l, k) for k in range(W) for l in range(n_ctrl)
+            if k % (6 if reg_is_six(l, n_ports, cp_type) else 4) == 0 and (l, k) not in pcf and (l, k) not in phich]
+    n = len(regs)
+    rows = -(-n // 32)
+    nd = 32 * rows - n
+    w = [r * 32 + _PERM[c] - nd for c in range(32) for r in range(rows) if r * 32 + _PERM[c] >= nd]
+    quad_reg = np.zeros(n, int)
+    for m in range(n):
+        quad_reg[w[(m + n_id_cell) % n]] = m
+    return dict(pcfich=pcf, phich=phich, pdcch=regs, quad_reg=quad_reg, n_reg=n, n_cce=n // 9)
+
+
+def dci_codeword(bits, rnti, L):
+    """The 72 L rate-matched bits of a DCI (36.212 5.3.3.2-4): CRC16 masked with the RNTI, tail-biting code."""
+    a = np.asarray(bits, np.uint8)
+    crc = O.crc16(a).astype(np.uint8) ^ np.array([(rnti >> (15 - i)) & 1 for i in range(16)], np.uint8)
+    c = np.concatenate([a, crc])
+    d = O.conv_encode(c).reshape(-1)
+    return d[ratematch_positions(72 * L, c.size)]
+
+
+def _precode(d, n_ports):
+    """Transmit diversity of a symbol sequence (6.3.4.3): [n_ports][len]; four ports: pair 2i on ports 0 and 2, 2i + 1
+    on ports 1 and 3."""
+    y = np.zeros((n_ports, d.size), complex)
+    if n_ports == 1:
+        y[0] = d
+        return y
+    for j in range(d.size // 2):
+        a, b = (0, 1) if n_ports == 2 else ((0, 2) if j % 2 == 0 else (1, 3))
+        y[a, 2 * j], y[a, 2 * j + 1] = d[2 * j] / np.sqrt(2), d[2 * j + 1] / np.sqrt(2)
+        y[b, 2 * j], y[b, 2 * j + 1] = -np.conj(d[2 * j + 1]) / np.sqrt(2), np.conj(d[2 * j]) / np.sqrt(2)
+    return y
+
+
+def _write_control(X, cell, n_symb):
+    """cell["pdcch"]: DCIs (sf, rnti, fmt, L, cce, bits), sf a grid subframe or (period, phase) for every subframe u with
+    u mod period = phase.  Each subframe's control region (cell["cfi"]) is cleared but for its CRS; its PHICH REGs get a
+    fixed PN QPSK sequence on port 0, its DCIs are encoded, placed at their CCEs, scrambled (6.8.2), precoded, permuted and
+    mapped (6.8.5), and the rest of its PDCCH quadruplets are NIL (zero), or random QPSK from cell["pdcch_fill"] (a
+    seed) when it is given."""
+    if "cfi" not in cell:
+        raise ValueError('a cell with "pdcch" needs "cfi": the control region is sized by it')
+    R, P, cp, nid = cell["n_rb_dl"], cell["n_ports"], cell["cp_type"], cell["n_id_cell"]
+    seq, dur, res = list(cell["cfi"]), cell["phich_duration"], cell["phich_resource"]
+    fill = np.random.default_rng(cell["pdcch_fill"]) if "pdcch_fill" in cell else None
+    _, shift = O.rs_dl(nid, cp)
+    for u in range(X.shape[1] // (2 * n_symb)):
+        n_ctrl = n_ctrl_of(seq[u % len(seq)], R, dur)
+        t = control_regs(R, P, cp, nid, dur, res, n_ctrl)
+        g0 = 2 * n_symb * u
+        for l in range(n_ctrl):
+            keep = np.zeros(12 * R, bool)
+            for p in range(P):
+                sh = shift[(2 * u % 20) * n_symb + l, p]
+                if not np.isnan(sh):
+                    keep[int(sh) + 6 * np.arange(2 * R)] = True
+            X[:, g0 + l, ~keep] = 0
+        ph = sorted(t["phich"])
+        b = O.lte_pn(nid + 1, 8 * len(ph)).astype(float)
+        for i, (l, k0) in enumerate(ph):
+            X[0, g0 + l, reg_data_cols(l, k0, nid, P, cp)] = ((1 - 2 * b[8 * i:8 * i + 8:2]) + 1j * (1 - 2 * b[8 * i + 1:8 * i + 8:2])) / np.sqrt(2)
+        n_bits = 8 * t["n_reg"]
+        bits = np.zeros(n_bits, np.uint8)
+        used = np.zeros(n_bits, bool)
+        for sf, rnti, fmt, L, cce, payload in cell["pdcch"]:
+            if (sf != u) if isinstance(sf, int) else (u % sf[0] != sf[1]):
+                continue
+            bits[72 * cce:72 * (cce + L)] = dci_codeword(payload, rnti, L)
+            used[72 * cce:72 * (cce + L)] = True
+        e = (bits ^ O.lte_pn((u % 10) * 512 + nid, n_bits)).astype(float)
+        d = ((1 - 2 * e[0::2]) + 1j * (1 - 2 * e[1::2])) / np.sqrt(2)
+        d[~used[0::2]] = 0
+        if fill is not None:
+            nil = ~used[0::2]
+            d[nil] = ((1 - 2 * fill.integers(0, 2, nil.sum())) + 1j * (1 - 2 * fill.integers(0, 2, nil.sum()))) / np.sqrt(2)
+        y = _precode(d, P)
+        for j in range(t["n_reg"]):
+            l, k0 = t["pdcch"][t["quad_reg"][j]]
+            X[:, g0 + l, reg_data_cols(l, k0, nid, P, cp)] = y[:, 4 * j:4 * j + 4]
 
 
 def channel_response(paths, f):
