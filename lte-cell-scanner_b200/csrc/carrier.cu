@@ -11,10 +11,8 @@
 //      (and twelve columns) in order, and thread 0 adds the RBs in order.  All sums are FP64, so a cell's record is the
 //      same on every run and independent of the other cells of the call.
 // Each cell is checked and its windows laid out on the host first (plan_cell, carrier_plan.cpp, from tfg_geometry); the
-// CRS signs and shifts come from RsDl (chain_host.cpp).  The grid, its checks and its staging are carrier_grid.cuh's,
-// which liblcs_cir.so shares.
-#include <new>
-
+// CRS signs and shifts come from RsDl (chain_host.cpp).  The grid and the host path of a call (grid_cells) are
+// carrier_grid.cuh's, which every module on the grid shares.
 #include "../../include/lcs_carrier.h"
 #include "carrier_grid.cuh"
 
@@ -133,84 +131,34 @@ __global__ void __launch_bounds__(MEAS_THREADS) carrier_meas_kernel(const float2
 using namespace lcs;
 using namespace lcs::carrier;
 
-struct lcs_carrier {
-  lcs_ctx* ctx = nullptr;
-  GridScratch g;                           // the recording's span, the staged tables and one chunk's grids
-  DevBuf<lcs_carrier_meas> d_out;
-  KernelClock clock;                       // both launches of each chunk
-};
-
-namespace {
-
-lcs_status cfail(const lcs_carrier* h, const std::string& msg) {
-  return fail(h->ctx, LCS_ERR_ARG, "lcs_carrier_cells: " + msg);
-}
-
-}  // namespace
+struct lcs_carrier : GridModule<lcs_carrier_meas> {};
 
 extern "C" {
 
-lcs_status lcs_carrier_create(lcs_ctx* ctx, lcs_carrier** out) {
-  if (!ctx || !out) return fail(ctx, LCS_ERR_ARG, "lcs_carrier_create: null argument");
-  lcs_carrier* h = new (std::nothrow) lcs_carrier();
-  if (!h) return fail(ctx, LCS_ERR_STATE, "lcs_carrier_create: out of memory");
-  h->ctx = ctx;
-  *out = h;
-  return LCS_OK;
-}
+lcs_status lcs_carrier_create(lcs_ctx* ctx, lcs_carrier** out) { return grid_create(ctx, out, "lcs_carrier_create"); }
 
-void lcs_carrier_destroy(lcs_carrier* h) {
-  if (!h) return;
-  cudaSetDevice(h->ctx->device);             // its buffers and events belong to the context's device
-  delete h;
-}
+void lcs_carrier_destroy(lcs_carrier* h) { grid_destroy(h); }
 
 lcs_status lcs_carrier_cells(lcs_carrier* h, const void* iq, int iq_format, int on_device, uint64_t n_in, double fs_in,
                              double fc_in, const lcs_cell* cells, uint32_t n_cells, double fs_programmed,
                              lcs_carrier_meas* out) {
-  if (!h) return LCS_ERR_ARG;
-  int D = 0;
-  const std::string bad = check_call(iq, iq_format, on_device, n_in, fs_in, fc_in, n_cells, cells, out, fs_programmed, D);
-  if (!bad.empty()) return cfail(h, bad);
-  if (!n_cells) return LCS_OK;
-  lcs_ctx* ctx = h->ctx;
-  LCS_CUDA(ctx, cudaSetDevice(ctx->device));
-  // every cell checked, and its windows laid out, before any device work
-  std::vector<CellPlan> ch;
-  long long lo, hi;
-  const std::string why = plan_cells(cells, n_cells, n_in, D, fs_in, fc_in, fs_programmed, ch, lo, hi);
-  if (!why.empty()) return cfail(h, why);
-  cudaStream_t st = ctx->streams[0];
-  const unsigned char* d_in;
-  long long base;
-  LCS_CUDA(ctx, h->g.prepare(iq, sample_bytes(iq_format), on_device, lo, hi, 128 * D, st, &d_in, &base));
-  LCS_CUDA(ctx, h->d_out.ensure(std::min(n_cells, CHUNK)));
-  ChunkTables t;
-  for (uint32_t c0 = 0; c0 < n_cells; c0 += CHUNK) {
-    const uint32_t nc = std::min(CHUNK, n_cells - c0);
-    LCS_CUDA(ctx, stage_chunk(h->g, &ch[c0], nc, nc * sizeof(MeasCell) + 16, t));
-    MeasCell* mc = h->g.up.take<MeasCell>(nc);
-    for (uint32_t i = 0; i < nc; i++) mc[i] = MeasCell{t.off[i], ch[c0 + i].R, ch[c0 + i].n_ports, ch[c0 + i].nw, 0};
-    LCS_CUDA(ctx, h->g.up.upload(st));
-    LCS_CUDA(ctx, cudaMemsetAsync(h->d_out.p, 0, nc * sizeof(lcs_carrier_meas), st));   // the records' padding too
-    LCS_CUDA(ctx, h->clock.begin(st));
-    if (!launch_grid(h->g, t, iq_format, d_in, base, fs_in, D, st)) return cfail(h, "no grid kernel for this iq_format");
-    carrier_meas_kernel<<<nc, MEAS_THREADS, 0, st>>>(h->g.d_grid.p, h->g.up.dev(t.rs), h->g.up.dev(t.shift),
-                                                     h->g.up.dev(mc), h->d_out.p);
-    ctx->launches += LCS_CARRIER_LAUNCHES_PER_CHUNK;
-    LCS_CUDA(ctx, cudaGetLastError());
-    LCS_CUDA(ctx, h->clock.end(st, LCS_CARRIER_LAUNCHES_PER_CHUNK));
-    LCS_CUDA(ctx, cudaMemcpyAsync(out + c0, h->d_out.p, nc * sizeof(lcs_carrier_meas), cudaMemcpyDeviceToHost, st));
-    LCS_CUDA(ctx, cudaStreamSynchronize(st));
-  }
-  return LCS_OK;
+  MeasCell* mc = nullptr;
+  return grid_cells(
+      h, "lcs_carrier_cells", CHUNK, LCS_CARRIER_LAUNCHES_PER_CHUNK, iq, iq_format, on_device, n_in, fs_in, fc_in, cells,
+      n_cells, fs_programmed, out, plan_cell, [](uint32_t n) { return n * sizeof(MeasCell) + 16; },
+      [&](const GridChunk& c) {
+        mc = h->g.up.take<MeasCell>(c.n);
+        for (uint32_t i = 0; i < c.n; i++) mc[i] = MeasCell{c.t.off[i], c.plan[i].R, c.plan[i].n_ports, c.plan[i].nw, 0};
+        return cudaSuccess;
+      },
+      [&](const GridChunk& c) {
+        carrier_meas_kernel<<<c.n, MEAS_THREADS, 0, c.st>>>(h->g.d_grid.p, h->g.up.dev(c.t.rs), h->g.up.dev(c.t.shift),
+                                                            h->g.up.dev(mc), h->d_out.p);
+      });
 }
 
 lcs_status lcs_carrier_timing_read(lcs_carrier* h, double* kernel_ms, uint64_t* launches) {
-  if (!h) return LCS_ERR_ARG;
-  if (!kernel_ms || !launches) return fail(h->ctx, LCS_ERR_ARG, "lcs_carrier_timing_read: null pointer");
-  LCS_CUDA(h->ctx, h->clock.read(kernel_ms, launches));
-  return LCS_OK;
+  return grid_timing_read(h, kernel_ms, launches, "lcs_carrier_timing_read");
 }
 
 }  // extern "C"

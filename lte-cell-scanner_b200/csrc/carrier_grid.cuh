@@ -1,10 +1,11 @@
 // carrier_grid.cuh - the full-bandwidth OFDM grid of found cells, from the wideband recording they were found in: the grid
-// Y[t][c] of include/lcs_carrier.h, built for the CRS symbols only.  Shared by liblcs_carrier.so (carrier.cu) and
-// liblcs_cir.so (cir.cu): both check a call's arguments and plan its cells the same way (check_call, plan_cell), stage
-// each chunk's windows and CRS tables the same way (stage_chunk) and launch the same carrier_grid_kernel.
+// Y[t][c] of include/lcs_carrier.h, built for the CRS symbols only, and the one host path of every module on it:
+// liblcs_carrier.so (carrier.cu), liblcs_cir.so (cir.cu), liblcs_pcfich.so (pcfich.cu) and liblcs_pdcch.so (pdcch.cu).
+// Each module's handle is a GridModule, and its lcs_X_cells is grid_cells with the module's planner, slices and kernels.
 #pragma once
 #include <cmath>
 #include <limits>
+#include <new>
 #include <string>
 #include <vector>
 
@@ -100,22 +101,6 @@ inline std::string check_call(const void* iq, int iq_format, int on_device, uint
   if (!n_in || n_in / D >= (1ull << 31)) return "n_in must be positive and below 2^31 D";
   if (!std::isfinite(fc_in)) return "fc_in must be finite";
   if (!(std::isfinite(fs_programmed) && fs_programmed > 0)) return "fs_programmed must be finite and positive";
-  return "";
-}
-
-// Every cell checked and its windows laid out (plan_cell): "" or why a cell cannot be measured, naming it; [lo, hi) is
-// the span of the recording the windows cover.
-inline std::string plan_cells(const lcs_cell* cells, uint32_t n_cells, uint64_t n_in, int D, double fs_in, double fc_in,
-                              double fs_programmed, std::vector<CellPlan>& ch, long long& lo, long long& hi) {
-  ch.assign(n_cells, CellPlan());
-  lo = std::numeric_limits<long long>::max();
-  hi = 0;
-  for (uint32_t i = 0; i < n_cells; i++) {
-    const std::string why = plan_cell(cells[i], n_in, D, fs_in, fc_in, fs_programmed, ch[i]);
-    if (!why.empty()) return "cell " + std::to_string(i) + ": " + why;
-    lo = std::min(lo, ch[i].q.front());
-    hi = std::max(hi, ch[i].q.back() + 128ll * D);
-  }
   return "";
 }
 
@@ -225,6 +210,112 @@ inline bool launch_grid(const GridScratch& g, const ChunkTables& t, int iq_forma
   return StreamFormats::dispatch(iq_format, [&](auto FMT) {
            carrier_grid_kernel<FMT><<<(unsigned)((t.n_win + per - 1) / per), THREADS, 0, st>>>(P);
          }) == LCS_OK;
+}
+
+// ---- the host path of every module on the grid ------------------------------------------------------------------------
+// What a module's handle keeps between calls; each module's opaque handle type derives from it.
+template <class Meas>
+struct GridModule {
+  lcs_ctx* ctx = nullptr;
+  GridScratch g;                     // the recording's span, the staged tables and one chunk's grids
+  DevBuf<Meas> d_out;                // one chunk's records
+  KernelClock clock;                 // the launches of each chunk
+};
+
+// lcs_X_create, lcs_X_destroy and lcs_X_timing_read of a module's handle type H; fn is the C function's name.
+template <class H>
+lcs_status grid_create(lcs_ctx* ctx, H** out, const char* fn) {
+  if (!ctx || !out) return fail(ctx, LCS_ERR_ARG, std::string(fn) + ": null argument");
+  H* h = new (std::nothrow) H();
+  if (!h) return fail(ctx, LCS_ERR_STATE, std::string(fn) + ": out of memory");
+  h->ctx = ctx;
+  *out = h;
+  return LCS_OK;
+}
+
+template <class H>
+void grid_destroy(H* h) {
+  if (!h) return;
+  cudaSetDevice(h->ctx->device);     // its buffers and events belong to the context's device
+  delete h;
+}
+
+template <class H>
+lcs_status grid_timing_read(H* h, double* kernel_ms, uint64_t* launches, const char* fn) {
+  if (!h) return LCS_ERR_ARG;
+  if (!kernel_ms || !launches) return fail(h->ctx, LCS_ERR_ARG, std::string(fn) + ": null pointer");
+  LCS_CUDA(h->ctx, h->clock.read(kernel_ms, launches));
+  return LCS_OK;
+}
+
+// One chunk of a call, as a module's fill and launch see it.
+struct GridChunk {
+  ChunkTables t;                     // its staged tables and grids
+  const CellPlan* plan = nullptr;    // its cells' plans
+  const lcs_cell* cell = nullptr;    // and its cells
+  uint32_t n = 0;
+  int D = 0;
+  cudaStream_t st = nullptr;
+};
+
+struct NoHostStep {
+  template <class Meas> void operator()(Meas&, const CellPlan&) const {}
+};
+
+// lcs_X_cells of a module (fn its name, `chunk` cells per chunk, `launches` kernels per chunk).  The call's arguments are
+// checked, and every cell planned by plan (plan_cell's signature) before any device work; the span of the recording its
+// windows cover is uploaded.  Then each chunk, on the context's stream 0, is staged with bytes(n) more bytes for the
+// module's slices, which fill(chunk) takes and fills (readying the module's own device scratch too); it is uploaded, its
+// records zeroed, and carrier_grid_kernel and launch(chunk) run between the clock's events; its records are copied out,
+// the stream synchronised and done(record, plan) run on each.
+template <class H, class Meas, class Plan, class Bytes, class Fill, class Launch, class Done = NoHostStep>
+lcs_status grid_cells(H* h, const char* fn, uint32_t chunk, uint64_t launches, const void* iq, int iq_format,
+                      int on_device, uint64_t n_in, double fs_in, double fc_in, const lcs_cell* cells, uint32_t n_cells,
+                      double fs_programmed, Meas* out, Plan plan, Bytes bytes, Fill fill, Launch launch,
+                      Done done = Done()) {
+  if (!h) return LCS_ERR_ARG;
+  lcs_ctx* ctx = h->ctx;
+  const std::string pre = std::string(fn) + ": ";
+  int D = 0;
+  const std::string bad = check_call(iq, iq_format, on_device, n_in, fs_in, fc_in, n_cells, cells, out, fs_programmed, D);
+  if (!bad.empty()) return fail(ctx, LCS_ERR_ARG, pre + bad);
+  if (!n_cells) return LCS_OK;
+  LCS_CUDA(ctx, cudaSetDevice(ctx->device));
+  std::vector<CellPlan> ch(n_cells);
+  long long lo = std::numeric_limits<long long>::max(), hi = 0;
+  for (uint32_t i = 0; i < n_cells; i++) {
+    const std::string why = plan(cells[i], n_in, D, fs_in, fc_in, fs_programmed, ch[i]);
+    if (!why.empty()) return fail(ctx, LCS_ERR_ARG, pre + "cell " + std::to_string(i) + ": " + why);
+    lo = std::min(lo, ch[i].q.front());
+    hi = std::max(hi, ch[i].q.back() + 128ll * D);
+  }
+  GridChunk c;
+  c.D = D;
+  c.st = ctx->streams[0];
+  const unsigned char* d_in;
+  long long base;
+  LCS_CUDA(ctx, h->g.prepare(iq, sample_bytes(iq_format), on_device, lo, hi, 128 * D, c.st, &d_in, &base));
+  LCS_CUDA(ctx, h->d_out.ensure(std::min(n_cells, chunk)));
+  for (uint32_t c0 = 0; c0 < n_cells; c0 += chunk) {
+    c.n = std::min(chunk, n_cells - c0);
+    c.plan = &ch[c0];
+    c.cell = cells + c0;
+    LCS_CUDA(ctx, stage_chunk(h->g, c.plan, c.n, bytes(c.n), c.t));
+    LCS_CUDA(ctx, fill(c));
+    LCS_CUDA(ctx, h->g.up.upload(c.st));
+    LCS_CUDA(ctx, cudaMemsetAsync(h->d_out.p, 0, c.n * sizeof(Meas), c.st));   // the records' padding too
+    LCS_CUDA(ctx, h->clock.begin(c.st));
+    if (!launch_grid(h->g, c.t, iq_format, d_in, base, fs_in, D, c.st))
+      return fail(ctx, LCS_ERR_ARG, pre + "no grid kernel for this iq_format");
+    launch(c);
+    ctx->launches += launches;
+    LCS_CUDA(ctx, cudaGetLastError());
+    LCS_CUDA(ctx, h->clock.end(c.st, launches));
+    LCS_CUDA(ctx, cudaMemcpyAsync(out + c0, h->d_out.p, c.n * sizeof(Meas), cudaMemcpyDeviceToHost, c.st));
+    LCS_CUDA(ctx, cudaStreamSynchronize(c.st));
+    for (uint32_t i = 0; i < c.n; i++) done(out[c0 + i], ch[c0 + i]);
+  }
+  return LCS_OK;
 }
 
 }  // namespace carrier

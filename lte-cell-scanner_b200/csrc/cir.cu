@@ -11,8 +11,6 @@
 //      last CTA of a (cell, port) to finish, which a device counter behind a fence tells it is last, walks the complete
 //      pdp in ascending tap order for the statistics.  Nothing depends on the order CTAs finish in, so a cell's record is
 //      bitwise the same whatever else the call measures.
-#include <new>
-
 #include "../../include/lcs_cir.h"
 #include "carrier_grid.cuh"
 
@@ -189,89 +187,43 @@ using namespace lcs;
 using namespace lcs::carrier;
 using namespace lcs::cir;
 
-struct lcs_cir {
-  lcs_ctx* ctx = nullptr;
-  GridScratch g;                                 // the recording's span, the staged tables and one chunk's grids
+struct lcs_cir : GridModule<lcs_cir_meas> {
   DevBuf<double> d_noise;                        // [CHUNK][4][TAPS] noise per tap
   DevBuf<unsigned int> d_count;                  // [CHUNK][4] finished tap blocks
-  DevBuf<lcs_cir_meas> d_out;
-  KernelClock clock;                             // both launches of each chunk
 };
-
-namespace {
-
-lcs_status cfail(const lcs_cir* h, const std::string& msg) { return fail(h->ctx, LCS_ERR_ARG, "lcs_cir_cells: " + msg); }
-
-}  // namespace
 
 extern "C" {
 
-lcs_status lcs_cir_create(lcs_ctx* ctx, lcs_cir** out) {
-  if (!ctx || !out) return fail(ctx, LCS_ERR_ARG, "lcs_cir_create: null argument");
-  lcs_cir* h = new (std::nothrow) lcs_cir();
-  if (!h) return fail(ctx, LCS_ERR_STATE, "lcs_cir_create: out of memory");
-  h->ctx = ctx;
-  *out = h;
-  return LCS_OK;
-}
+lcs_status lcs_cir_create(lcs_ctx* ctx, lcs_cir** out) { return grid_create(ctx, out, "lcs_cir_create"); }
 
-void lcs_cir_destroy(lcs_cir* h) {
-  if (!h) return;
-  cudaSetDevice(h->ctx->device);                 // its buffers and events belong to the context's device
-  delete h;
-}
+void lcs_cir_destroy(lcs_cir* h) { grid_destroy(h); }
 
 lcs_status lcs_cir_cells(lcs_cir* h, const void* iq, int iq_format, int on_device, uint64_t n_in, double fs_in,
                          double fc_in, const lcs_cell* cells, uint32_t n_cells, double fs_programmed, lcs_cir_meas* out) {
-  if (!h) return LCS_ERR_ARG;
-  int D = 0;
-  const std::string bad = check_call(iq, iq_format, on_device, n_in, fs_in, fc_in, n_cells, cells, out, fs_programmed, D);
-  if (!bad.empty()) return cfail(h, bad);
-  if (!n_cells) return LCS_OK;
-  lcs_ctx* ctx = h->ctx;
-  LCS_CUDA(ctx, cudaSetDevice(ctx->device));
-  std::vector<CellPlan> ch;                      // every cell checked, and its windows laid out, before any device work
-  long long lo, hi;
-  const std::string why = plan_cells(cells, n_cells, n_in, D, fs_in, fc_in, fs_programmed, ch, lo, hi);
-  if (!why.empty()) return cfail(h, why);
-  cudaStream_t st = ctx->streams[0];
-  const unsigned char* d_in;
-  long long base;
-  LCS_CUDA(ctx, h->g.prepare(iq, sample_bytes(iq_format), on_device, lo, hi, 128 * D, st, &d_in, &base));
-  const uint32_t n_chunk = std::min(n_cells, CHUNK);
-  LCS_CUDA(ctx, h->d_out.ensure(n_chunk));
-  LCS_CUDA(ctx, h->d_noise.ensure((size_t)n_chunk * 4 * TAPS));
-  LCS_CUDA(ctx, h->d_count.ensure((size_t)n_chunk * 4));
-  ChunkTables t;
-  for (uint32_t c0 = 0; c0 < n_cells; c0 += CHUNK) {
-    const uint32_t nc = std::min(CHUNK, n_cells - c0);
-    LCS_CUDA(ctx, stage_chunk(h->g, &ch[c0], nc, nc * sizeof(CirCell) + 16, t));
-    CirCell* cc = h->g.up.take<CirCell>(nc);
-    for (uint32_t i = 0; i < nc; i++) {
-      const CellPlan& c = ch[c0 + i];
-      cc[i] = CirCell{t.off[i], D * cells[c0 + i].frame_start / fs_in, c.R, c.n_ports, c.nw, 0};
-    }
-    LCS_CUDA(ctx, h->g.up.upload(st));
-    LCS_CUDA(ctx, cudaMemsetAsync(h->d_out.p, 0, nc * sizeof(lcs_cir_meas), st));   // the records' padding too
-    LCS_CUDA(ctx, cudaMemsetAsync(h->d_count.p, 0, nc * 4 * sizeof(unsigned int), st));
-    LCS_CUDA(ctx, h->clock.begin(st));
-    if (!launch_grid(h->g, t, iq_format, d_in, base, fs_in, D, st)) return cfail(h, "no grid kernel for this iq_format");
-    cir_kernel<<<dim3(TAP_BLOCKS, 4, nc), CIR_THREADS, 0, st>>>(h->g.d_grid.p, h->g.up.dev(t.rs), h->g.up.dev(t.shift),
-                                                               h->g.up.dev(cc), h->d_noise.p, h->d_count.p, h->d_out.p);
-    ctx->launches += LCS_CIR_LAUNCHES_PER_CHUNK;
-    LCS_CUDA(ctx, cudaGetLastError());
-    LCS_CUDA(ctx, h->clock.end(st, LCS_CIR_LAUNCHES_PER_CHUNK));
-    LCS_CUDA(ctx, cudaMemcpyAsync(out + c0, h->d_out.p, nc * sizeof(lcs_cir_meas), cudaMemcpyDeviceToHost, st));
-    LCS_CUDA(ctx, cudaStreamSynchronize(st));
-  }
-  return LCS_OK;
+  CirCell* cc = nullptr;
+  return grid_cells(
+      h, "lcs_cir_cells", CHUNK, LCS_CIR_LAUNCHES_PER_CHUNK, iq, iq_format, on_device, n_in, fs_in, fc_in, cells, n_cells,
+      fs_programmed, out, plan_cell, [](uint32_t n) { return n * sizeof(CirCell) + 16; },
+      [&](const GridChunk& c) {
+        cc = h->g.up.take<CirCell>(c.n);
+        for (uint32_t i = 0; i < c.n; i++) {
+          const CellPlan& p = c.plan[i];
+          cc[i] = CirCell{c.t.off[i], c.D * c.cell[i].frame_start / fs_in, p.R, p.n_ports, p.nw, 0};
+        }
+        // the first chunk is the largest: it sizes the scratch for the call
+        cudaError_t e = h->d_noise.ensure((size_t)c.n * 4 * TAPS);
+        if (e == cudaSuccess) e = h->d_count.ensure((size_t)c.n * 4);
+        return e == cudaSuccess ? cudaMemsetAsync(h->d_count.p, 0, c.n * 4 * sizeof(unsigned int), c.st) : e;
+      },
+      [&](const GridChunk& c) {
+        cir_kernel<<<dim3(TAP_BLOCKS, 4, c.n), CIR_THREADS, 0, c.st>>>(h->g.d_grid.p, h->g.up.dev(c.t.rs),
+                                                                       h->g.up.dev(c.t.shift), h->g.up.dev(cc),
+                                                                       h->d_noise.p, h->d_count.p, h->d_out.p);
+      });
 }
 
 lcs_status lcs_cir_timing_read(lcs_cir* h, double* kernel_ms, uint64_t* launches) {
-  if (!h) return LCS_ERR_ARG;
-  if (!kernel_ms || !launches) return fail(h->ctx, LCS_ERR_ARG, "lcs_cir_timing_read: null pointer");
-  LCS_CUDA(h->ctx, h->clock.read(kernel_ms, launches));
-  return LCS_OK;
+  return grid_timing_read(h, kernel_ms, launches, "lcs_cir_timing_read");
 }
 
 }  // extern "C"

@@ -3,7 +3,8 @@
 //
 // pcfich_kernel runs one CTA per cell.  Thread (s, j) equalises pair j of subframe s (rules 2-4) into shared memory; then
 // one thread per subframe decides it (rule 5) and one thread counts the decisions (rule 6), every sum in FP64 in a fixed
-// order, so a cell's record is bitwise the same whatever else the call decodes.
+// order, so a cell's record is bitwise the same whatever else the call decodes.  pcfich_fill and pcfich_launch stage and
+// launch it in a chunk of either module.
 #pragma once
 #include "../../include/lcs_pcfich.h"
 #include "carrier_grid.cuh"
@@ -165,6 +166,30 @@ inline void pcfich_scrambling(int n_id, uint32_t* scr) {
     for (int b = 0; b < 32; b++) w |= (uint32_t)(bits[b] & 1) << b;
     scr[sf] = w;
   }
+}
+
+// The PCFICH stage of a chunk of grid_cells: pcfich_kernel's slices of the staging (pcfich_bytes of them for n cells),
+// taken and filled by pcfich_fill, and its launch on the chunk's grids into out [n].
+struct PcfichSlices {
+  PcfichCell* cell;
+  uint32_t* scr;                                 // [cell][10]
+};
+
+inline size_t pcfich_bytes(uint32_t n) { return n * sizeof(PcfichCell) + 16 + n * 10 * sizeof(uint32_t) + 16; }
+
+inline PcfichSlices pcfich_fill(GridScratch& g, const GridChunk& c) {
+  const PcfichSlices s{g.up.take<PcfichCell>(c.n), g.up.take<uint32_t>(c.n * 10)};
+  for (uint32_t i = 0; i < c.n; i++) {
+    const CellPlan& p = c.plan[i];
+    s.cell[i] = PcfichCell{c.t.off[i], p.R, p.n_ports, p.nw, p.n_id_cell};
+    pcfich_scrambling(p.n_id_cell, s.scr + i * 10);
+  }
+  return s;
+}
+
+inline void pcfich_launch(const GridScratch& g, const GridChunk& c, const PcfichSlices& s, lcs_pcfich_meas* out) {
+  pcfich_kernel<<<c.n, PC_THREADS, 0, c.st>>>(g.d_grid.p, g.up.dev(c.t.rs), g.up.dev(c.t.shift), g.up.dev(s.cell),
+                                              g.up.dev(s.scr), out);
 }
 
 }  // namespace pcfich

@@ -10,8 +10,6 @@
 //      over trellis states; then one thread resolves the duplicates and writes the subframe's record (rule 12).  Every
 //      sum is FP64 in a fixed order, so a cell's record is bitwise the same whatever else the call decodes.
 // The host then parses each DCI's fields and counts the cell's DCIs (rule 13).
-#include <new>
-
 #include "../../include/lcs_pdcch.h"
 #include "pcfich_kernel.cuh"
 #include "pdcch_plan.hpp"
@@ -291,18 +289,41 @@ using namespace lcs;
 using namespace lcs::carrier;
 using namespace lcs::pdcch;
 
-struct lcs_pdcch {
-  lcs_ctx* ctx = nullptr;
-  GridScratch g;                                 // the recording's span, the staged tables and one chunk's grids
+struct lcs_pdcch : GridModule<lcs_pdcch_meas> {
   DevBuf<lcs_pcfich_meas> d_pc;                  // one chunk's CFI decisions
-  DevBuf<lcs_pdcch_meas> d_out;
-  KernelClock clock;                             // the three launches of each chunk
 };
 
 namespace {
 
-lcs_status pfail(const lcs_pdcch* h, const std::string& msg) {
-  return fail(h->ctx, LCS_ERR_ARG, "lcs_pdcch_cells: " + msg);
+// One cell's PdcchCell (rules 1-10 of lcs_pdcch.h): its control region tables for every n_ctrl, the DCI sizes,
+// rate-matching positions and scrambling words.
+PdcchCell pdcch_cell(const CellPlan& c, const lcs_cell& cell, unsigned long long off) {
+  PdcchCell p = {};
+  p.off = off;
+  p.R = c.R;
+  p.n_ports = c.n_ports;
+  p.nw = c.nw;
+  p.n_id = c.n_id_cell;
+  p.cp_type = c.cp_type;
+  p.phich_duration = cell.phich_duration;
+  p.size[0] = size_1a(c.R);
+  p.size[1] = size_1c(c.R);
+  for (int f = 0; f < 2; f++) {
+    p.K[f] = p.size[f] + 16;
+    const std::vector<uint8_t> pos = ratematch_positions(p.K[f]);
+    for (size_t b = 0; b < pos.size(); b++) {
+      p.pos[f][b] = pos[b];
+      p.inv[f][pos[b]] = (uint8_t)b;
+    }
+  }
+  for (int n = 1; n <= n_max(c.R); n++) {
+    const CtrlTable ct = control_table(c.R, c.n_ports, c.cp_type, c.n_id_cell, cell.phich_duration, cell.phich_resource, n);
+    p.n_reg[n - 1] = ct.n_reg;
+    p.n_cce[n - 1] = ct.n_cce;
+    std::copy(ct.quad.begin(), ct.quad.end(), p.quad[n - 1]);
+  }
+  for (int u = 0; u < 10; u++) scrambling(c.n_id_cell, u, p.scr[u]);
+  return p;
 }
 
 // Rule 13 on the host: each DCI's fields and the cell's counts.
@@ -327,107 +348,35 @@ void finish(lcs_pdcch_meas& m, int R) {
 
 extern "C" {
 
-lcs_status lcs_pdcch_create(lcs_ctx* ctx, lcs_pdcch** out) {
-  if (!ctx || !out) return fail(ctx, LCS_ERR_ARG, "lcs_pdcch_create: null argument");
-  lcs_pdcch* h = new (std::nothrow) lcs_pdcch();
-  if (!h) return fail(ctx, LCS_ERR_STATE, "lcs_pdcch_create: out of memory");
-  h->ctx = ctx;
-  *out = h;
-  return LCS_OK;
-}
+lcs_status lcs_pdcch_create(lcs_ctx* ctx, lcs_pdcch** out) { return grid_create(ctx, out, "lcs_pdcch_create"); }
 
-void lcs_pdcch_destroy(lcs_pdcch* h) {
-  if (!h) return;
-  cudaSetDevice(h->ctx->device);                 // its buffers and events belong to the context's device
-  delete h;
-}
+void lcs_pdcch_destroy(lcs_pdcch* h) { grid_destroy(h); }
 
 lcs_status lcs_pdcch_cells(lcs_pdcch* h, const void* iq, int iq_format, int on_device, uint64_t n_in, double fs_in,
                            double fc_in, const lcs_cell* cells, uint32_t n_cells, double fs_programmed,
                            lcs_pdcch_meas* out) {
-  if (!h) return LCS_ERR_ARG;
-  int D = 0;
-  const std::string bad = check_call(iq, iq_format, on_device, n_in, fs_in, fc_in, n_cells, cells, out, fs_programmed, D);
-  if (!bad.empty()) return pfail(h, bad);
-  if (!n_cells) return LCS_OK;
-  lcs_ctx* ctx = h->ctx;
-  LCS_CUDA(ctx, cudaSetDevice(ctx->device));
-  std::vector<CellPlan> ch(n_cells);             // every cell checked, and its windows laid out, before any device work
-  long long lo = std::numeric_limits<long long>::max(), hi = 0;
-  for (uint32_t i = 0; i < n_cells; i++) {
-    const std::string why = plan_pdcch(cells[i], n_in, D, fs_in, fc_in, fs_programmed, ch[i]);
-    if (!why.empty()) return pfail(h, "cell " + std::to_string(i) + ": " + why);
-    lo = std::min(lo, ch[i].q.front());
-    hi = std::max(hi, ch[i].q.back() + 128ll * D);
-  }
-  cudaStream_t st = ctx->streams[0];
-  const unsigned char* d_in;
-  long long base;
-  LCS_CUDA(ctx, h->g.prepare(iq, sample_bytes(iq_format), on_device, lo, hi, 128 * D, st, &d_in, &base));
-  LCS_CUDA(ctx, h->d_pc.ensure(std::min(n_cells, CHUNK)));
-  LCS_CUDA(ctx, h->d_out.ensure(std::min(n_cells, CHUNK)));
-  ChunkTables t;
-  for (uint32_t c0 = 0; c0 < n_cells; c0 += CHUNK) {
-    const uint32_t nc = std::min(CHUNK, n_cells - c0);
-    LCS_CUDA(ctx, stage_chunk(h->g, &ch[c0], nc,
-                              nc * (sizeof(pcfich::PcfichCell) + 10 * sizeof(uint32_t) + sizeof(PdcchCell)) + 3 * 16, t));
-    pcfich::PcfichCell* pc = h->g.up.take<pcfich::PcfichCell>(nc);
-    uint32_t* scr = h->g.up.take<uint32_t>(nc * 10);
-    PdcchCell* pd = h->g.up.take<PdcchCell>(nc);
-    for (uint32_t i = 0; i < nc; i++) {
-      const CellPlan& c = ch[c0 + i];
-      const lcs_cell& cell = cells[c0 + i];
-      pc[i] = pcfich::PcfichCell{t.off[i], c.R, c.n_ports, c.nw, c.n_id_cell};
-      pcfich::pcfich_scrambling(c.n_id_cell, scr + i * 10);
-      PdcchCell& p = pd[i];
-      p = PdcchCell{};
-      p.off = t.off[i];
-      p.R = c.R;
-      p.n_ports = c.n_ports;
-      p.nw = c.nw;
-      p.n_id = c.n_id_cell;
-      p.cp_type = c.cp_type;
-      p.phich_duration = cell.phich_duration;
-      p.size[0] = size_1a(c.R);
-      p.size[1] = size_1c(c.R);
-      for (int f = 0; f < 2; f++) {
-        p.K[f] = p.size[f] + 16;
-        const std::vector<uint8_t> pos = ratematch_positions(p.K[f]);
-        for (size_t b = 0; b < pos.size(); b++) {
-          p.pos[f][b] = pos[b];
-          p.inv[f][pos[b]] = (uint8_t)b;
-        }
-      }
-      for (int n = 1; n <= n_max(c.R); n++) {
-        const CtrlTable ct = control_table(c.R, c.n_ports, c.cp_type, c.n_id_cell, cell.phich_duration, cell.phich_resource, n);
-        p.n_reg[n - 1] = ct.n_reg;
-        p.n_cce[n - 1] = ct.n_cce;
-        std::copy(ct.quad.begin(), ct.quad.end(), p.quad[n - 1]);
-      }
-      for (int u = 0; u < 10; u++) scrambling(c.n_id_cell, u, p.scr[u]);
-    }
-    LCS_CUDA(ctx, h->g.up.upload(st));
-    LCS_CUDA(ctx, h->clock.begin(st));
-    if (!launch_grid(h->g, t, iq_format, d_in, base, fs_in, D, st)) return pfail(h, "no grid kernel for this iq_format");
-    pcfich::pcfich_kernel<<<nc, pcfich::PC_THREADS, 0, st>>>(h->g.d_grid.p, h->g.up.dev(t.rs), h->g.up.dev(t.shift),
-                                                             h->g.up.dev(pc), h->g.up.dev(scr), h->d_pc.p);
-    pdcch_kernel<<<nc * N_SF, PD_THREADS, 0, st>>>(h->g.d_grid.p, h->g.up.dev(t.rs), h->g.up.dev(t.shift), h->g.up.dev(pd),
-                                                   h->d_pc.p, h->d_out.p);
-    ctx->launches += LCS_PDCCH_LAUNCHES_PER_CHUNK;
-    LCS_CUDA(ctx, cudaGetLastError());
-    LCS_CUDA(ctx, h->clock.end(st, LCS_PDCCH_LAUNCHES_PER_CHUNK));
-    LCS_CUDA(ctx, cudaMemcpyAsync(out + c0, h->d_out.p, nc * sizeof(lcs_pdcch_meas), cudaMemcpyDeviceToHost, st));
-    LCS_CUDA(ctx, cudaStreamSynchronize(st));
-    for (uint32_t i = 0; i < nc; i++) finish(out[c0 + i], ch[c0 + i].R);
-  }
-  return LCS_OK;
+  pcfich::PcfichSlices s{};
+  PdcchCell* pd = nullptr;
+  return grid_cells(
+      h, "lcs_pdcch_cells", CHUNK, LCS_PDCCH_LAUNCHES_PER_CHUNK, iq, iq_format, on_device, n_in, fs_in, fc_in, cells,
+      n_cells, fs_programmed, out, plan_pdcch,
+      [](uint32_t n) { return pcfich::pcfich_bytes(n) + n * sizeof(PdcchCell) + 16; },
+      [&](const GridChunk& c) {
+        s = pcfich::pcfich_fill(h->g, c);
+        pd = h->g.up.take<PdcchCell>(c.n);
+        for (uint32_t i = 0; i < c.n; i++) pd[i] = pdcch_cell(c.plan[i], c.cell[i], c.t.off[i]);
+        return h->d_pc.ensure(c.n);              // the first chunk is the largest: it sizes d_pc for the call
+      },
+      [&](const GridChunk& c) {
+        pcfich::pcfich_launch(h->g, c, s, h->d_pc.p);
+        pdcch_kernel<<<c.n * N_SF, PD_THREADS, 0, c.st>>>(h->g.d_grid.p, h->g.up.dev(c.t.rs), h->g.up.dev(c.t.shift),
+                                                          h->g.up.dev(pd), h->d_pc.p, h->d_out.p);
+      },
+      [](lcs_pdcch_meas& m, const CellPlan& c) { finish(m, c.R); });
 }
 
 lcs_status lcs_pdcch_timing_read(lcs_pdcch* h, double* kernel_ms, uint64_t* launches) {
-  if (!h) return LCS_ERR_ARG;
-  if (!kernel_ms || !launches) return fail(h->ctx, LCS_ERR_ARG, "lcs_pdcch_timing_read: null pointer");
-  LCS_CUDA(h->ctx, h->clock.read(kernel_ms, launches));
-  return LCS_OK;
+  return grid_timing_read(h, kernel_ms, launches, "lcs_pdcch_timing_read");
 }
 
 }  // extern "C"

@@ -141,28 +141,27 @@ def meas_lib():
     return _bind(MEAS_LIB_PATH, MEAS_HEADER)
 
 
-def carrier_lib():
-    """liblcs_carrier.so (include/lcs_carrier.h); it takes the contexts of lib()."""
+def _grid_lib(path, header):
+    """A module on the whole-carrier grid (include/lcs_carrier.h, lcs_cir.h, lcs_pcfich.h or lcs_pdcch.h); it takes the
+    contexts of lib()."""
     lib()
-    return _bind(CARRIER_LIB_PATH, CARRIER_HEADER)
+    return _bind(path, header)
+
+
+def carrier_lib():
+    return _grid_lib(CARRIER_LIB_PATH, CARRIER_HEADER)
 
 
 def cir_lib():
-    """liblcs_cir.so (include/lcs_cir.h); it takes the contexts of lib()."""
-    lib()
-    return _bind(CIR_LIB_PATH, CIR_HEADER)
+    return _grid_lib(CIR_LIB_PATH, CIR_HEADER)
 
 
 def pcfich_lib():
-    """liblcs_pcfich.so (include/lcs_pcfich.h); it takes the contexts of lib()."""
-    lib()
-    return _bind(PCFICH_LIB_PATH, PCFICH_HEADER)
+    return _grid_lib(PCFICH_LIB_PATH, PCFICH_HEADER)
 
 
 def pdcch_lib():
-    """liblcs_pdcch.so (include/lcs_pdcch.h); it takes the contexts of lib()."""
-    lib()
-    return _bind(PDCCH_LIB_PATH, PDCCH_HEADER)
+    return _grid_lib(PDCCH_LIB_PATH, PDCCH_HEADER)
 
 
 def _p(a):
@@ -851,32 +850,47 @@ class CellMeasure(_Handle):
         return out
 
 
-def _measure_recording(h, fn, dtype, iq, fmt, fs_in, fc_in, cells, fs_programmed):
-    """fn (lcs_carrier_cells, lcs_cir_cells, lcs_pcfich_cells or lcs_pdcch_cells) of handle h on the recording iq: a record array of dtype, one row per
-    cell."""
-    iq_format = _iq_format(fmt)
-    cells = list(cells)
-    n = len(cells)
-    arr = (Cell * max(n, 1))()
-    for i, c in enumerate(cells):
-        C.memmove(C.addressof(arr) + i * C.sizeof(Cell), C.byref(c), C.sizeof(Cell))
-    if hasattr(iq, "is_cuda"):
-        if not (iq.is_cuda and iq.is_contiguous()):
-            raise ValueError("measure: expected a contiguous CUDA tensor")
-        shape = tuple(iq.shape) + ((2,) if iq.is_complex() else ())
-        import torch
-        torch.cuda.current_stream(iq.device).synchronize()
-        ptr, on_device = iq.data_ptr(), 1
-    else:
-        iq = _samples(iq, fmt)
-        shape, ptr, on_device = iq.shape, iq.ctypes.data, 0
-    if len(shape) != 2 or shape[1] != 2:
-        raise ValueError("expected a recording [n_in][2]")
-    out = np.zeros(n, dtype)
-    h._iq = iq                                          # kept alive until the call has returned
-    _chk(fn(h._h, ptr, iq_format, on_device, shape[0], fs_in, fc_in, arr, n, fs_programmed, _p(out)), h.ctx._h)
-    h._iq = None
-    return out
+class _GridModule(_Handle):
+    """A module on the whole-carrier grid: `_lib` is its library, `_prefix` the prefix of its C functions (lcs_carrier,
+    lcs_cir, lcs_pcfich or lcs_pdcch) and `_dtype` its record."""
+    _prefix = _dtype = None
+
+    def __init__(self, ctx):
+        self.ctx = ctx
+        self._h = C.c_void_p()
+        self._destroy = self._prefix + "_destroy"
+        self._timing_read = self._prefix + "_timing_read"
+        _chk(getattr(self._lib(), self._prefix + "_create")(ctx._h, C.byref(self._h)), ctx._h)
+
+    def measure(self, iq, fmt, fs_in, fc_in, cells, fs_programmed):
+        """Measure `cells` (Cells, or any struct of lcs_cell's layout) in the recording iq [n_in][2] of format fmt (ci16,
+        cs8, cu8 or cf32; complex64 [n_in] is accepted for cf32) at fs_in, centred on fc_in.  iq may be a contiguous
+        CUDA tensor (read in place; its stream is synchronised first).  Returns a record array of the module's dtype, one
+        row per cell."""
+        iq_format = _iq_format(fmt)
+        cells = list(cells)
+        n = len(cells)
+        arr = (Cell * max(n, 1))()
+        for i, c in enumerate(cells):
+            C.memmove(C.addressof(arr) + i * C.sizeof(Cell), C.byref(c), C.sizeof(Cell))
+        if hasattr(iq, "is_cuda"):
+            if not (iq.is_cuda and iq.is_contiguous()):
+                raise ValueError("measure: expected a contiguous CUDA tensor")
+            shape = tuple(iq.shape) + ((2,) if iq.is_complex() else ())
+            import torch
+            torch.cuda.current_stream(iq.device).synchronize()
+            ptr, on_device = iq.data_ptr(), 1
+        else:
+            iq = _samples(iq, fmt)
+            shape, ptr, on_device = iq.shape, iq.ctypes.data, 0
+        if len(shape) != 2 or shape[1] != 2:
+            raise ValueError("expected a recording [n_in][2]")
+        out = np.zeros(n, self._dtype)
+        self._iq = iq                                   # kept alive until the call has returned
+        _chk(getattr(self._lib(), self._prefix + "_cells")(self._h, ptr, iq_format, on_device, shape[0], fs_in, fc_in, arr,
+                                                           n, fs_programmed, _p(out)), self.ctx._h)
+        self._iq = None
+        return out
 
 
 # lcs_carrier_meas as a numpy record
@@ -886,25 +900,12 @@ CARRIER_MEAS = np.dtype([("rsrp", np.float64, 4), ("noise", np.float64, 4), ("si
 CARRIER_CHUNK = 32                    # LCS_CARRIER_CHUNK: cells per chunk, two launches each
 
 
-class CarrierMeasure(_Handle):
+class CarrierMeasure(_GridModule):
     """lcs_carrier: RSRP, RSRQ and SINR of found cells over all their resource blocks, and per resource block, measured on
     the wideband recording they were found in (DESIGN.md section 4.10)."""
-    _destroy = "lcs_carrier_destroy"
-    _timing_read = "lcs_carrier_timing_read"
     _lib = staticmethod(carrier_lib)
-
-    def __init__(self, ctx):
-        self.ctx = ctx
-        self._h = C.c_void_p()
-        _chk(carrier_lib().lcs_carrier_create(ctx._h, C.byref(self._h)), ctx._h)
-
-    def measure(self, iq, fmt, fs_in, fc_in, cells, fs_programmed):
-        """Measure `cells` (Cells, or any struct of lcs_cell's layout) in the recording iq [n_in][2] of format fmt (ci16,
-        cs8, cu8 or cf32; complex64 [n_in] is accepted for cf32) at fs_in, centred on fc_in.  iq may be a contiguous
-        CUDA tensor (read in place; its stream is synchronised first).  Returns a CARRIER_MEAS record array, one row per
-        cell."""
-        return _measure_recording(self, carrier_lib().lcs_carrier_cells, CARRIER_MEAS, iq, fmt, fs_in, fc_in, cells,
-                                  fs_programmed)
+    _prefix = "lcs_carrier"
+    _dtype = CARRIER_MEAS
 
 
 # lcs_cir_meas as a numpy record
@@ -920,22 +921,13 @@ def cir_delays():
     return (np.arange(CIR_TAPS) - 64) * (1 / 30.72e6)
 
 
-class CellImpulse(_Handle):
+class CellImpulse(_GridModule):
     """lcs_cir: the power delay profile of found cells over their whole carrier, with its first-path and peak delay, mean
     delay, RMS delay spread and the frame's arrival time, measured on the wideband recording they were found in (DESIGN.md
     section 4.11)."""
-    _destroy = "lcs_cir_destroy"
-    _timing_read = "lcs_cir_timing_read"
     _lib = staticmethod(cir_lib)
-
-    def __init__(self, ctx):
-        self.ctx = ctx
-        self._h = C.c_void_p()
-        _chk(cir_lib().lcs_cir_create(ctx._h, C.byref(self._h)), ctx._h)
-
-    def measure(self, iq, fmt, fs_in, fc_in, cells, fs_programmed):
-        """As CarrierMeasure.measure; returns a CIR_MEAS record array, one row per cell."""
-        return _measure_recording(self, cir_lib().lcs_cir_cells, CIR_MEAS, iq, fmt, fs_in, fc_in, cells, fs_programmed)
+    _prefix = "lcs_cir"
+    _dtype = CIR_MEAS
 
 
 # lcs_pcfich_meas as a numpy record
@@ -946,22 +938,12 @@ PCFICH_MEAS = np.dtype([("metric", np.float64, (PCFICH_SUBFRAMES, 3)), ("sinr", 
 PCFICH_CHUNK = 32                     # LCS_PCFICH_CHUNK: cells per chunk, two launches each
 
 
-class ControlFormat(_Handle):
+class ControlFormat(_GridModule):
     """lcs_pcfich: the control format indicator of found cells in every subframe, decoded from their PCFICH over the
     whole carrier of the wideband recording they were found in (DESIGN.md section 4.12)."""
-    _destroy = "lcs_pcfich_destroy"
-    _timing_read = "lcs_pcfich_timing_read"
     _lib = staticmethod(pcfich_lib)
-
-    def __init__(self, ctx):
-        self.ctx = ctx
-        self._h = C.c_void_p()
-        _chk(pcfich_lib().lcs_pcfich_create(ctx._h, C.byref(self._h)), ctx._h)
-
-    def measure(self, iq, fmt, fs_in, fc_in, cells, fs_programmed):
-        """As CarrierMeasure.measure; returns a PCFICH_MEAS record array, one row per cell."""
-        return _measure_recording(self, pcfich_lib().lcs_pcfich_cells, PCFICH_MEAS, iq, fmt, fs_in, fc_in, cells,
-                                  fs_programmed)
+    _prefix = "lcs_pcfich"
+    _dtype = PCFICH_MEAS
 
 
 # lcs_pdcch_dci and lcs_pdcch_meas as numpy records
@@ -981,20 +963,10 @@ PDCCH_MEAS = np.dtype([("dci", PDCCH_DCI, (PDCCH_SUBFRAMES, PDCCH_MAX_DCI)), ("c
 PDCCH_CHUNK = 32                      # LCS_PDCCH_CHUNK: cells per chunk, three launches each
 
 
-class ControlChannel(_Handle):
+class ControlChannel(_GridModule):
     """lcs_pdcch: the common-search-space DCIs (SI-, P- and RA-RNTI, formats 1A and 1C) of found cells in every
     subframe, decoded from their PDCCH over the whole carrier of the wideband recording they were found in (DESIGN.md
     section 4.13)."""
-    _destroy = "lcs_pdcch_destroy"
-    _timing_read = "lcs_pdcch_timing_read"
     _lib = staticmethod(pdcch_lib)
-
-    def __init__(self, ctx):
-        self.ctx = ctx
-        self._h = C.c_void_p()
-        _chk(pdcch_lib().lcs_pdcch_create(ctx._h, C.byref(self._h)), ctx._h)
-
-    def measure(self, iq, fmt, fs_in, fc_in, cells, fs_programmed):
-        """As CarrierMeasure.measure; returns a PDCCH_MEAS record array, one row per cell."""
-        return _measure_recording(self, pdcch_lib().lcs_pdcch_cells, PDCCH_MEAS, iq, fmt, fs_in, fc_in, cells,
-                                  fs_programmed)
+    _prefix = "lcs_pdcch"
+    _dtype = PDCCH_MEAS

@@ -116,8 +116,8 @@ def carrier_main(a):
     cells = cells * a.copies
     ctx = L.Context(0)
     d_iq = torch.from_numpy(iq).cuda()
-    m = (L.ControlChannel(ctx) if a.pdcch else L.ControlFormat(ctx) if a.pcfich else
-         L.CellImpulse(ctx) if a.cir else L.CarrierMeasure(ctx))
+    name = "pdcch" if a.pdcch else "pcfich" if a.pcfich else "cir" if a.cir else "carrier"
+    m = {"carrier": L.CarrierMeasure, "cir": L.CellImpulse, "pcfich": L.ControlFormat, "pdcch": L.ControlChannel}[name](ctx)
     m.measure(d_iq, "ci16", fs_in, FC, cells, 1.92e6)              # warm-up
     m.timing_read()
     wall = []
@@ -129,38 +129,17 @@ def carrier_main(a):
     m.close()
     n = len(cells)
     dev_s = ms / 1e3 / a.reps
-    if a.pdcch:
-        print(json.dumps({
-            "pdcch": True, "fs_in": fs_in, "cells": n, "reps": a.reps, "launches": launches,
-            "pdcch_device_us_per_cell": 1e6 * dev_s / n, "pdcch_host_us_per_cell": 1e6 * float(np.median(wall)) / n,
-            "gpu": gpu_name(),
-        }), flush=True)
-        ctx.close()
-        return
-    if a.pcfich:
-        print(json.dumps({
-            "pcfich": True, "fs_in": fs_in, "cells": n, "reps": a.reps, "launches": launches,
-            "pcfich_device_us_per_cell": 1e6 * dev_s / n, "pcfich_host_us_per_cell": 1e6 * float(np.median(wall)) / n,
-            "gpu": gpu_name(),
-        }), flush=True)
-        ctx.close()
-        return
-    if a.cir:
+    rec = {name: True, "fs_in": fs_in, "cells": n, "reps": a.reps, "launches": launches,
+           name + "_device_us_per_cell": 1e6 * dev_s / n, name + "_host_us_per_cell": 1e6 * float(np.median(wall)) / n}
+    if name == "carrier":
+        bytes_ = sum(carrier_bytes(c, D) for c in cells)
+        rec.update(carrier_bytes_per_cell=bytes_ / n, carrier_gbytes_per_s=bytes_ / dev_s / 1e9,
+                   bound_hbm_us_per_cell=1e6 * bytes_ / HBM_BPS / n)
+    if name == "cir":
         macs = sum(cir_macs(c) for c in cells)
-        print(json.dumps({
-            "cir": True, "fs_in": fs_in, "cells": n, "reps": a.reps, "launches": launches,
-            "cir_device_us_per_cell": 1e6 * dev_s / n, "cir_host_us_per_cell": 1e6 * float(np.median(wall)) / n,
-            "cir_cmacs_per_cell": macs / n, "cir_fp64_tflops": 8 * macs / dev_s / 1e12, "gpu": gpu_name(),
-        }), flush=True)
-        ctx.close()
-        return
-    bytes_ = sum(carrier_bytes(c, D) for c in cells)
-    print(json.dumps({
-        "carrier": True, "fs_in": fs_in, "cells": n, "reps": a.reps, "launches": launches,
-        "carrier_device_us_per_cell": 1e6 * dev_s / n, "carrier_host_us_per_cell": 1e6 * float(np.median(wall)) / n,
-        "carrier_bytes_per_cell": bytes_ / n, "carrier_gbytes_per_s": bytes_ / dev_s / 1e9,
-        "bound_hbm_us_per_cell": 1e6 * bytes_ / HBM_BPS / n, "gpu": gpu_name(),
-    }), flush=True)
+        rec.update(cir_cmacs_per_cell=macs / n, cir_fp64_tflops=8 * macs / dev_s / 1e12)
+    rec["gpu"] = gpu_name()
+    print(json.dumps(rec), flush=True)
     ctx.close()
 
 
