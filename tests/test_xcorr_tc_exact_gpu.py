@@ -115,7 +115,7 @@ def test_default_and_bench_grids_keep_the_tensor_cores():
 
 def test_fma32_rounds_once():
     """fma32 against exact rational arithmetic, on random operands and on sums that fall exactly between two float32
-    values in float64 (where rounding the float64 sum again would be wrong)."""
+    values in float64 (where rounding the float64 sum again would be wrong), with normal and subnormal results."""
     from fractions import Fraction
     rng = np.random.default_rng(3)
     a = (rng.standard_normal(4000) * 2.0 ** rng.integers(-20, 20, 4000)).astype(np.float32)
@@ -124,6 +124,17 @@ def test_fma32_rounds_once():
     # c = 1 + 2^-24 (a float32 midpoint in float64 once the tiny product is added and rounded away)
     a[:4] = np.float32(2.0 ** -30); b[:4] = np.float32([1.0, -1.0, 2.0 ** -25, -(2.0 ** -25)]); c[:4] = np.float32(1.0) + np.float32(2.0 ** -23)
     a[4:8] = np.float32(1.0 + 2.0 ** -23); b[4:8] = np.float32([2.0 ** -24, -(2.0 ** -24), 2.0 ** -25, 3.0]); c[4:8] = np.float32(1.0)
+    # subnormal results: a quarter of random operands below 2^-126, and a product 2^-150 (1 -+ 2^-46) that takes the
+    # float64 sum with an odd c = (2^9 + 1) 2^-149 exactly halfway between two subnormals
+    sub = slice(1000, 2000)
+    a[sub] = (rng.standard_normal(1000) * 2.0 ** rng.integers(-80, -60, 1000)).astype(np.float32)
+    b[sub] = (rng.standard_normal(1000) * 2.0 ** rng.integers(-80, -60, 1000)).astype(np.float32)
+    c[sub] = (rng.standard_normal(1000) * 2.0 ** rng.integers(-150, -127, 1000)).astype(np.float32)
+    a[8:12] = np.float32((1 + 2.0 ** -23) * 2.0 ** -75)
+    b[8:12] = np.float32([(1 - 2.0 ** -23) * 2.0 ** -75, -(1 - 2.0 ** -23) * 2.0 ** -75, (1 + 2.0 ** -23) * 2.0 ** -75,
+                          -(1 + 2.0 ** -23) * 2.0 ** -75])
+    c[8:12] = np.float32(2.0 ** -140 + 2.0 ** -149)
+    assert (np.abs(c[8:12]) < 2.0 ** -126).all() and (np.abs(c[sub]) < 2.0 ** -126).mean() > 0.9
     got = M.fma32(a, b, c)
     for x, y, z, g in zip(a, b, c, got):
         exact = Fraction(float(x)) * Fraction(float(y)) + Fraction(float(z))

@@ -196,19 +196,19 @@ def templates(td, S, f, fc_req, fc_prog, fs_prog):
 # ---------------------------------------------------------------------------------------------------------------------
 def fma32(a, b, c):
     """RN_float32(a * b + c) for float32 arrays with one rounding: the product is exact in float64, the sum is
-    float64 + TwoSum error, and a float64 sum that lies exactly between two float32 values is resolved by the error's sign."""
+    float64 + TwoSum error, and a float64 sum that lies exactly between two float32 values (normal or subnormal) is
+    resolved by the error's sign."""
     p = a.astype(np.float64) * b.astype(np.float64)
     c = c.astype(np.float64)
     s = p + c
     bb = s - p
     e = (p - (s - bb)) + (c - bb)
     r = s.astype(np.float32)
-    bits = s.view(np.int64)
-    tie = ((bits & 0x1FFFFFFF) == 0x10000000) & (e != 0) & (np.abs(s) >= 2.0 ** -126)
+    d = s - r.astype(np.float64)                                   # exact: s and r are within one float32 step
+    other = np.nextafter(r, np.where(d > 0, np.float32(np.inf), np.float32(-np.inf)))
+    tie = (d != 0) & (e != 0) & (2 * d == other.astype(np.float64) - r.astype(np.float64))
     if tie.any():
-        toward0 = (bits[tie] & ~np.int64(0x1FFFFFFF)).view(np.float64).astype(np.float32)      # exact: 24 significant bits
-        away = np.nextafter(toward0, np.copysign(np.float32(np.inf), toward0))
-        r[tie] = np.where((e[tie] > 0) == (s[tie] > 0), away, toward0)
+        r[tie] = np.where((e[tie] > 0) == (d[tie] > 0), other[tie], r[tie])
     return r
 
 
