@@ -88,18 +88,23 @@ extern "C" void xc_single(const float* x, int64_t n_x, const float* w, const int
 _lib = None
 
 
+def compile_model(source, name):
+    """A model's C++ arithmetic compiled into a temporary directory and loaded: -ffp-contract=off keeps every product
+    and sum separately rounded; std::fmaf is the one fused rounding (checked against fma32 by the tests)."""
+    d = tempfile.mkdtemp(prefix=name + "_")
+    src, so = os.path.join(d, "model.cpp"), os.path.join(d, "model.so")
+    with open(src, "w") as fh:
+        fh.write(source)
+    subprocess.check_call(["g++", "-O3", "-march=native", "-ffp-contract=off", "-fno-fast-math", "-fopenmp", "-fPIC",
+                           "-shared", "-std=c++17", src, "-o", so])
+    return ctypes.CDLL(so)
+
+
 def lib():
-    """The compiled arithmetic: -ffp-contract=off keeps every product and sum separately rounded; std::fmaf is the one
-    fused rounding (checked against fma32 by the tests)."""
+    """The compiled arithmetic of `single` (compile_model)."""
     global _lib
     if _lib is None:
-        d = tempfile.mkdtemp(prefix="xcorr_fp32_model_")
-        src, so = os.path.join(d, "model.cpp"), os.path.join(d, "model.so")
-        with open(src, "w") as fh:
-            fh.write(SRC)
-        subprocess.check_call(["g++", "-O3", "-march=native", "-ffp-contract=off", "-fno-fast-math", "-fopenmp", "-fPIC",
-                               "-shared", "-std=c++17", src, "-o", so])
-        _lib = ctypes.CDLL(so)
+        _lib = compile_model(SRC, "xcorr_fp32_model")
     return _lib
 
 
