@@ -77,7 +77,8 @@ extern "C" {
  *      an accepted L = 8 candidate with the same format, rnti and payload is dropped.  dci[s] holds the L = 8 candidates
  *      first, then L = 4, CCEs ascending: n_dci[s] <= 6.
  *  13. Record.  Per DCI format, agg (L), cce, rnti, n_bits (size), quality (q) and payload = sum a_i 2^(size - 1 - i),
- *      and the fields parsed from it on the host: for 1A (36.212 5.3.3.1.3) localized, the resource block assignment as
+ *      and the fields parsed from it on the host: for 1A (36.212 5.3.3.1.3) localized (the raw localized/distributed
+ *      VRB assignment flag: 1 means distributed), the resource block assignment as
  *      riv and decoded on R to rb_start and n_rb (36.213 7.1.6.3; -1 when riv is not a valid RIV), mcs, harq, ndi, rv and
  *      tpc; for 1C (5.3.3.1.4) gap, riv (raw) and tbs_index.  Fields a format does not have are 0 (rb_start, n_rb -1).
  *      Per subframe cfi, n_ctrl, n_reg, n_cce and n_dci.  Per cell count[] the DCIs with SI-, P- and RA-RNTI,
@@ -93,7 +94,7 @@ typedef struct lcs_pdcch_dci {
   uint32_t n_bits;                             /* payload size */
   uint32_t riv;                                /* resource block assignment field */
   int32_t rb_start, n_rb;                      /* 1A: riv decoded on R; -1 otherwise */
-  uint32_t localized, mcs, harq, ndi, rv, tpc; /* 1A */
+  uint32_t localized, mcs, harq, ndi, rv, tpc; /* 1A; localized is the raw flag: 1 means distributed VRBs */
   uint32_t gap, tbs_index;                     /* 1C */
 } lcs_pdcch_dci;
 

@@ -1,6 +1,7 @@
 // carrier_grid.cuh - the full-bandwidth OFDM grid of found cells, from the wideband recording they were found in: the grid
 // Y[t][c] of include/lcs_carrier.h, built for the CRS symbols only, and the one host path of every module on it:
-// liblcs_carrier.so (carrier.cu), liblcs_cir.so (cir.cu), liblcs_pcfich.so (pcfich.cu) and liblcs_pdcch.so (pdcch.cu).
+// liblcs_carrier.so (carrier.cu), liblcs_cir.so (cir.cu), liblcs_pcfich.so (pcfich.cu), liblcs_pdcch.so (pdcch.cu) and
+// liblcs_sib1.so (sib1.cu).
 // Each module's handle is a GridModule, and its lcs_X_cells is grid_cells with the module's planner, slices and kernels.
 #pragma once
 #include <cmath>

@@ -14,16 +14,6 @@ namespace pdcch {
 namespace {
 const int kPerm[32] = {1, 17, 9, 25, 5, 21, 13, 29, 3, 19, 11, 27, 7, 23, 15, 31,
                        0, 16, 8, 24, 4, 20, 12, 28, 2, 18, 10, 26, 6, 22, 14, 30};   // 36.212 Table 5.1.4-2
-
-int ceil_log2(long long x) {
-  int b = 0;
-  while ((1ll << b) < x) b++;
-  return b;
-}
-
-uint32_t field(uint64_t payload, int n_bits, int first, int width) {
-  return (uint32_t)((payload >> (n_bits - first - width)) & ((1ull << width) - 1));
-}
 }  // namespace
 
 std::string plan_pdcch(const lcs_cell& c, uint64_t n_in, int D, double fs_in, double fc_in, double fs_programmed,
@@ -123,49 +113,6 @@ std::vector<uint8_t> ratematch_positions(int K) {
         if (y >= nd) pos.push_back((uint8_t)(s * K + y - nd));
       }
   return pos;
-}
-
-uint32_t riv_encode(int R, int start, int length) {
-  return length - 1 <= R / 2 ? (uint32_t)(R * (length - 1) + start) : (uint32_t)(R * (R - length + 1) + (R - 1 - start));
-}
-
-bool riv_decode(int R, uint32_t riv, int& start, int& length) {
-  const int a = (int)(riv / R), b = (int)(riv % R);
-  if (a + b < R) {
-    length = a + 1;
-    start = b;
-  } else {
-    length = R - a + 1;
-    start = R - 1 - b;
-  }
-  return a <= R && length >= 1 && start >= 0 && start + length <= R && riv_encode(R, start, length) == riv;
-}
-
-void parse_dci(lcs_pdcch_dci& d, int R) {
-  const uint64_t p = d.payload;
-  const int n = (int)d.n_bits;
-  d.riv = d.localized = d.mcs = d.harq = d.ndi = d.rv = d.tpc = d.gap = d.tbs_index = 0;
-  d.rb_start = d.n_rb = -1;
-  if (d.format == LCS_DCI_1A) {                 // flag, localized, RIV, MCS, HARQ, NDI, RV, TPC (36.212 5.3.3.1.3)
-    const int nra = ceil_log2((long long)R * (R + 1) / 2);
-    d.localized = field(p, n, 1, 1);
-    d.riv = field(p, n, 2, nra);
-    d.mcs = field(p, n, 2 + nra, 5);
-    d.harq = field(p, n, 7 + nra, 3);
-    d.ndi = field(p, n, 10 + nra, 1);
-    d.rv = field(p, n, 11 + nra, 2);
-    d.tpc = field(p, n, 13 + nra, 2);
-    int start, length;
-    if (riv_decode(R, d.riv, start, length)) {
-      d.rb_start = start;
-      d.n_rb = length;
-    }
-  } else if (d.format == LCS_DCI_1C) {          // gap (R >= 50), RIV, TBS index (36.212 5.3.3.1.4)
-    const int g = R >= 50;
-    d.gap = g ? field(p, n, 0, 1) : 0;
-    d.riv = field(p, n, g, n - g - 5);
-    d.tbs_index = field(p, n, n - 5, 5);
-  }
 }
 
 }  // namespace pdcch

@@ -1,5 +1,5 @@
 // pdcch_plan.hpp - host planning of the PDCCH decoder (pdcch.cu, contract in include/lcs_pdcch.h): a cell's windows, its
-// control-region tables, its DCI sizes and scrambling, and the parsing of a decoded DCI, with no device work.
+// control-region tables, its DCI sizes and scrambling, with no device work (a decoded DCI's fields: dci_fields.hpp).
 #pragma once
 #include <cstdint>
 #include <string>
@@ -7,6 +7,7 @@
 
 #include "../../include/lcs_pdcch.h"
 #include "carrier_plan.hpp"
+#include "dci_fields.hpp"
 
 namespace lcs {
 namespace pdcch {
@@ -41,13 +42,6 @@ void scrambling(int n_id, int u, uint32_t* w);
 // 36.212 5.1.4.2: pos[i], i < 3K, the coded bit (row j * K + column k of the [3][K] block) of rate-matched bit i; bit
 // i + 3K m is the same coded bit again.
 std::vector<uint8_t> ratematch_positions(int K);
-
-// Rule 13's fields of d from its format, n_bits and payload.
-void parse_dci(lcs_pdcch_dci& d, int R);
-
-// 36.213 7.1.6.3: the RIV of (start, length) on R RBs, and back (false when riv is not one).
-uint32_t riv_encode(int R, int start, int length);
-bool riv_decode(int R, uint32_t riv, int& start, int& length);
 
 }  // namespace pdcch
 }  // namespace lcs

@@ -83,6 +83,11 @@ static void print_usage() {
   cout << "     --pdcch-csv OUT.csv         with --pdcch: one line per decoded DCI (SI-, P- and RA-RNTI, formats 1A and 1C)," << endl;
   cout << "                                 n_id_cell,fc_hz,subframe,cfi,format,agg,cce,rnti,n_bits,payload_hex,quality," << endl;
   cout << "                                 rb_start,n_rb,mcs,rv (- for a field the format does not have)" << endl;
+  cout << "     --sib1                      with --wideband: add PLMN (the first MCC-MNC), TAC and CID columns, decoded from" << endl;
+  cout << "                                 each cell's SIB1 on the PDSCH of its SIB1 occasions, with the SFN of its MIB;" << endl;
+  cout << "                                 --fs-in as for --measure-carrier.  A cell whose SIB1 did not decode shows - - -" << endl;
+  cout << "     --sib1-csv OUT.csv          with --sib1: one line per SIB1 occasion, n_id_cell,fc_hz,subframe,sfn,format," << endl;
+  cout << "                                 rb_start,n_rb,tbs,rv,crc_ok,iterations,sinr_db,tb_hex (- where nothing was found)" << endl;
   cout << "  -r --record / -i --device-index need a live rtl-sdr dongle: not supported by this build" << endl;
 }
 
@@ -178,8 +183,8 @@ int main(int argc, char* const argv[]) {
   bool save_cap = false, use_recorded_data = false, raw = false, batched = false;
   string data_dir = ".", wideband, format = "ci16";
   double fs_in = -1, fc_in = -1;
-  bool resample = false, measure = false, measure_carrier = false, cir = false, cfi = false, pdcch = false;
-  string spectrum, carrier_csv, cir_csv, cfi_csv, pdcch_csv;
+  bool resample = false, measure = false, measure_carrier = false, cir = false, cfi = false, pdcch = false, sib1 = false;
+  string spectrum, carrier_csv, cir_csv, cfi_csv, pdcch_csv, sib1_csv;
   long nfft = 4096;
   static struct option long_options[] = {
       {"help", no_argument, 0, 'h'},          {"verbose", no_argument, 0, 'v'},       {"brief", no_argument, 0, 'b'},
@@ -193,6 +198,7 @@ int main(int argc, char* const argv[]) {
       {"cir", no_argument, 0, 'X'},             {"cir-csv", required_argument, 0, 'Y'},
       {"cfi", no_argument, 0, 'Q'},             {"cfi-csv", required_argument, 0, 'Z'},
       {"pdcch", no_argument, 0, 'H'},           {"pdcch-csv", required_argument, 0, 'J'},
+      {"sib1", no_argument, 0, 'U'},            {"sib1-csv", required_argument, 0, 'G'},
       {0, 0, 0, 0}};
   for (;;) {
     int idx = 0;
@@ -228,6 +234,8 @@ int main(int argc, char* const argv[]) {
       case 'Z': cfi_csv = optarg; break;
       case 'H': pdcch = true; break;
       case 'J': pdcch_csv = optarg; break;
+      case 'U': sib1 = true; break;
+      case 'G': sib1_csv = optarg; break;
       case 'i': break;
       default: return -1;
     }
@@ -248,6 +256,9 @@ int main(int argc, char* const argv[]) {
   if (!pdcch_csv.empty() && !pdcch) { cerr << "Error: --pdcch-csv needs --pdcch" << endl; return -1; }
   if (pdcch && wideband.empty()) { cerr << "Error: --pdcch needs --wideband" << endl; return -1; }
   if (pdcch && !search) { cerr << "Error: --pdcch needs a search (-s)" << endl; return -1; }
+  if (!sib1_csv.empty() && !sib1) { cerr << "Error: --sib1-csv needs --sib1" << endl; return -1; }
+  if (sib1 && wideband.empty()) { cerr << "Error: --sib1 needs --wideband" << endl; return -1; }
+  if (sib1 && !search) { cerr << "Error: --sib1 needs a search (-s)" << endl; return -1; }
   if (nfft < 64 || nfft > 65536 || (nfft & (nfft - 1))) { cerr << "Error: --nfft must be a power of two in [64, 65536]" << endl; return -1; }
   const bool wide = !wideband.empty();
   int wide_format = LCS_IQ_CI16;   // --format, for the spectrum and the search
@@ -310,10 +321,10 @@ int main(int argc, char* const argv[]) {
     } else {
       down = (uint32_t)std::lround(fs_in / 1.92e6);
     }
-    if (measure_carrier || cir || cfi || pdcch) {
+    if (measure_carrier || cir || cfi || pdcch || sib1) {
       const long D = std::lround(fs_in / 1.92e6);
       if (!((D == 2 || D == 4 || D == 8 || D == 16 || D == 32) && std::fabs(fs_in - D * 1.92e6) <= 1e-6)) {
-        cerr << "Error: " << (measure_carrier ? "--measure-carrier" : (cir ? "--cir" : (cfi ? "--cfi" : "--pdcch")))
+        cerr << "Error: " << (measure_carrier ? "--measure-carrier" : (cir ? "--cir" : (cfi ? "--cfi" : (pdcch ? "--pdcch" : "--sib1"))))
              << " needs --fs-in = D * 1.92 MHz with D in {2, 4, 8, 16, 32}" << endl;
         return -1;
       }
@@ -350,6 +361,8 @@ int main(int argc, char* const argv[]) {
   if (!cfi_csv.empty() && !(cfi_file = open_output(cfi_csv))) return -1;
   FILE* pdcch_file = nullptr;
   if (!pdcch_csv.empty() && !(pdcch_file = open_output(pdcch_csv))) return -1;
+  FILE* sib1_file = nullptr;
+  if (!sib1_csv.empty() && !(sib1_file = open_output(sib1_csv))) return -1;
   if (verbosity >= 1) {
     cout << "LTE CellSearch (GPU drop-in, " << lcs_version() << ") beginning" << endl;
     if (freq_start == freq_end) cout << "  Search frequency: " << freq_start / 1e6 << " MHz" << endl;
@@ -557,6 +570,39 @@ int main(int argc, char* const argv[]) {
         if (!ok) throw("cannot write the PDCCH CSV file");
       }
     }
+    vector<lcs_sib1_meas> smeas;    // --sib1: that of the k-th final cell, if sok[k]
+    vector<bool> sok;
+    if (sib1) {
+      measure_sib1(wide_iq.data(), wide_format, wide_n, fs_in, fc_in, vector<Cell>(cells_final.begin(), cells_final.end()),
+                   fs_programmed, smeas, sok);
+      if (sib1_file) {
+        bool ok = std::fprintf(sib1_file, "n_id_cell,fc_hz,subframe,sfn,format,rb_start,n_rb,tbs,rv,crc_ok,iterations,"
+                                          "sinr_db,tb_hex\n") > 0;
+        size_t k = 0;
+        for (list<Cell>::iterator it = cells_final.begin(); it != cells_final.end(); ++it, ++k)
+          for (int o = 0; sok[k] && o < LCS_SIB1_OCCASIONS; o++) {
+            const lcs_sib1_occasion& x = smeas[k].occ[o];
+            string rest = "-,-,-,-,-,-,-,-,-";
+            if (x.found && x.n_re) {
+              string hex;
+              char b[3];
+              for (uint32_t i = 0; i < x.tbs / 8; i++) {
+                std::snprintf(b, sizeof(b), "%02x", x.tb[i]);
+                hex += b;
+              }
+              rest = string(x.format == LCS_DCI_1A ? "1A" : "1C") + "," + std::to_string(x.vrb_start) + "," +
+                     std::to_string(x.n_vrb) + "," + std::to_string(x.tbs) + "," + std::to_string(x.rv) + "," +
+                     std::to_string(x.crc_ok) + "," + std::to_string(x.iterations) + "," + csv_db(x.sinr) + "," + hex;
+            } else if (x.found) {
+              rest = string(x.format == LCS_DCI_1A ? "1A" : "1C") + ",-,-,-,-,-,-,-,-";
+            }
+            ok = ok && std::fprintf(sib1_file, "%d,%.17g,%u,%u,%s\n", (int)(*it).n_id_cell(), (*it).fc_requested, x.subframe,
+                                    x.sfn, rest.c_str()) > 0;
+          }
+        ok = std::fclose(sib1_file) == 0 && ok;
+        if (!ok) throw("cannot write the SIB1 CSV file");
+      }
+    }
     if (cells_final.size() == 0) {
       cout << "No LTE cells were found..." << endl;
     } else {   // CellSearch.cpp:579-613
@@ -564,7 +610,7 @@ int main(int argc, char* const argv[]) {
       cout << "A: #antenna ports C: CP type ; P: PHICH duration ; PR: PHICH resource type" << endl;
       cout << "CID A      fc   foff RXPWR C nRB P  PR CrystalCorrectionFactor" << (spec ? " CarrierPower[dBFS]" : "")
            << (measure ? " RSRP[dBFS] RSRQ[dB] SINR[dB]" : "") << (measure_carrier ? " RSRPc[dBFS] RSRQc[dB] SINRc[dB]" : "")
-           << (cir ? " TOA[us] DS[ns]" : "") << (cfi ? " CFI" : "") << (pdcch ? " SI" : "") << endl;
+           << (cir ? " TOA[us] DS[ns]" : "") << (cfi ? " CFI" : "") << (pdcch ? " SI" : "") << (sib1 ? " PLMN TAC CID" : "") << endl;
       size_t k = 0;
       for (list<Cell>::iterator it = cells_final.begin(); it != cells_final.end(); ++it, ++k) {
         stringstream ss;
@@ -618,6 +664,16 @@ int main(int argc, char* const argv[]) {
             ss << " " << pmeas[k].count[0];
           else
             ss << " -";
+        }
+        if (sib1) {
+          const lcs_sib1_meas& m = smeas[k];
+          if (sok[k] && m.parse_ok) {
+            char plmn[32];
+            std::snprintf(plmn, sizeof(plmn), "%03u-%0*u", m.plmn[0].mcc, (int)m.plmn[0].mnc_digits, m.plmn[0].mnc);
+            ss << " " << plmn << " " << m.tac << " " << m.cell_identity;
+          } else {
+            ss << " - - -";
+          }
         }
         cout << ss.str() << endl;
       }

@@ -100,7 +100,8 @@ void measure_cells(const void* iq, int iq_format, uint32_t n_cap, const std::vec
   check(measure_lists(iq, iq_format, 0, n_cap, detected_cells, fs_programmed, meas, &where), where);
 }
 
-// One measurement of the wideband recording (lcs_carrier_cells, lcs_cir_cells, lcs_pcfich_cells or lcs_pdcch_cells, through
+// One measurement of the wideband recording (lcs_carrier_cells, lcs_cir_cells, lcs_pcfich_cells, lcs_pdcch_cells or
+// lcs_sib1_cells, through
 // handle type H) of every cell of `cells`: all in one call, and when a cell is rejected each on its own, so that only the rejected ones go
 // unmeasured.
 template <class H, class M, class Create, class Cells, class Destroy>
@@ -150,6 +151,12 @@ void measure_pdcch(const void* iq, int iq_format, uint64_t n, double fs_in, doub
                    const double& fs_programmed, std::vector<lcs_pdcch_meas>& meas, std::vector<bool>& ok) {
   measure_recording<lcs_pdcch>(lcs_pdcch_create, lcs_pdcch_cells, lcs_pdcch_destroy, "lcs_pdcch", iq, iq_format, n, fs_in,
                                fc_in, cells, fs_programmed, meas, ok);
+}
+
+void measure_sib1(const void* iq, int iq_format, uint64_t n, double fs_in, double fc_in, const std::vector<Cell>& cells,
+                  const double& fs_programmed, std::vector<lcs_sib1_meas>& meas, std::vector<bool>& ok) {
+  measure_recording<lcs_sib1>(lcs_sib1_create, lcs_sib1_cells, lcs_sib1_destroy, "lcs_sib1", iq, iq_format, n, fs_in, fc_in,
+                              cells, fs_programmed, meas, ok);
 }
 
 void sweep_search_cu8(const std::vector<unsigned char>& iq, uint32_t n_cap, const std::vector<double>& fc_requested,

@@ -25,6 +25,7 @@
 #include "../../include/lcs_cir.h"
 #include "../../include/lcs_pcfich.h"
 #include "../../include/lcs_pdcch.h"
+#include "../../include/lcs_sib1.h"
 
 // --- include/common.h.in ---
 typedef char int8;
@@ -136,6 +137,10 @@ void measure_pcfich(const void* iq, int iq_format, uint64_t n, double fs_in, dou
 // `cells`, as measure_carriers: meas[i] is that of cells[i], and ok[i] is false for a cell lcs_pdcch_cells rejects.
 void measure_pdcch(const void* iq, int iq_format, uint64_t n, double fs_in, double fc_in, const std::vector<Cell>& cells,
                    const double& fs_programmed, std::vector<lcs_pdcch_meas>& meas, std::vector<bool>& ok);
+// SIB1 (lcs_sib1 of liblcs_sib1.so, DESIGN.md section 4.14) of every cell of `cells`, each with the SFN its MIB decode
+// gave, as measure_carriers: meas[i] is that of cells[i], and ok[i] is false for a cell lcs_sib1_cells rejects.
+void measure_sib1(const void* iq, int iq_format, uint64_t n, double fs_in, double fc_in, const std::vector<Cell>& cells,
+                  const double& fs_programmed, std::vector<lcs_sib1_meas>& meas, std::vector<bool>& ok);
 // Welch power spectral density (lcs_psd of liblcs_psd.so, DESIGN.md section 4.8) of the whole recording in `path` ([n][2] in iq_format,
 // sample_bytes per sample, at fs_in, read in blocks): psd [nfft] in fftshift order, full-scale^2 per Hz, over n_segments segments.
 void wideband_psd(const std::string& path, int iq_format, size_t sample_bytes, double fs_in, uint32_t nfft,

@@ -2,8 +2,9 @@
 it: liblcs_psd.so, the Welch spectrum of include/lcs_psd.h, liblcs_meas.so, the per-cell RSRP / RSRQ / SINR of
 include/lcs_meas.h, liblcs_carrier.so, the same over each cell's whole carrier, of include/lcs_carrier.h,
 liblcs_cir.so, the power delay profile of each cell over its whole carrier, of include/lcs_cir.h, liblcs_pcfich.so,
-the control format indicator of each cell in every subframe, of include/lcs_pcfich.h, and liblcs_pdcch.so, the
-common-search-space DCIs of each cell in every subframe, of include/lcs_pdcch.h.
+the control format indicator of each cell in every subframe, of include/lcs_pcfich.h, liblcs_pdcch.so, the
+common-search-space DCIs of each cell in every subframe, of include/lcs_pdcch.h, and liblcs_sib1.so, the SIB1 of each
+cell, of include/lcs_sib1.h.
 
 This module is plumbing for tests/, bench.py and __graft_entry__.py: every call goes through the
 same `extern "C"` entry points a C++/IT++ host would bind (INTEGRATION.md).  lib() gives every
@@ -33,6 +34,8 @@ PCFICH_LIB_PATH = os.environ.get("LCS_PCFICH_LIB") or os.path.join(HERE, "liblcs
 PCFICH_HEADER = os.path.join(HERE, "..", "include", "lcs_pcfich.h")
 PDCCH_LIB_PATH = os.environ.get("LCS_PDCCH_LIB") or os.path.join(HERE, "liblcs_pdcch.so")
 PDCCH_HEADER = os.path.join(HERE, "..", "include", "lcs_pdcch.h")
+SIB1_LIB_PATH = os.environ.get("LCS_SIB1_LIB") or os.path.join(HERE, "liblcs_sib1.so")
+SIB1_HEADER = os.path.join(HERE, "..", "include", "lcs_sib1.h")
 
 IQ_CF32, IQ_CU8, IQ_C128, IQ_CI16, IQ_CS8 = 0, 1, 2, 3, 4
 KERNEL_AUTO, KERNEL_FP32, KERNEL_TC = 0, 1, 2
@@ -142,8 +145,8 @@ def meas_lib():
 
 
 def _grid_lib(path, header):
-    """A module on the whole-carrier grid (include/lcs_carrier.h, lcs_cir.h, lcs_pcfich.h or lcs_pdcch.h); it takes the
-    contexts of lib()."""
+    """A module on the whole-carrier grid (include/lcs_carrier.h, lcs_cir.h, lcs_pcfich.h, lcs_pdcch.h or lcs_sib1.h); it
+    takes the contexts of lib()."""
     lib()
     return _bind(path, header)
 
@@ -162,6 +165,10 @@ def pcfich_lib():
 
 def pdcch_lib():
     return _grid_lib(PDCCH_LIB_PATH, PDCCH_HEADER)
+
+
+def sib1_lib():
+    return _grid_lib(SIB1_LIB_PATH, SIB1_HEADER)
 
 
 def _p(a):
@@ -852,7 +859,7 @@ class CellMeasure(_Handle):
 
 class _GridModule(_Handle):
     """A module on the whole-carrier grid: `_lib` is its library, `_prefix` the prefix of its C functions (lcs_carrier,
-    lcs_cir, lcs_pcfich or lcs_pdcch) and `_dtype` its record."""
+    lcs_cir, lcs_pcfich, lcs_pdcch or lcs_sib1) and `_dtype` its record."""
     _prefix = _dtype = None
 
     def __init__(self, ctx):
@@ -970,3 +977,35 @@ class ControlChannel(_GridModule):
     _lib = staticmethod(pdcch_lib)
     _prefix = "lcs_pdcch"
     _dtype = PDCCH_MEAS
+
+
+# lcs_sib1_occasion and lcs_sib1_meas as numpy records
+SIB1_OCCASIONS = 3                    # LCS_SIB1_OCCASIONS
+SIB1_TB_BYTES = 280                   # LCS_SIB1_TB_BYTES
+SIB1_OCC = np.dtype([("sinr", np.float64), ("dci", PDCCH_DCI), ("subframe", np.uint32), ("sfn", np.uint32),
+                     ("found", np.uint32), ("cfi", np.uint32), ("n_ctrl", np.uint32), ("format", np.uint32),
+                     ("distributed", np.uint32), ("gap", np.uint32), ("vrb_start", np.int32), ("n_vrb", np.int32),
+                     ("n_prb", np.uint32), ("prb", np.uint8, (2, 100)), ("tbs", np.uint32), ("K", np.uint32), ("F", np.uint32),
+                     ("rv", np.uint32), ("n_re", np.uint32), ("crc_ok", np.uint32), ("iterations", np.uint32),
+                     ("tb", np.uint8, SIB1_TB_BYTES)], align=True)
+SIB1_PLMN = np.dtype([("mcc", np.uint32), ("mnc", np.uint32), ("mnc_digits", np.uint32), ("reserved", np.uint32)], align=True)
+SIB1_MEAS = np.dtype([("occ", SIB1_OCC, SIB1_OCCASIONS), ("n_found", np.uint32), ("n_crc_ok", np.uint32),
+                      ("consistent", np.uint32), ("parse_ok", np.uint32), ("n_plmn", np.uint32), ("plmn", SIB1_PLMN, 6),
+                      ("tac", np.uint32), ("cell_identity", np.uint32), ("cell_barred", np.uint32),
+                      ("intra_freq_reselection", np.uint32), ("csg_indication", np.uint32),
+                      ("csg_identity_present", np.uint32), ("csg_identity", np.uint32), ("q_rx_lev_min", np.int32),
+                      ("q_rx_lev_min_offset", np.uint32), ("p_max_present", np.uint32), ("p_max", np.int32),
+                      ("freq_band_indicator", np.uint32), ("n_si", np.uint32), ("si_periodicity", np.uint32, 32),
+                      ("si_sib_mask", np.uint32, 32), ("tdd_present", np.uint32), ("tdd_subframe_assignment", np.uint32),
+                      ("tdd_special_subframe_patterns", np.uint32), ("si_window_ms", np.uint32),
+                      ("system_info_value_tag", np.uint32), ("non_critical_extension", np.uint32)], align=True)
+SIB1_CHUNK = 32                       # LCS_SIB1_CHUNK: cells per chunk, five launches each
+
+
+class SystemInfo(_GridModule):
+    """lcs_sib1: SystemInformationBlockType1 of found cells (their PLMNs, tracking area code and cell identity), decoded
+    from the PDSCH their SI-RNTI DCIs schedule in the three SIB1 occasions of the wideband recording they were found in
+    (DESIGN.md section 4.14).  Each cell's `sfn` must be that of its grid frame 0, as lcs_decode_mib reports it."""
+    _lib = staticmethod(sib1_lib)
+    _prefix = "lcs_sib1"
+    _dtype = SIB1_MEAS

@@ -1,11 +1,12 @@
-"""Bit-exact fingerprint of the four modules on the whole-carrier grid (lcs_carrier_cells, lcs_cir_cells, lcs_pcfich_cells
-and lcs_pdcch_cells): per module one SHA-256 over the record bytes of every call, with the kernels the calls launched and
-the count its timing_read reports, then the status and message of one rejected call.
+"""Bit-exact fingerprint of the five modules on the whole-carrier grid (lcs_carrier_cells, lcs_cir_cells, lcs_pcfich_cells,
+lcs_pdcch_cells and lcs_sib1_cells): per module one SHA-256 over the record bytes of every call, with the kernels the
+calls launched and the count its timing_read reports, then the status and message of one rejected call.
 
 The GPU tests compare against float64 restatements within an FP32 tolerance, so they cannot show that a change left every
 byte alone; two builds that print the same lines here computed the same thing.  The calls run on seeded lte_dl_synth
 recordings: every IQ format and every D from 2 to 32, host and device input, 1, 2 and 4 ports in both CPs, cells sending
-a CFI schedule and planted common-search-space DCIs, single-cell calls, and one 40-cell call of two chunks.
+a CFI schedule and planted common-search-space DCIs, single-cell calls, and one 40-cell call of two chunks.  lcs_sib1_cells
+runs the same calls with an SFN given to each cell, then the planted-SIB1 recordings of tests/test_sib1_gpu.py.
 
 Usage: python tools/grid_digest.py        (needs an H100; a minute or so)
 """
@@ -73,27 +74,53 @@ def calls():
     return out
 
 
+def sib1_calls(todo):
+    """The calls of calls() with an SFN for each cell, then one call per planted-SIB1 case of test_sib1_gpu."""
+    import torch
+    from test_sib1_gpu import CASES, case_cell
+    out = []
+    for iq, fmt, D, cells in todo:
+        cs = []
+        for k, c in enumerate(cells):
+            x = L.Cell()
+            C.memmove(C.byref(x), C.byref(c), C.sizeof(L.Cell))
+            x.sfn = (37 * k + D) % 1024
+            cs.append(x)
+        out.append((iq, fmt, D, cs))
+    for k, case in enumerate(CASES):
+        D, fmt, dev, off = case[0], case[1], case[2], case[6]
+        c, d = case_cell(case)
+        iq = recording([(FC_IN + off, [c])], n_samples(D), D, fmt, seed=100 + k)
+        out.append((torch.from_numpy(iq).cuda() if dev else iq, fmt, D, [L.new_cell(**d)]))
+    return out
+
+
+def digest(ctx, name, cls, todo):
+    m = cls(ctx)
+    h = hashlib.sha256()
+    n0 = ctx.launches
+    for iq, fmt, D, cells in todo:
+        h.update(m.measure(iq, fmt, D * FS, FC_IN, cells, FS).tobytes())
+    launches = ctx.launches - n0
+    print("%-8s %s  launches %d  timed %d" % (name, h.hexdigest(), launches, m.timing_read()[1]), flush=True)
+    iq, fmt, D, cells = todo[2]
+    bad = L.Cell()
+    C.memmove(C.byref(bad), C.byref(cells[0]), C.sizeof(L.Cell))
+    bad.n_ports = 3
+    try:
+        m.measure(iq, fmt, D * FS, FC_IN, [cells[0], bad], FS)
+        print("%-8s rejected: nothing" % name, flush=True)
+    except L.LcsError as e:
+        print("%-8s rejected: %s" % (name, e), flush=True)
+    m.close()
+
+
 def main():
     todo = calls()
     ctx = L.Context(0)
     for name, cls in MODULES:
-        m = cls(ctx)
-        h = hashlib.sha256()
-        n0 = ctx.launches
-        for iq, fmt, D, cells in todo:
-            h.update(m.measure(iq, fmt, D * FS, FC_IN, cells, FS).tobytes())
-        launches = ctx.launches - n0
-        print("%-8s %s  launches %d  timed %d" % (name, h.hexdigest(), launches, m.timing_read()[1]), flush=True)
-        iq, fmt, D, cells = todo[2]
-        bad = L.Cell()
-        C.memmove(C.byref(bad), C.byref(cells[0]), C.sizeof(L.Cell))
-        bad.n_ports = 3
-        try:
-            m.measure(iq, fmt, D * FS, FC_IN, [cells[0], bad], FS)
-            print("%-8s rejected: nothing" % name, flush=True)
-        except L.LcsError as e:
-            print("%-8s rejected: %s" % (name, e), flush=True)
-        m.close()
+        digest(ctx, name, cls, todo)
+    digest(ctx, "sib1", L.SystemInfo, sib1_calls(todo))
     ctx.close()
 
 

@@ -29,10 +29,16 @@ With --pdcch it times the common-search-space DCI decoder (lcs_pdcch_cells, DESI
 recording and cells in the same way (PHICH duration normal, N_g = 1): one JSON line with the device time per cell
 (lcs_pdcch_timing_read), the launches and the card, read in the same run.
 
+With --sib1 it times the SIB1 decoder (lcs_sib1_cells, DESIGN.md section 4.14) on the same recording and cells in the
+same way, each cell also sending a 1A-scheduled SIB1 of 328 bits on 6 PRBs in its SIB1 occasions (lte_dl_synth's "sib1"
+key): one JSON line with the device time per cell (lcs_sib1_timing_read), the occasions decoded and passing CRC, the
+launches and the card, and a split of the device time per cell by kernel from torch.profiler in a separate call.
+
 Usage: python tools/meas_bench.py [--channels 64] [--reps 20]
        python tools/meas_bench.py --carrier [--copies 8] [--reps 20]
        python tools/meas_bench.py --cir [--copies 8] [--reps 20]
        python tools/meas_bench.py --pcfich [--copies 8] [--reps 20]
+       python tools/meas_bench.py --sib1 [--copies 8] [--reps 20]
        python tools/meas_bench.py --pdcch [--copies 8] [--reps 20]
 """
 import argparse
@@ -104,20 +110,24 @@ def carrier_main(a):
         for i in range(8):
             c = cell(3 * (8 * j + i) + i % 3, (1, 2, 4)[i % 3], 1 + (i % 4 == 3), 1000 + 517 * i)
             c["n_rb_dl"] = 50
+            if a.sib1:
+                c.update(cfi=(3,), sib1=dict(format="1A", L=8, cce=0, riv=50 * 5 + 6 * i, mcs=10, tpc=0,
+                                             tb=bytes((17 * i + b) % 256 for b in range(41))))
             cs.append(c)
         carriers.append((FC + off, cs))
         for c in cs:
             cells.append(L.new_cell(fc_requested=FC + off, fc_programmed=FC + off, n_id_1=c["n_id_cell"] // 3,
                                     n_id_2=c["n_id_cell"] % 3, cp_type=c["cp_type"], n_ports=c["n_ports"],
                                     frame_start=float(c["t0"]), freq_superfine=0.0, n_rb_dl=50, phich_duration=1,
-                                    phich_resource=3))
+                                    phich_resource=2 if a.sib1 else 3, sfn=c["sfn0"]))
     x, _ = S.synth_wide_full(D * (5000 + 122 * 960 + 400), fs_in, FC, carriers, 30.0, 0)
     iq = S.quantise(x, "ci16", 0.1 / np.sqrt(np.mean(np.abs(x) ** 2)))
     cells = cells * a.copies
     ctx = L.Context(0)
     d_iq = torch.from_numpy(iq).cuda()
-    name = "pdcch" if a.pdcch else "pcfich" if a.pcfich else "cir" if a.cir else "carrier"
-    m = {"carrier": L.CarrierMeasure, "cir": L.CellImpulse, "pcfich": L.ControlFormat, "pdcch": L.ControlChannel}[name](ctx)
+    name = "sib1" if a.sib1 else "pdcch" if a.pdcch else "pcfich" if a.pcfich else "cir" if a.cir else "carrier"
+    m = {"carrier": L.CarrierMeasure, "cir": L.CellImpulse, "pcfich": L.ControlFormat, "pdcch": L.ControlChannel,
+         "sib1": L.SystemInfo}[name](ctx)
     m.measure(d_iq, "ci16", fs_in, FC, cells, 1.92e6)              # warm-up
     m.timing_read()
     wall = []
@@ -126,8 +136,12 @@ def carrier_main(a):
         m.measure(d_iq, "ci16", fs_in, FC, cells, 1.92e6)
         wall.append(time.perf_counter() - t)
     ms, launches = m.timing_read()
-    m.close()
     n = len(cells)
+    split = None
+    if name == "sib1":
+        out = m.measure(d_iq, "ci16", fs_in, FC, cells, 1.92e6)
+        split = kernel_split(lambda: m.measure(d_iq, "ci16", fs_in, FC, cells, 1.92e6), n)
+    m.close()
     dev_s = ms / 1e3 / a.reps
     rec = {name: True, "fs_in": fs_in, "cells": n, "reps": a.reps, "launches": launches,
            name + "_device_us_per_cell": 1e6 * dev_s / n, name + "_host_us_per_cell": 1e6 * float(np.median(wall)) / n}
@@ -138,9 +152,30 @@ def carrier_main(a):
     if name == "cir":
         macs = sum(cir_macs(c) for c in cells)
         rec.update(cir_cmacs_per_cell=macs / n, cir_fp64_tflops=8 * macs / dev_s / 1e12)
+    if split is not None:
+        rec.update(sib1_occasions_found=int(out["n_found"].sum()), sib1_occasions_crc_ok=int(out["n_crc_ok"].sum()),
+                   sib1_occasions=3 * n, kernel_us_per_cell=split)
     rec["gpu"] = gpu_name()
     print(json.dumps(rec), flush=True)
     ctx.close()
+
+
+def kernel_split(call, n):
+    """Device time per cell of each kernel of one call(), from torch.profiler with CUDA activities (a run of its own)."""
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        call()
+        torch.cuda.synchronize()
+    split = {}
+    for ev in prof.key_averages():
+        us = getattr(ev, "device_time_total", None)
+        if us is None:
+            us = ev.cuda_time_total
+        for k in ("carrier_grid_kernel", "pcfich_kernel", "pdcch_kernel", "pdsch_kernel", "turbo_kernel"):
+            if k in ev.key and us > 0:
+                split[k] = split.get(k, 0.0) + us / n
+    return split
 
 
 def main():
@@ -151,10 +186,11 @@ def main():
     ap.add_argument("--cir", action="store_true", help="time lcs_cir_cells instead")
     ap.add_argument("--pcfich", action="store_true", help="time lcs_pcfich_cells instead")
     ap.add_argument("--pdcch", action="store_true", help="time lcs_pdcch_cells instead")
-    ap.add_argument("--copies", type=int, default=8, help="with --carrier, --cir, --pcfich or --pdcch: how often each of "
+    ap.add_argument("--sib1", action="store_true", help="time lcs_sib1_cells instead")
+    ap.add_argument("--copies", type=int, default=8, help="with --carrier, --cir, --pcfich, --pdcch or --sib1: how often each of "
                     "the 24 cells is measured per call")
     a = ap.parse_args()
-    if a.carrier or a.cir or a.pcfich or a.pdcch:
+    if a.carrier or a.cir or a.pcfich or a.pdcch or a.sib1:
         return carrier_main(a)
     import torch
     bufs = [S.synth_cu8(153600, cs, fc=FC, snr_db=12.0, seed=i) for i, cs in enumerate(BUFFERS)]

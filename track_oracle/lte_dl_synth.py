@@ -274,7 +274,8 @@ def _grid_full(cell, n_frames, rng):
     """Transmitted grid of all n_rb_dl RBs per port, [n_ports][n_sym][12 R]: the 6-RB content of _grid in the centre,
     full-band CRS, and QPSK times sqrt(cell["load"]) (default 1) on port 0 on every other RE outside the centre.  With
     cell["cfi"], a sequence of CFIs, subframe u (counted from the grid's first) carries the PCFICH of cfi[u mod len] in
-    its symbol 0, written last; with cell["pdcch"] as well, its control region carries those DCIs (_write_control)."""
+    its symbol 0, written last; with cell["pdcch"] as well, its control region carries those DCIs (_write_control); with
+    cell["sib1"] as well, its SIB1 occasions carry that SIB1 (_write_sib1)."""
     R, P, cp = cell["n_rb_dl"], cell["n_ports"], cell["cp_type"]
     X6, n_symb = _grid(cell, n_frames, cell.get("sfn0", 0), rng)
     n_sym = X6.shape[1]
@@ -293,8 +294,12 @@ def _grid_full(cell, n_frames, rng):
             X[:, g, idx] = 0
             X[p, g, idx] = rs[slot, sym]
     X[:, :, 6 * R - 36:6 * R + 36] = X6
+    if "sib1" in cell:
+        cell = dict(cell, pdcch=list(cell.get("pdcch", [])) + sib1_dcis(cell, n_sym // (2 * n_symb)))
     if "pdcch" in cell:
         _write_control(X, cell, n_symb)
+    if "sib1" in cell:
+        _write_sib1(X, cell, n_symb)
     if "cfi" in cell:
         cols, seq = pcfich_res(cell["n_id_cell"], R), list(cell["cfi"])
         for u in range(n_sym // (2 * n_symb)):
@@ -547,3 +552,256 @@ def synth_wide_offset(n, fs_in, fc_in, fc_c, cell, clock_ratio, f_res, snr_db=30
     sigma2 = D * AMP ** 2 / 10 ** (snr_db / 10)
     x += np.sqrt(sigma2 / 2) * (rng.standard_normal(n) + 1j * rng.standard_normal(n))
     return x, Y
+
+
+# ---- SIB1 on the PDSCH (36.211 6.2.3, 6.3, 36.212 5.1.1-5.1.4, 36.213 7.1.6-7.1.7, 36.331 5.2.1.2) --------------------------
+_TURBO_PERM = [0, 16, 8, 24, 4, 20, 12, 28, 2, 18, 10, 26, 6, 22, 14, 30, 1, 17, 9, 25, 5, 21, 13, 29, 3, 19, 11, 27, 7, 23,
+               15, 31]                                                          # 36.212 Table 5.1.4-1
+
+
+def turbo_sizes():
+    """The 188 code block sizes K of 36.212 Table 5.1.3-3."""
+    return ([40 + 8 * i for i in range(60)] + [512 + 16 * i for i in range(1, 33)] + [1024 + 32 * i for i in range(1, 33)]
+            + [2048 + 64 * i for i in range(1, 65)])
+
+
+_QPP = [
+    (3, 10), (7, 12), (19, 42), (7, 16), (7, 18), (11, 20), (5, 22), (11, 24), (7, 26), (41, 84), (103, 90),
+    (15, 32), (9, 34), (17, 108), (9, 38), (21, 120), (101, 84), (21, 44), (57, 46), (23, 48), (13, 50), (27, 52),
+    (11, 36), (27, 56), (85, 58), (29, 60), (33, 62), (15, 32), (17, 198), (33, 68), (103, 210), (19, 36),
+    (19, 74), (37, 76), (19, 78), (21, 120), (21, 82), (115, 84), (193, 86), (21, 44), (133, 90), (81, 46),
+    (45, 94), (23, 48), (243, 98), (151, 40), (155, 102), (25, 52), (51, 106), (47, 72), (91, 110), (29, 168),
+    (29, 114), (247, 58), (29, 118), (89, 180), (91, 122), (157, 62), (55, 84), (31, 64), (17, 66), (35, 68),
+    (227, 420), (65, 96), (19, 74), (37, 76), (41, 234), (39, 80), (185, 82), (43, 252), (21, 86), (155, 44),
+    (79, 120), (139, 92), (23, 94), (217, 48), (25, 98), (17, 80), (127, 102), (25, 52), (239, 106), (17, 48),
+    (137, 110), (215, 112), (29, 114), (15, 58), (147, 118), (29, 60), (59, 122), (65, 124), (55, 84), (31, 64),
+    (17, 66), (171, 204), (67, 140), (35, 72), (19, 74), (39, 76), (19, 78), (199, 240), (21, 82), (211, 252),
+    (21, 86), (43, 88), (149, 60), (45, 92), (49, 846), (71, 48), (13, 28), (17, 80), (25, 102), (183, 104),
+    (55, 954), (127, 96), (27, 110), (29, 112), (29, 114), (57, 116), (45, 354), (31, 120), (59, 610), (185, 124),
+    (113, 420), (31, 64), (17, 66), (171, 136), (209, 420), (253, 216), (367, 444), (265, 456), (181, 468),
+    (39, 80), (27, 164), (127, 504), (143, 172), (43, 88), (29, 300), (45, 92), (157, 188), (47, 96), (13, 28),
+    (111, 240), (443, 204), (51, 104), (51, 212), (451, 192), (257, 220), (57, 336), (313, 228), (271, 232),
+    (179, 236), (331, 120), (363, 244), (375, 248), (127, 168), (31, 64), (33, 130), (43, 264), (33, 134),
+    (477, 408), (35, 138), (233, 280), (357, 142), (337, 480), (37, 146), (71, 444), (71, 120), (37, 152),
+    (39, 462), (127, 234), (39, 158), (39, 80), (31, 96), (113, 902), (41, 166), (251, 336), (43, 170), (21, 86),
+    (43, 174), (45, 176), (45, 178), (161, 120), (89, 182), (323, 184), (47, 186), (23, 94), (47, 190), (263, 480)]  # 36.212 Table 5.1.3-3, (f1, f2) of each K
+
+
+def qpp_table():
+    """(f1, f2) of each K of turbo_sizes()."""
+    return np.array(_QPP)
+
+
+def crc24a(bits):
+    """The 24 parity bits of 36.212 5.1.1 (g_CRC24A = 0x864CFB) of a bit sequence."""
+    r = 0
+    for b in bits:
+        fb = ((r >> 23) & 1) ^ int(b)
+        r = (r << 1) & 0xFFFFFF
+        if fb:
+            r ^= 0x864CFB
+    return np.array([(r >> (23 - i)) & 1 for i in range(24)], np.uint8)
+
+
+def _rsc(c):
+    """One constituent encoder (36.212 5.1.3.2.1): parity of c, then the 3 termination steps' (x, z)."""
+    s1 = s2 = s3 = 0
+    z = np.zeros(c.size, np.uint8)
+    for k, u in enumerate(c):
+        a = int(u) ^ s2 ^ s3
+        z[k] = a ^ s1 ^ s3
+        s1, s2, s3 = a, s1, s2
+    tail = []
+    for _ in range(3):
+        tail.append((s2 ^ s3, s1 ^ s3))
+        s1, s2, s3 = 0, s1, s2
+    return z, tail
+
+
+def turbo_encode(c):
+    """d [3][K + 4] of code block c (filler bits as 0), 36.212 5.1.3.2."""
+    K = c.size
+    f1, f2 = qpp_table()[turbo_sizes().index(K)]
+    pi = (f1 * np.arange(K) + f2 * np.arange(K) ** 2) % K
+    z1, t1 = _rsc(c)
+    z2, t2 = _rsc(c[pi])
+    d = np.zeros((3, K + 4), np.uint8)
+    d[0, :K], d[1, :K], d[2, :K] = c, z1, z2
+    (x0, zz0), (x1, zz1), (x2, zz2) = t1
+    (y0, w0), (y1, w1), (y2, w2) = t2
+    d[:, K:] = [[x0, zz1, y0, w1], [zz0, x2, w0, y2], [x1, zz2, y1, w2]]
+    return d
+
+
+def circular_buffer(K, F):
+    """36.212 5.1.4.1.1-2: for each position of w, (stream, index) of d, or None for a NULL (dummy or filler)."""
+    D = K + 4
+    rows = -(-D // 32)
+    kp, nd = 32 * rows, 32 * rows - D
+    y = [None] * nd + list(range(D))
+    v = [[], [], []]
+    for k in range(kp):
+        j = _TURBO_PERM[k // rows] + 32 * (k % rows)
+        for s in (0, 1):
+            v[s].append(None if y[j] is None or y[j] < F else (s, y[j]))
+        j2 = (j + 1) % kp
+        v[2].append(None if y[j2] is None else (2, y[j2]))
+    # column-by-column read of each stream: v_s[k] for k = column-major index
+    w = v[0] + [x for pair in zip(v[1], v[2]) for x in pair]
+    return w
+
+
+def k0_position(K, rv):
+    rows = -(-(K + 4) // 32)
+    return rows * (2 * -(-(96 * rows) // (8 * rows)) * rv + 2)
+
+
+def rate_match(d, K, F, rv, E):
+    """e [E] of d for redundancy version rv (N_cb = K_w), NULLs skipped."""
+    w = circular_buffer(K, F)
+    k0, out, j = k0_position(K, rv), [], 0
+    while len(out) < E:
+        x = w[(k0 + j) % len(w)]
+        if x is not None:
+            out.append(d[x[0], x[1]])
+        j += 1
+    return np.array(out, np.uint8)
+
+
+TBS_1A = [(32, 56), (56, 88), (72, 144), (104, 176), (120, 208), (144, 224), (176, 256), (224, 328), (256, 392),
+          (296, 456), (328, 504), (376, 584), (440, 680), (488, 744), (552, 840), (600, 904), (632, 968), (696, 1064),
+          (776, 1160), (840, 1288), (904, 1384), (1000, 1480), (1064, 1608), (1128, 1736), (1192, 1800), (1256, 1864),
+          (1480, 2216)]                                                       # 36.213 Table 7.1.7.2.1-1, N_PRB 2 and 3
+TBS_1C = [40, 56, 72, 120, 136, 144, 176, 208, 224, 256, 280, 296, 328, 336, 392, 488, 552, 600, 632, 696, 776, 840, 904,
+          1000, 1064, 1128, 1224, 1288, 1384, 1480, 1608, 1736]                # 36.213 Table 7.1.7.2.3-1
+N_GAP = {6: (3, None), 15: (8, None), 25: (12, None), 50: (27, 9), 75: (32, 16), 100: (48, 16)}   # 36.211 Table 6.2.3.2-1
+RBG = {6: 1, 15: 2, 25: 2, 50: 3, 75: 4, 100: 4}                                                  # 36.213 Table 7.1.6.1-1
+
+
+def n_vrb(R, gap):
+    g = N_GAP[R][gap]
+    return (R // (2 * g)) * 2 * g if gap else 2 * min(g, R - g)
+
+
+def vrb_to_prb(R, gap, n, slot):
+    """36.211 6.2.3.2: the PRB of distributed VRB n in slot parity `slot`."""
+    g, P = N_GAP[R][gap], RBG[R]
+    nt = 2 * g if gap else n_vrb(R, 0)
+    n_row = -(-nt // (4 * P)) * P
+    n_null = 4 * n_row - nt
+    v, blk = n % nt, nt * (n // nt)
+    p1, p2 = 2 * n_row * (v % 2) + v // 2 + blk, n_row * (v % 4) + v // 4 + blk
+    if n_null and v >= nt - n_null:
+        p = p1 - n_row + (n_null // 2 if v % 2 == 0 else 0)
+    elif n_null and v % 4 >= 2:
+        p = p2 - n_null // 2
+    else:
+        p = p2
+    if slot:
+        p = (p + nt // 2) % nt + blk
+    return p if p < nt // 2 else p + g - nt // 2
+
+
+def riv_decode(N, riv):
+    """(start, length) of a RIV on N RBs (36.213 7.1.6.3), None when it is not one."""
+    for length in range(1, N + 1):
+        for start in range(N - length + 1):
+            r = N * (length - 1) + start if length - 1 <= N // 2 else N * (N - length + 1) + (N - 1 - start)
+            if r == riv:
+                return start, length
+    return None
+
+
+def sib1_allocation(R, s):
+    """(tbs, [PRBs of slot 0, of slot 1]) of a cell's "sib1" dict."""
+    if s["format"] == "1A":
+        start, length = riv_decode(R, s["riv"])
+        tbs = TBS_1A[s["mcs"]][s.get("tpc", 0) & 1]
+        vrbs = range(start, start + length)
+        if not s.get("distributed", 0):
+            return tbs, [list(vrbs), list(vrbs)]
+        gap = 0
+    else:
+        step, gap = (2 if R < 50 else 4), s.get("gap", 0)
+        start, length = riv_decode(n_vrb(R, gap) // step, s["riv"])
+        vrbs = range(step * start, step * (start + length))
+        tbs = TBS_1C[s["tbs_index"]]
+    return tbs, [sorted(vrb_to_prb(R, gap, n, sl) for n in vrbs) for sl in (0, 1)]
+
+
+def sib1_dci_bits(R, s):
+    """The payload bits of the SI-RNTI DCI of a "sib1" dict (36.212 5.3.3.1.3-4)."""
+    bits = lambda v, n: [(v >> (n - 1 - i)) & 1 for i in range(n)]
+    if s["format"] == "1A":
+        n_ra = int(np.ceil(np.log2(R * (R + 1) // 2)))
+        a = [1, s.get("distributed", 0)] + bits(s["riv"], n_ra) + bits(s["mcs"], 5) + [0, 0, 0, 0] + bits(s.get("rv_field", 0), 2) \
+            + bits(s.get("tpc", 0), 2)
+        return a + [0] * (DCI_SIZES_1A[R] - len(a))
+    g = [s.get("gap", 0)] if R >= 50 else []
+    n = DCI_SIZES_1C[R] - len(g) - 5
+    return g + bits(s["riv"], n) + bits(s["tbs_index"], 5)
+
+
+def sib1_frames(cell, n_frames):
+    """The grid frames a cell sends SIB1 in: cell["sib1"]["frames"], or every frame with an even SFN."""
+    s = cell["sib1"]
+    return s.get("frames", [f for f in range(n_frames) if (cell.get("sfn0", 0) + f) % 2 == 0])
+
+
+def sib1_dcis(cell, n_subframes):
+    s = cell["sib1"]
+    R = cell["n_rb_dl"]
+    return [(10 * f + 5, 0xFFFF, s["format"], s.get("L", 8), s.get("cce", 0), sib1_dci_bits(R, s))
+            for f in sib1_frames(cell, -(-n_subframes // 10)) if 10 * f + 5 < n_subframes]
+
+
+def pdsch_res(R, P, cp, nid, n_ctrl, prbs):
+    """The data REs (l, k) of a SIB1 occasion in mapping order (36.211 6.3.5): symbols n_ctrl .. 2 n_symb - 1 of subframe
+    5, k first, the PRBs of each slot, without CRS of ports < P or the PSS / SSS columns of slot 10."""
+    n_symb = 7 if cp == 1 else 6
+    _, shift = O.rs_dl(nid, cp)
+    out = []
+    for l in range(n_ctrl, 2 * n_symb):
+        sl, ls = l // n_symb, l % n_symb
+        crs = set()
+        for p in range(P):
+            sh = shift[(10 + sl) * n_symb + ls, p]
+            if not np.isnan(sh):
+                crs |= set(range(int(sh), 12 * R, 6))
+        row = [k for prb in prbs[sl] for k in range(12 * prb, 12 * prb + 12)
+               if k not in crs and not (sl == 0 and ls >= n_symb - 2 and 6 * R - 36 <= k < 6 * R + 36)]
+        assert len(row) % 2 == 0, "a transmit-diversity pair would cross symbols"
+        out += [(l, k) for k in row]
+    return out
+
+
+def sib1_rv(sfn):
+    return (-(-3 * ((sfn // 2) % 4) // 2)) % 4
+
+
+def _write_sib1(X, cell, n_symb):
+    """cell["sib1"]: dict of the SIB1 bytes `tb` (TBS / 8 of them), the DCI (format "1A" or "1C", L, cce, riv, and
+    distributed, mcs, tpc, rv_field for 1A, gap, tbs_index for 1C) and optionally the grid `frames` it is sent in.  In
+    each such frame f, subframe 10 f + 5 carries the transport block with CRC24A, turbo-coded, rate-matched for the RV
+    of its SFN, scrambled, QPSK-mapped, precoded over all ports and written over the data REs of its allocation."""
+    s, R, P, cp, nid = cell["sib1"], cell["n_rb_dl"], cell["n_ports"], cell["cp_type"], cell["n_id_cell"]
+    seq, dur = list(cell["cfi"]), cell["phich_duration"]
+    tbs, prbs = sib1_allocation(R, s)
+    a = np.unpackbits(np.frombuffer(bytes(s["tb"]), np.uint8))
+    assert a.size == tbs, (a.size, tbs)
+    b = np.concatenate([a, crc24a(a)])
+    K = min(k for k in turbo_sizes() if k >= b.size)
+    F = K - b.size
+    d = turbo_encode(np.concatenate([np.zeros(F, np.uint8), b]))
+    n_sub = X.shape[1] // (2 * n_symb)
+    for f in sib1_frames(cell, -(-n_sub // 10)):
+        u = 10 * f + 5
+        if u >= n_sub:
+            continue
+        res = pdsch_res(R, P, cp, nid, n_ctrl_of(seq[u % len(seq)], R, dur), prbs)
+        e = rate_match(d, K, F, sib1_rv(cell.get("sfn0", 0) + f), 2 * len(res))
+        e = e ^ O.lte_pn(0xFFFF * 16384 + 5 * 512 + nid, e.size).astype(np.uint8)
+        x = ((1 - 2 * e[0::2].astype(float)) + 1j * (1 - 2 * e[1::2].astype(float))) / np.sqrt(2)
+        y = _precode(x, P)
+        l, k = np.array(res).T
+        X[:, 2 * n_symb * u + l, k] = y
